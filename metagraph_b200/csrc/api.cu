@@ -707,6 +707,10 @@ int launch_seed(const mgb_index_t *index, const Batch &b, uint32_t n_strands, St
         const uint64_t pb = std::min<uint64_t>((items + 7) / 8, (uint64_t)index->num_sms * 16);
         CUDA_TRY(index->view.wide ? kern_any::launch_premap((unsigned)pb, st.s, a) : kern_dna::launch_premap((unsigned)pb, st.s, a));
     }
+    if (index->view.kh_slots) {
+        CUDA_TRY(kern_dna::launch_seed_hash(index->num_sms, st.s, a));
+        return 0;
+    }
     // one strand per lane, 128 strands per block; enough blocks to fill the machine, grid-stride beyond that
     uint64_t blocks = std::min<uint64_t>((items + 127) / 128, (uint64_t)index->num_sms * 16);
     CUDA_TRY(index->view.wide ? kern_any::launch_seed((unsigned)blocks, st.s, a) : kern_dna::launch_seed((unsigned)blocks, st.s, a));

@@ -420,7 +420,8 @@ __global__ void __launch_bounds__(256) k_premap(SeedArgs a) {
 //   warm  the next k-mer is the child of the current edge: ONE 8-byte adjacency load per step and lane, 32
 //         independent pointer chases per warp, all lanes in the same three-instruction-deep loop.
 // (One quad per strand running both regimes kept 8 of 32 lanes busy on average: 8 quads in 8 different states.)
-// Same results as map_to_edges() in seed_core.cuh, which the host emulation still runs.
+// Same results as map_to_edges() in seed_core.cuh, which the host emulation still runs. Graphs with the k-mer hash
+// index take k_seed_hash instead.
 __global__ void __launch_bounds__(128) k_seed(SeedArgs a) {
     const IndexView &ix = a.ix;
     const int K = (int)ix.k;
@@ -428,67 +429,6 @@ __global__ void __launch_bounds__(128) k_seed(SeedArgs a) {
     const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
     const uint64_t items = (uint64_t)a.n_reads * a.n_strands;
-    if (ix.kh_slots) {
-        // ---- with the k-mer hash index: one strand per lane from start to end. Every k-mer costs one load: the
-        // adjacency record while the walk is warm, a hash probe (+ the value on a hit) when it is not; the packed
-        // k-mer is a rolling value. Every lane of a warp makes the same number of steps for reads of one length.
-        const uint32_t sigma = ix.sigma;
-        for (uint64_t item = warp * 32 + lane; item < items; item += nwarps * 32) {
-            const uint32_t r = (uint32_t)(item / a.n_strands), s = (uint32_t)(item % a.n_strands);
-            const uint64_t b = a.offsets[r];
-            const int L = (int)(a.offsets[r + 1] - b);
-            if (L < K) continue;
-            const int nk = L - K + 1;
-            const uint8_t *codes = (s ? a.cr : a.cf) + b;
-            uint64_t *out = (s ? a.nodes_r : a.nodes_f) + a.koff[r];
-            unsigned long long key = 0;
-            int last_bad = -1;
-            for (int j = 0; j < K - 1; ++j) {
-                const uint32_t c = codes[j];
-                if (c < 1 || c >= sigma) last_bad = j;
-                key = (key >> 2) | ((unsigned long long)((c - 1) & 3u) << (2 * (K - 1)));
-            }
-            uint64_t edge = 0;
-            const unsigned long long *keys = ix.kh_keys;
-            const uint64_t slots = ix.kh_slots;
-            // one step per k-mer, written with selects rather than branches: the lanes of a warp are in different
-            // regimes (warm / cold / inside an invalid window) at the same step and should still issue together
-            for (int pos = 0; pos < nk; ++pos) {
-                const uint32_t c = codes[pos + K - 1];
-                if (c < 1 || c >= sigma) last_bad = pos + K - 1;
-                key = (key >> 2) | ((unsigned long long)((c - 1) & 3u) << (2 * (K - 1)));
-                const bool ok = last_bad < pos;                        // no invalid character in the window
-                const bool warm = ok && edge != 0, cold = ok && edge == 0;
-                const unsigned long long want = key | (1ull << 63);
-                uint64_t slot = kh_slot_of(want, slots);
-                uint2 ar = make_uint2(0u, 0u);
-                ulonglong2 ka = make_ulonglong2(0ull, 0ull), kb = ka;
-                if (warm) ar = load_adj(ix, edge);                     // boss.cpp:1024-1043
-                if (cold) {                                            // map_to_edge (boss.hpp:766-777): the k-mer's bucket
-                    ka = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot));
-                    kb = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot + 2));
-                }
-                int h = ka.x == want ? 0 : ka.y == want ? 1 : kb.x == want ? 2 : kb.y == want ? 3 : -1;
-                // a full bucket without the k-mer: its run goes on in the next buckets (rare at this load factor)
-                bool more = cold && h < 0 && ka.x != 0 && ka.y != 0 && kb.x != 0 && kb.y != 0;
-                while (more) {
-                    slot += 4; if (slot >= slots) slot = 0;
-                    ka = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot));
-                    kb = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot + 2));
-                    h = ka.x == want ? 0 : ka.y == want ? 1 : kb.x == want ? 2 : kb.y == want ? 3 : -1;
-                    more = h < 0 && ka.x != 0 && ka.y != 0 && kb.x != 0 && kb.y != 0;
-                }
-                uint64_t found = 0;
-                if (cold && h >= 0) found = ix.kh_vals[slot + h];
-                const uint64_t child = adj_child(ar, c);              // 0 for lanes that are not warm (ar = 0)
-                const bool child_ok = (ar.y >> (8 + c)) & 1u;
-                edge = warm ? child : found;                           // (0 when the window is invalid)
-                const bool store = warm ? (child != 0 && child_ok) : (found != 0 && in_graph(ix, found));
-                if (store) out[pos] = edge;
-            }
-        }
-        return;
-    }
     const int S = (ix.sfx_len && (int)ix.sfx_len <= K - 1) ? (int)ix.sfx_len : 0;
     const uint64_t base = ix.sigma - 1;
     for (uint64_t chunk = warp * 32; chunk < items; chunk += nwarps * 32) {
@@ -586,6 +526,178 @@ __global__ void __launch_bounds__(128) k_seed(SeedArgs a) {
     }
 }
 
+#if !defined(MGB_WIDE_ONLY)
+// k_seed_hash: strands per lane, threads per block and the blocks per SM its registers are sized for (build-time probes,
+// scripts/build_variant.sh -D...; DESIGN.md §3.2 has the measurements). One strand per lane at 40 resident warps per SM
+// (48 registers) is the default: more strands per lane at fewer warps were slower, as the kernel is limited by the DRAM
+// accesses it makes, not by the loads one lane keeps in flight.
+#ifndef MGB_SEED_STRANDS
+#define MGB_SEED_STRANDS 1
+#endif
+#ifndef MGB_SEED_THREADS
+#define MGB_SEED_THREADS 128
+#endif
+#ifndef MGB_SEED_MIN_BLOCKS
+#define MGB_SEED_MIN_BLOCKS 10
+#endif
+static constexpr int kSeedStrands = MGB_SEED_STRANDS;
+static constexpr int kSeedThreads = MGB_SEED_THREADS;
+
+// The characters of a strand in order, read 8 at a time: w0 is the aligned 8-byte word holding the next character,
+// w1 the word after it, loaded 8 characters before it is needed. Words are only loaded if they hold a character of the
+// strand (an aligned word never crosses a page). One byte load per character instead measured 19 % slower on c2 (2 strands per lane): with
+// tens of thousands of strands in flight, their lines do not stay in L1 from one character to the next.
+struct CodeStream {
+    const uint8_t *p;             // next character
+    int left;                     // characters from p to the end of the strand
+    unsigned long long w0, w1;
+    MGB_D void start(const uint8_t *codes, int L) {
+        p = codes; left = L; w0 = 0; w1 = 0;
+        const unsigned long long *w = reinterpret_cast<const unsigned long long*>((uintptr_t)codes & ~(uintptr_t)7);
+        if (L > 0) w0 = __ldg(w);
+        if (L > 8 - (int)((uintptr_t)codes & 7)) w1 = __ldg(w + 1);
+    }
+    MGB_D uint32_t next() {
+        const uint32_t c = (uint32_t)(w0 >> (8 * ((uintptr_t)p & 7))) & 0xFFu;
+        ++p; --left;
+        if (((uintptr_t)p & 7) == 0) {
+            w0 = w1;
+            w1 = left > 8 ? __ldg(reinterpret_cast<const unsigned long long*>(p) + 1) : 0ull;
+        }
+        return c;
+    }
+};
+
+// BOSS::map_to_edges (boss.cpp:996-1045) on graphs with the k-mer hash index (DNA block layout, k <= 31). Every k-mer
+// costs one load: the adjacency record of the previous k-mer's edge while the walk is warm (boss.cpp:1024-1043), the
+// k-mer's bucket (+ the value on a hit) when it is cold (map_to_edge, boss.hpp:766-777); the packed k-mer is a rolling
+// value. A strand is a chain of dependent loads; a lane carries kSeedStrands strands in lock-step: a step first issues
+// the load of every strand, then consumes them. The characters come from CodeStream, off the chain of the walk. Steps
+// are written with selects rather than branches: strands in different regimes (warm / cold / inside an invalid window /
+// finished) issue together. Node ids are stored a whole 32-byte sector at a time: single 8-byte stores leave sectors
+// partly written in L2, and evicting one of those most likely costs the DRAM (ECC, no write mask) a read-modify-write
+// (c2 prepare + seed: 19.3 ms -> 14.8 ms). Unlike k_seed, the kernel has no quad-cooperative BOSS lookups, so it needs
+// 48 registers instead of 80-96. Persistent grid: lane t of n_lanes takes the strands t + n_lanes * (kSeedStrands * round + m), m < kSeedStrands, so a last, partial round is spread over every lane.
+__global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash(const __grid_constant__ SeedArgs a) {
+    constexpr int M = kSeedStrands;
+    const IndexView &ix = a.ix;
+    const int K = (int)ix.k;
+    const int top = 2 * (K - 1);                                      // shift of the newest character in the key
+    const uint32_t sigma = ix.sigma;
+    const unsigned long long *keys = ix.kh_keys;
+    const uint64_t slots = ix.kh_slots;
+    const uint64_t lanes = (uint64_t)gridDim.x * blockDim.x;
+    const uint64_t items = (uint64_t)a.n_reads * a.n_strands;
+    for (uint64_t first = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; first < items; first += lanes * M) {
+        CodeStream cs[M];
+        uint64_t *out[M];
+        int nk[M], last_bad[M];
+        unsigned long long key[M];
+        uint64_t edge[M];
+        int steps = 0;
+        uint64_t sb0[M], sb1[M], sb2[M], sb3[M];                       // the strand's output sector being filled
+#pragma unroll
+        for (int m = 0; m < M; ++m) { sb0[m] = sb1[m] = sb2[m] = sb3[m] = 0; }
+#pragma unroll
+        for (int m = 0; m < M; ++m) {
+            const uint64_t item = first + m * lanes;
+            const uint8_t *codes = a.cf; int L = 0;
+            out[m] = a.nodes_f;
+            if (item < items) {
+                const uint32_t r = (uint32_t)(item / a.n_strands), s = (uint32_t)(item % a.n_strands);
+                const uint64_t b = a.offsets[r];
+                L = (int)(a.offsets[r + 1] - b);
+                codes = (s ? a.cr : a.cf) + b;
+                out[m] = (s ? a.nodes_r : a.nodes_f) + a.koff[r];
+            }
+            nk[m] = L >= K ? L - K + 1 : 0;
+            cs[m].start(codes, nk[m] ? L : 0);
+            steps = nk[m] > steps ? nk[m] : steps;
+            key[m] = 0; last_bad[m] = -1; edge[m] = 0;
+        }
+        for (int j = 0; j < K - 1; ++j) {
+#pragma unroll
+            for (int m = 0; m < M; ++m) {
+                const uint32_t c = cs[m].next();
+                if (c < 1 || c >= sigma) last_bad[m] = j;
+                key[m] = (key[m] >> 2) | ((unsigned long long)((c - 1) & 3u) << top);
+            }
+        }
+        for (int pos = 0; pos < steps; ++pos) {
+            uint32_t c[M];
+            bool warm[M], cold[M];
+            unsigned long long want[M];
+            uint64_t slot[M];
+            uint2 ar[M];
+            ulonglong2 ka[M], kb[M];
+            // ---- issue: every strand's record or bucket, and the character of its next step
+#pragma unroll
+            for (int m = 0; m < M; ++m) {
+                c[m] = cs[m].next();
+                if (c[m] < 1 || c[m] >= sigma) last_bad[m] = pos + K - 1;
+                key[m] = (key[m] >> 2) | ((unsigned long long)((c[m] - 1) & 3u) << top);
+                const bool ok = pos < nk[m] && last_bad[m] < pos;      // a k-mer without an invalid character
+                warm[m] = ok && edge[m] != 0; cold[m] = ok && edge[m] == 0;
+                want[m] = key[m] | (1ull << 63);
+                slot[m] = kh_slot_of(want[m], slots);
+                ar[m] = make_uint2(0u, 0u);
+                ka[m] = make_ulonglong2(0ull, 0ull); kb[m] = ka[m];
+                if (warm[m]) ar[m] = load_adj(ix, edge[m]);
+                if (cold[m]) {
+                    ka[m] = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot[m]));
+                    kb[m] = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot[m] + 2));
+                }
+            }
+            // ---- buckets: the k-mer's slot; a full bucket without it continues in the next one (rare at this load factor)
+            int h[M];
+#pragma unroll
+            for (int m = 0; m < M; ++m) {
+                h[m] = ka[m].x == want[m] ? 0 : ka[m].y == want[m] ? 1 : kb[m].x == want[m] ? 2 : kb[m].y == want[m] ? 3 : -1;
+                bool more = cold[m] && h[m] < 0 && ka[m].x != 0 && ka[m].y != 0 && kb[m].x != 0 && kb[m].y != 0;
+                while (more) {
+                    slot[m] += 4; if (slot[m] >= slots) slot[m] = 0;
+                    const ulonglong2 x = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot[m]));
+                    const ulonglong2 y = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot[m] + 2));
+                    h[m] = x.x == want[m] ? 0 : x.y == want[m] ? 1 : y.x == want[m] ? 2 : y.y == want[m] ? 3 : -1;
+                    more = h[m] < 0 && x.x != 0 && x.y != 0 && y.x != 0 && y.y != 0;
+                }
+            }
+            uint64_t found[M];
+#pragma unroll
+            for (int m = 0; m < M; ++m) found[m] = (cold[m] && h[m] >= 0) ? __ldg(ix.kh_vals + slot[m] + h[m]) : 0u;
+            // ---- consume: the k-mer's edge, stored if it is a node of the graph
+#pragma unroll
+            for (int m = 0; m < M; ++m) {
+                const uint64_t child = adj_child(ar[m], c[m]);        // 0 unless warm (ar = 0)
+                const bool child_ok = (ar[m].y >> (8 + c[m])) & 1u;
+                edge[m] = warm[m] ? child : found[m];                  // 0 when the window is invalid
+                const bool store = warm[m] ? (child != 0 && child_ok) : (found[m] != 0 && in_graph(ix, found[m]));
+                // node ids leave in whole 32-byte sectors (slot q of the sector of out[pos]); a sector the strand shares
+                // with its neighbours gets single stores of the strand's own slots. Zeros are written too: the node
+                // arrays start zero-filled.
+                const uint64_t v = store ? edge[m] : 0;
+                uint64_t *pa = out[m] + pos;
+                const int q = (int)(((uintptr_t)pa >> 3) & 3);
+                sb0[m] = q == 0 ? v : sb0[m]; sb1[m] = q == 1 ? v : sb1[m];
+                sb2[m] = q == 2 ? v : sb2[m]; sb3[m] = q == 3 ? v : sb3[m];
+                if (pos < nk[m] && (q == 3 || pos == nk[m] - 1)) {
+                    uint64_t *sec = pa - q;
+                    if (q == 3 && pos >= 3) {
+                        reinterpret_cast<ulonglong2*>(sec)[0] = make_ulonglong2(sb0[m], sb1[m]);
+                        reinterpret_cast<ulonglong2*>(sec)[1] = make_ulonglong2(sb2[m], sb3[m]);
+                    } else {
+                        if (pos - q >= 0) sec[0] = sb0[m];
+                        if (q >= 1 && pos - q + 1 >= 0) sec[1] = sb1[m];
+                        if (q >= 2 && pos - q + 2 >= 0) sec[2] = sb2[m];
+                        if (q >= 3) sec[3] = sb3[m];
+                    }
+                }
+            }
+        }
+    }
+}
+#endif // !MGB_WIDE_ONLY
+
 #endif // MGB_ALIGN_KERNEL_ONLY
 
 #ifndef MGB_ALIGN_MIN_BLOCKS
@@ -626,6 +738,19 @@ cudaError_t launch_subk(unsigned grid, cudaStream_t s, const SubkArgs &a, uint32
 }
 cudaError_t launch_premap(unsigned grid, cudaStream_t s, const SeedArgs &a) { k_premap<<<grid, 256, 0, s>>>(a); return cudaGetLastError(); }
 cudaError_t launch_seed(unsigned grid, cudaStream_t s, const SeedArgs &a) { k_seed<<<grid, 128, 0, s>>>(a); return cudaGetLastError(); }
+#if !defined(MGB_WIDE_ONLY)
+// persistent grid: as many blocks as are resident at once, or fewer when the strands do not fill them
+cudaError_t launch_seed_hash(int num_sms, cudaStream_t s, const SeedArgs &a) {
+    int per_sm = 0;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_seed_hash, kSeedThreads, 0);
+    if (e != cudaSuccess) return e;
+    const uint64_t per_block = (uint64_t)kSeedThreads * kSeedStrands;
+    const uint64_t need = ((uint64_t)a.n_reads * a.n_strands + per_block - 1) / per_block;
+    const uint64_t resident = (uint64_t)per_sm * num_sms;
+    k_seed_hash<<<(unsigned)(need < resident ? need : resident), kSeedThreads, 0, s>>>(a);
+    return cudaGetLastError();
+}
+#endif
 #endif
 cudaError_t launch_align(unsigned grid, size_t smem_block, cudaStream_t s, const AlignArgs &a) {
     k_align<<<grid, kAlignThreads, smem_block, s>>>(a);
