@@ -13,6 +13,7 @@
  *   mgb_map_to_nodes      <- map_to_nodes_sequentially() (graph/representation/base/
  *                            sequence_graph.cpp:541-551 -> dbg_succinct.cpp:285-305 ->
  *                            boss.cpp:996-1045 BOSS::map_to_edges)
+ *   mgb_map_to_nodes_strands  the same for a sequence and its reverse complement at once
  *   mgb_config_check      <- DBGAligner::DBGAligner (graph/alignment/dbg_aligner.cpp:26-60)
  *   mgb_align_batch       <- IDBGAligner::align_batch (graph/alignment/dbg_aligner.hpp:32-33,
  *                            dbg_aligner.cpp:251-355) with Seeder = SuffixSeeder<UniMEMSeeder>,
@@ -178,6 +179,12 @@ int mgb_config_check(const mgb_index_t *index, const mgb_config_t *config);
  * sum(max(0, len_i - k + 1)) entries, laid out consecutively per sequence. */
 int mgb_map_to_nodes(const mgb_index_t *index, const char *seqs, const uint64_t *offsets,
                      uint32_t n_seqs, uint64_t *out_nodes);
+
+/* Exact seeding of both raw strands, in any mode: out_fwd receives the node ids of the k-mers of each sequence
+ * and out_rc those of its reverse complement, each laid out as out_nodes of mgb_map_to_nodes. Ids are the stored
+ * graph's own (BOSS edges): there is no PRIMARY-mode merge of the two strands. DNA graphs only. */
+int mgb_map_to_nodes_strands(const mgb_index_t *index, const char *seqs, const uint64_t *offsets,
+                             uint32_t n_seqs, uint64_t *out_fwd, uint64_t *out_rc);
 
 /* Full seed-and-extend of a batch of reads; results in input order. */
 int mgb_align_batch(const mgb_index_t *index, const mgb_config_t *config, const char *seqs,

@@ -78,6 +78,8 @@ def load_library(path=None):
     L.mgb_config_check.argtypes = [vp, ctypes.POINTER(mgb_config_t)]
     L.mgb_map_to_nodes.restype = i
     L.mgb_map_to_nodes.argtypes = [vp, vp, vp, u32, vp]
+    L.mgb_map_to_nodes_strands.restype = i
+    L.mgb_map_to_nodes_strands.argtypes = [vp, vp, vp, u32, vp, vp]
     L.mgb_align_batch.restype = i
     L.mgb_align_batch.argtypes = [vp, ctypes.POINTER(mgb_config_t), vp, vp, u32, ctypes.POINTER(vp)]
     L.mgb_results_num_reads.restype = u32
@@ -123,7 +125,7 @@ def check(L, rc):
 REQUIRED_SYMBOLS = [
     "mgb_last_error", "mgb_device_count", "mgb_index_create", "mgb_index_destroy", "mgb_index_num_edges",
     "mgb_index_device_bytes", "mgb_index_k", "mgb_config_init", "mgb_config_init_cli", "mgb_map_to_nodes",
-    "mgb_align_batch", "mgb_results_num_reads", "mgb_results_read_range", "mgb_results_num_alignments",
+    "mgb_map_to_nodes_strands",    "mgb_align_batch", "mgb_results_num_reads", "mgb_results_read_range", "mgb_results_num_alignments",
     "mgb_results_alignments", "mgb_results_stats", "mgb_results_free", "mgb_results_export_bytes",
     "mgb_results_export", "mgb_results_import", "mgb_boss_build", "mgb_boss_free",
     "mgb_boss_mask_dummy", "mgb_set_pipeline_pieces", "mgb_set_host_threads", "mgb_dbg_load", "mgb_dbg_last_error", "mgb_boss_last_error", "mgb_config_check", "mgb_dbg_load_suffix_ranges", "mgb_dbg_free_suffix_ranges", "mgb_index_set_mode",

@@ -100,6 +100,14 @@ class BOSSTable:
         return valid
 
 
+def _split(out, nk):
+    res, p = [], 0
+    for n in nk:
+        res.append(out[p:p + int(n)])
+        p += int(n)
+    return res
+
+
 class DBGSuccinctIndex:
     """BOSS index resident in one GPU's HBM (DBGSuccinct's role for the aligner)."""
 
@@ -155,11 +163,19 @@ class DBGSuccinctIndex:
         out = np.zeros(int(nk.sum()) + 1, dtype=np.uint64)
         _lib.check(self._L, self._L.mgb_map_to_nodes(self.handle, buf.ctypes.data, offsets.ctypes.data,
                                                      len(lens), out.ctypes.data))
-        res, p = [], 0
-        for n in nk:
-            res.append(out[p:p + int(n)])
-            p += int(n)
-        return res
+        return _split(out, nk)
+
+    def map_to_nodes_strands(self, seqs, packed=None):
+        """node ids of all k-mers of each sequence and of its reverse complement in the stored graph, whatever the
+        mode (no PRIMARY merge of the strands): two lists of uint64 arrays"""
+        buf, offsets = packed if packed is not None else _pack(seqs)
+        lens = (offsets[1:] - offsets[:-1]).astype(np.int64)
+        nk = np.maximum(lens - self.k + 1, 0)
+        fwd = np.zeros(int(nk.sum()) + 1, dtype=np.uint64)
+        rev = np.zeros(int(nk.sum()) + 1, dtype=np.uint64)
+        _lib.check(self._L, self._L.mgb_map_to_nodes_strands(self.handle, buf.ctypes.data, offsets.ctypes.data,
+                                                             len(lens), fwd.ctypes.data, rev.ctypes.data))
+        return _split(fwd, nk), _split(rev, nk)
 
 
 class Alignment:

@@ -515,7 +515,12 @@ int mgb_index_create(const uint8_t *W, const uint8_t *last, uint64_t n_plus_1, c
             std::swap(ra.c_cur, ra.c_nxt);
         }
         kern_dna::k_radj_pack<<<grid, 256>>>(ra, radj_multi_shift(idx->view));
-        if (kmer) kern_dna::k_kmer_insert<<<grid, 256>>>(kmer, n, kh_keys, kh_vals, kh_slots);
+        if (kmer) {
+            kern_dna::k_kmer_insert<<<grid, 256>>>(kmer, n, kh_keys, kh_vals, kh_slots);
+            IndexView hv = idx->view;
+            hv.kh_keys = kh_keys; hv.kh_vals = kh_vals; hv.kh_slots = kh_slots;
+            kern_dna::k_adj_rc<<<grid, 256>>>(hv, const_cast<uint2*>(hv.adj), kmer);
+        }
         if (e == cudaSuccess) e = cudaGetLastError();
         if (e == cudaSuccess) e = cudaDeviceSynchronize();
         cudaFree(bwd_arr); cudaFree(c0); cudaFree(c1); cudaFree(multi); cudaFree(kmer);
@@ -760,6 +765,38 @@ int mgb_map_to_nodes(const mgb_index_t *index, const char *seqs, const uint64_t 
                 }
             }
         }
+    }
+#if !defined(MGB_HOST_EMU)
+    cudaStreamSynchronize(st.s);
+#endif
+    return rc;
+}
+
+int mgb_map_to_nodes_strands(const mgb_index_t *index, const char *seqs, const uint64_t *offsets,
+                             uint32_t n_seqs, uint64_t *out_fwd, uint64_t *out_rc) {
+    if (!index || !seqs || !offsets || !out_fwd || !out_rc) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!index->at.has_complement) return fail(MGB_ERR_BAD_CONFIG, "a reverse-complement strand needs a DNA graph");
+    Stream st;
+    int rc = 0;
+    struct WsGuard { const mgb_index_t *ix; Workspace *w; ~WsGuard() { ix->ws_release(w); } } wsg{ index, index->ws_acquire() };
+#if !defined(MGB_HOST_EMU)
+    CUDA_TRY(cudaSetDevice(index->device));
+    if ((rc = wsg.w->ready())) return rc;
+    st.s = wsg.w->stream;
+#endif
+    {
+        DevBufs bufs(st, wsg.w, 0);
+        Batch b; std::vector<uint64_t> koff; mgb_stats_t stats; std::memset(&stats, 0, sizeof(stats));
+        rc = upload_batch(index, seqs, offsets, n_seqs, true, st, bufs, &b, &koff, &stats);
+        if (!rc) rc = dev_zero(b.nodes_f, (b.total_kmers + 1) * 8, st);
+        if (!rc) rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, st);
+        if (!rc) rc = launch_prepare(index, b, st, index->num_sms);
+        if (!rc) rc = launch_seed(index, b, 2, st, bufs);
+        if (!rc) rc = d2h(out_fwd, b.nodes_f, b.total_kmers * 8, st);
+        if (!rc) rc = d2h(out_rc, b.nodes_r, b.total_kmers * 8, st);
+#if !defined(MGB_HOST_EMU)
+        if (!rc) { cudaError_t e = cudaStreamSynchronize(st.s); if (e != cudaSuccess) rc = fail(MGB_ERR_CUDA, cudaGetErrorString(e)); }
+#endif
     }
 #if !defined(MGB_HOST_EMU)
     cudaStreamSynchronize(st.s);

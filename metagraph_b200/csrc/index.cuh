@@ -432,6 +432,10 @@ MGB_HD uint64_t fwd(const IndexView &ix, LineCache &lc, uint64_t i, uint32_t c) 
 //   x        last edge of the target node of e (0: e is a sink dummy, no outgoing edges)
 //   y[0:5)   labels ($ACGT) present among the target node's edges (flagged ones included)
 //   y[8:13)  labels whose edge is a valid, non-'$' DBG node (in_graph)
+//   y[16:21) graphs with the k-mer hash index only (DNA block layout, k <= 31): labels c whose edge's k-mer has its
+//            reverse complement in the hash index (kh_lookup != 0, in_graph or not), or whose k-mer is not a valid
+//            key. 0 tells k_seed_hash that the other strand's k-mer at the mirrored position is missing. Set by
+//            k_adj_rc; other layouts and the host emulation leave these bits 0 and never read them.
 // Edges of a node are sorted by label, so the edge with label c is first + popc(mask & ((1<<c)-1)).
 MGB_HD uint2 load_adj(const IndexView &ix, uint64_t e) {
 #if MGB_DEVICE_CODE
@@ -640,6 +644,13 @@ MGB_HD uint64_t kh_slot_of(uint64_t key, uint64_t slots) {
 #else
     return (uint64_t)(((unsigned __int128)(h ^ (h >> 29)) * (slots >> 2)) >> 64) << 2;
 #endif
+}
+// reverse complement of the packed k-mer `key` (k <= 31): position p takes 3 - (the code at k - 1 - p, minus 1), as
+// the complement of DNA code c is 5 - c
+MGB_HD uint64_t kh_revcomp(uint64_t key, uint32_t k) {
+    uint64_t r = 0;
+    for (uint32_t p = 0; p < k; ++p) { r = (r << 2) | (key & 3u); key >>= 2; }
+    return r ^ ((1ull << (2 * k)) - 1);
 }
 // edge of the k-mer `key62`, 0 if the graph does not have it (kh_slots is a multiple of 4)
 MGB_HD uint64_t kh_lookup(const IndexView &ix, uint64_t key62) {

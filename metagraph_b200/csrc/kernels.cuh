@@ -527,20 +527,14 @@ __global__ void __launch_bounds__(128) k_seed(SeedArgs a) {
 }
 
 #if !defined(MGB_WIDE_ONLY)
-// k_seed_hash: strands per lane, threads per block and the blocks per SM its registers are sized for (build-time probes,
-// scripts/build_variant.sh -D...; DESIGN.md §3.2 has the measurements). One strand per lane at 40 resident warps per SM
-// (48 registers) is the default: more strands per lane at fewer warps were slower, as the kernel is limited by the DRAM
-// accesses it makes, not by the loads one lane keeps in flight.
-#ifndef MGB_SEED_STRANDS
-#define MGB_SEED_STRANDS 1
-#endif
+// k_seed_hash: threads per block and the blocks per SM its registers are sized for (build-time probes,
+// scripts/build_variant.sh -D...; DESIGN.md §3.2 has the measurements).
 #ifndef MGB_SEED_THREADS
 #define MGB_SEED_THREADS 128
 #endif
 #ifndef MGB_SEED_MIN_BLOCKS
-#define MGB_SEED_MIN_BLOCKS 10
+#define MGB_SEED_MIN_BLOCKS 5
 #endif
-static constexpr int kSeedStrands = MGB_SEED_STRANDS;
 static constexpr int kSeedThreads = MGB_SEED_THREADS;
 
 // The characters of a strand in order, read 8 at a time: w0 is the aligned 8-byte word holding the next character,
@@ -567,132 +561,216 @@ struct CodeStream {
         return c;
     }
 };
+// The same backwards, from the last character of the strand: w0 holds the next character, w1 is the word before it.
+struct CodeStreamDown {
+    const uint8_t *p;             // next character
+    int left;                     // characters from the start of the strand to p, p included
+    unsigned long long w0, w1;
+    MGB_D void start(const uint8_t *codes, int L) {
+        p = codes + L - 1; left = L; w0 = 0; w1 = 0;
+        const unsigned long long *w = reinterpret_cast<const unsigned long long*>((uintptr_t)p & ~(uintptr_t)7);
+        if (L > 0) w0 = __ldg(w);
+        if (L > 1 + (int)((uintptr_t)p & 7)) w1 = __ldg(w - 1);
+    }
+    MGB_D uint32_t next() {
+        const uint32_t c = (uint32_t)(w0 >> (8 * ((uintptr_t)p & 7))) & 0xFFu;
+        --left;
+        if (((uintptr_t)p & 7) == 0) {
+            w0 = w1;
+            w1 = left > 8 ? __ldg(reinterpret_cast<const unsigned long long*>(p) - 2) : 0ull;
+        }
+        --p;
+        return c;
+    }
+};
 
-// BOSS::map_to_edges (boss.cpp:996-1045) on graphs with the k-mer hash index (DNA block layout, k <= 31). Every k-mer
-// costs one load: the adjacency record of the previous k-mer's edge while the walk is warm (boss.cpp:1024-1043), the
-// k-mer's bucket (+ the value on a hit) when it is cold (map_to_edge, boss.hpp:766-777); the packed k-mer is a rolling
-// value. A strand is a chain of dependent loads; a lane carries kSeedStrands strands in lock-step: a step first issues
-// the load of every strand, then consumes them. The characters come from CodeStream, off the chain of the walk. Steps
-// are written with selects rather than branches: strands in different regimes (warm / cold / inside an invalid window /
-// finished) issue together. Node ids are stored a whole 32-byte sector at a time: single 8-byte stores leave sectors
-// partly written in L2, and evicting one of those most likely costs the DRAM (ECC, no write mask) a read-modify-write
-// (c2 prepare + seed: 19.3 ms -> 14.8 ms). Unlike k_seed, the kernel has no quad-cooperative BOSS lookups, so it needs
-// 48 registers instead of 80-96. Persistent grid: lane t of n_lanes takes the strands t + n_lanes * (kSeedStrands * round + m), m < kSeedStrands, so a last, partial round is spread over every lane.
+// Packed k-mer at position 0 of a strand (key = sum of (code_p - 1) << 2p); *last_bad = position of its last invalid
+// character, -1 if none. The stream is left at position k.
+MGB_D unsigned long long first_kmer(CodeStream &cs, const uint8_t *codes, int L, int K, uint32_t sigma, int *last_bad) {
+    cs.start(codes, L);
+    unsigned long long key = 0;
+    int bad = -1;
+    for (int j = 0; j < K; ++j) {
+        const uint32_t c = cs.next();
+        if (c < 1 || c >= sigma) bad = j;
+        key = (key >> 2) | ((unsigned long long)((c - 1) & 3u) << (2 * (K - 1)));
+    }
+    *last_bad = bad;
+    return key;
+}
+
+// One k-mer lookup in the hash index (kh_lookup) in three parts, so that a lane keeps several in flight: issue() loads
+// the k-mer's bucket (nothing when `on` is false), find() settles it (a full bucket without the k-mer continues in the
+// next one, rare at this load factor), value() loads the edge (0: not in the graph).
+struct KhProbe {
+    unsigned long long want;
+    uint64_t slot;
+    ulonglong2 ka, kb;
+    int h;
+    MGB_D void issue(const IndexView &ix, unsigned long long key, bool on) {
+        want = key | (1ull << 63);
+        slot = kh_slot_of(want, ix.kh_slots);
+        ka = make_ulonglong2(0ull, 0ull); kb = ka;
+        if (on) {
+            ka = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot));
+            kb = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot + 2));
+        }
+    }
+    MGB_D void find(const IndexView &ix) {
+        h = ka.x == want ? 0 : ka.y == want ? 1 : kb.x == want ? 2 : kb.y == want ? 3 : -1;
+        bool more = h < 0 && ka.x != 0 && ka.y != 0 && kb.x != 0 && kb.y != 0;     // never when not issued
+        while (more) {
+            slot += 4; if (slot >= ix.kh_slots) slot = 0;
+            const ulonglong2 x = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot));
+            const ulonglong2 y = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot + 2));
+            h = x.x == want ? 0 : x.y == want ? 1 : y.x == want ? 2 : y.y == want ? 3 : -1;
+            more = h < 0 && x.x != 0 && x.y != 0 && y.x != 0 && y.y != 0;
+        }
+    }
+    MGB_D uint64_t value(const IndexView &ix) const { return h >= 0 ? __ldg(ix.kh_vals + slot + h) : 0u; }
+};
+
+// Node ids of a strand leave in whole 32-byte sectors: s0..s3 are the slots of the sector being filled (slot q of
+// node id i is (address / 8) % 4). A sector the strand shares with a neighbouring read gets single stores of the
+// strand's own slots. Single 8-byte stores left sectors partly written in L2, and evicting one of those most likely
+// costs the DRAM (ECC, no write mask) a read-modify-write (c2 prepare + seed: 19.3 ms -> 14.8 ms).
+struct SectorOut {
+    uint64_t s0, s1, s2, s3;
+    MGB_D void clear() { s0 = s1 = s2 = s3 = 0; }
+    MGB_D void put(int q, uint64_t v) {
+        s0 = q == 0 ? v : s0; s1 = q == 1 ? v : s1; s2 = q == 2 ? v : s2; s3 = q == 3 ? v : s3;
+    }
+    MGB_D void flush(uint64_t *sec, int lo, int hi) {      // slots lo..hi
+        if (lo == 0 && hi == 3) {
+            reinterpret_cast<ulonglong2*>(sec)[0] = make_ulonglong2(s0, s1);
+            reinterpret_cast<ulonglong2*>(sec)[1] = make_ulonglong2(s2, s3);
+        } else {
+            if (lo == 0) sec[0] = s0;
+            if (lo <= 1 && hi >= 1) sec[1] = s1;
+            if (lo <= 2 && hi >= 2) sec[2] = s2;
+            if (hi == 3) sec[3] = s3;
+        }
+    }
+    // ascending walk: node id v of k-mer `pos` of nk; stored once the sector is full or the strand ends. Zeros are
+    // stored too.
+    MGB_D void put_up(uint64_t *out, int pos, int nk, uint64_t v) {
+        uint64_t *pa = out + pos;
+        const int q = (int)(((uintptr_t)pa >> 3) & 3);
+        put(q, v);
+        if (q == 3 || pos == nk - 1) flush(pa - q, pos < q ? q - pos : 0, q);
+    }
+    // descending walk: node id v of k-mer j, sectors filled from slot 3 down. A sector of zeros is not stored: the
+    // node arrays start zero-filled. (Slots of the first sector above the strand's last k-mer are 0 after clear().)
+    MGB_D void put_down(uint64_t *out, int j, int nk, uint64_t v) {
+        uint64_t *pa = out + j;
+        const int q = (int)(((uintptr_t)pa >> 3) & 3);
+        put(q, v);
+        if ((q == 0 || j == 0) && (s0 | s1 | s2 | s3)) {
+            const int hi = q + (nk - 1 - j);
+            flush(pa - q, q, hi < 3 ? hi : 3);
+        }
+    }
+};
+
+// BOSS::map_to_edges (boss.cpp:996-1045) on graphs with the k-mer hash index (DNA block layout, k <= 31), one read per
+// lane. A strand walked in order costs one load per k-mer: the adjacency record of the previous k-mer's edge while the
+// walk is warm (boss.cpp:1024-1043), the k-mer's bucket (+ the value on a hit) when it is cold (map_to_edge,
+// boss.hpp:766-777); the packed k-mer is a rolling value. The characters come from CodeStream, off the chain of the walk.
+//
+// With both strands, the lane first looks up position 0 of each. If exactly one of them hits, the read runs PAIRED:
+// that strand (the primary) is walked in order, and the other one (the secondary) backwards in the same steps. The
+// secondary's k-mer at j = nk - 1 - t is the reverse complement of the primary's at t when both windows are valid
+// (pinned for the alphabet tables by tests/test_seed_pairing.py), and a random genome hardly ever holds both. So when
+// the primary's k-mer at t came from a warm step, bit 16 + c of the record it came from (k_adj_rc) settles the
+// secondary's k-mer with no load whenever it is 0. Otherwise the secondary looks it up cold. The secondary runs one step
+// behind, so its lookup is issued together with the primary's load of the next step. Its key is a rolling value of its
+// own characters, read backwards. Its first k-mer (position 0) is the probe's miss. If both probes hit (CANONICAL-mode
+// graphs, regions stored in both orientations) or neither does (an error in the first k-mer), the strands are walked
+// one after the other. (c2 prepare + seed: 14.8 ms -> 7.2 ms, DESIGN.md §3.2.)
+//
+// Steps are written with selects rather than branches: lanes in different regimes issue together. Persistent grid:
+// lane t of n_lanes takes the reads t + n_lanes * round.
 __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash(const __grid_constant__ SeedArgs a) {
-    constexpr int M = kSeedStrands;
     const IndexView &ix = a.ix;
     const int K = (int)ix.k;
     const int top = 2 * (K - 1);                                      // shift of the newest character in the key
+    const unsigned long long mask = (1ull << (2 * K)) - 1;
     const uint32_t sigma = ix.sigma;
-    const unsigned long long *keys = ix.kh_keys;
-    const uint64_t slots = ix.kh_slots;
+    const bool two = a.n_strands == 2;
     const uint64_t lanes = (uint64_t)gridDim.x * blockDim.x;
-    const uint64_t items = (uint64_t)a.n_reads * a.n_strands;
-    for (uint64_t first = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; first < items; first += lanes * M) {
-        CodeStream cs[M];
-        uint64_t *out[M];
-        int nk[M], last_bad[M];
-        unsigned long long key[M];
-        uint64_t edge[M];
-        int steps = 0;
-        uint64_t sb0[M], sb1[M], sb2[M], sb3[M];                       // the strand's output sector being filled
-#pragma unroll
-        for (int m = 0; m < M; ++m) { sb0[m] = sb1[m] = sb2[m] = sb3[m] = 0; }
-#pragma unroll
-        for (int m = 0; m < M; ++m) {
-            const uint64_t item = first + m * lanes;
-            const uint8_t *codes = a.cf; int L = 0;
-            out[m] = a.nodes_f;
-            if (item < items) {
-                const uint32_t r = (uint32_t)(item / a.n_strands), s = (uint32_t)(item % a.n_strands);
-                const uint64_t b = a.offsets[r];
-                L = (int)(a.offsets[r + 1] - b);
-                codes = (s ? a.cr : a.cf) + b;
-                out[m] = (s ? a.nodes_r : a.nodes_f) + a.koff[r];
-            }
-            nk[m] = L >= K ? L - K + 1 : 0;
-            cs[m].start(codes, nk[m] ? L : 0);
-            steps = nk[m] > steps ? nk[m] : steps;
-            key[m] = 0; last_bad[m] = -1; edge[m] = 0;
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < a.n_reads; r += lanes) {
+        const uint64_t b = a.offsets[r];
+        const int L = (int)(a.offsets[r + 1] - b);
+        const int nk = L >= K ? L - K + 1 : 0;
+        if (nk == 0) continue;
+        const uint64_t ko = a.koff[r];
+        // ---- position 0 of both strands, the two lookups in flight together
+        uint64_t f0, f1;
+        {
+            CodeStream c0, c1;
+            int bad0, bad1 = 0;
+            const unsigned long long k0 = first_kmer(c0, a.cf + b, L, K, sigma, &bad0);
+            const unsigned long long k1 = two ? first_kmer(c1, a.cr + b, L, K, sigma, &bad1) : 0ull;
+            KhProbe p0, p1;
+            p0.issue(ix, k0, bad0 < 0); p1.issue(ix, k1, two && bad1 < 0);
+            p0.find(ix); p1.find(ix);
+            f0 = p0.value(ix); f1 = p1.value(ix);
         }
-        for (int j = 0; j < K - 1; ++j) {
-#pragma unroll
-            for (int m = 0; m < M; ++m) {
-                const uint32_t c = cs[m].next();
-                if (c < 1 || c >= sigma) last_bad[m] = j;
-                key[m] = (key[m] >> 2) | ((unsigned long long)((c - 1) & 3u) << top);
+        const bool paired = two && ((f0 != 0) != (f1 != 0));
+        const int passes = two && !paired ? 2 : 1;
+        for (int pass = 0; pass < passes; ++pass) {
+            // the strand walked in order (the primary when paired) ...
+            const bool sp = paired ? f0 == 0 : pass == 1;
+            CodeStream cs;
+            int last_bad;
+            unsigned long long key = first_kmer(cs, (sp ? a.cr : a.cf) + b, L, K, sigma, &last_bad);
+            uint64_t edge = sp ? f1 : f0;                              // its k-mer at 0, from the probe
+            uint64_t *out = (sp ? a.nodes_r : a.nodes_f) + ko;
+            SectorOut so;
+            so.clear();
+            so.put_up(out, 0, nk, (edge != 0 && in_graph(ix, edge)) ? edge : 0);
+            // ... and the secondary, backwards: characters L - 1 .. nk of its k-mer at nk - 1 first
+            CodeStreamDown ds;
+            ds.start((sp ? a.cf : a.cr) + b, paired ? L : 0);
+            uint64_t *out2 = (sp ? a.nodes_f : a.nodes_r) + ko;
+            unsigned long long key2 = 0;
+            int bad2 = 0x7fffffff;                                     // lowest position of an invalid character read
+            for (int i = 0; paired && i < K - 1; ++i) {
+                const uint32_t c = ds.next();
+                if (c < 1 || c >= sigma) bad2 = L - 1 - i;
+                key2 = (key2 << 2) | ((c - 1) & 3u);
             }
-        }
-        for (int pos = 0; pos < steps; ++pos) {
-            uint32_t c[M];
-            bool warm[M], cold[M];
-            unsigned long long want[M];
-            uint64_t slot[M];
-            uint2 ar[M];
-            ulonglong2 ka[M], kb[M];
-            // ---- issue: every strand's record or bucket, and the character of its next step
-#pragma unroll
-            for (int m = 0; m < M; ++m) {
-                c[m] = cs[m].next();
-                if (c[m] < 1 || c[m] >= sigma) last_bad[m] = pos + K - 1;
-                key[m] = (key[m] >> 2) | ((unsigned long long)((c[m] - 1) & 3u) << top);
-                const bool ok = pos < nk[m] && last_bad[m] < pos;      // a k-mer without an invalid character
-                warm[m] = ok && edge[m] != 0; cold[m] = ok && edge[m] == 0;
-                want[m] = key[m] | (1ull << 63);
-                slot[m] = kh_slot_of(want[m], slots);
-                ar[m] = make_uint2(0u, 0u);
-                ka[m] = make_ulonglong2(0ull, 0ull); kb[m] = ka[m];
-                if (warm[m]) ar[m] = load_adj(ix, edge[m]);
-                if (cold[m]) {
-                    ka[m] = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot[m]));
-                    kb[m] = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot[m] + 2));
-                }
+            SectorOut so2;
+            so2.clear();
+            bool look2 = true;                 // the secondary's next k-mer needs a lookup (the probe was a cold hit)
+            for (int t = 1; t < nk; ++t) {
+                // ---- issue: the primary's record or bucket for k-mer t, the secondary's bucket for k-mer nk - t
+                const uint32_t c = cs.next();
+                if (c < 1 || c >= sigma) last_bad = t + K - 1;
+                key = (key >> 2) | ((unsigned long long)((c - 1) & 3u) << top);
+                const bool ok = last_bad < t;                          // a k-mer without an invalid character
+                const bool warm = ok && edge != 0, cold = ok && edge == 0;
+                const int j = nk - t;
+                const uint32_t c2 = ds.next();
+                if (c2 < 1 || c2 >= sigma) bad2 = j;
+                key2 = ((key2 << 2) | ((c2 - 1) & 3u)) & mask;
+                const bool cold2 = paired && look2 && bad2 >= j + K;
+                uint2 ar = make_uint2(0u, 0u);
+                if (warm) ar = load_adj(ix, edge);
+                KhProbe p, p2;
+                p.issue(ix, key, cold); p2.issue(ix, key2, cold2);
+                p.find(ix); p2.find(ix);
+                const uint64_t found = p.value(ix), found2 = p2.value(ix);
+                // ---- consume: the k-mers' edges, stored if they are nodes of the graph
+                const uint64_t child = adj_child(ar, c);              // 0 unless warm (ar = 0)
+                const bool child_ok = (ar.y >> (8 + c)) & 1u;
+                look2 = !(warm && child != 0 && !((ar.y >> (16 + c)) & 1u));
+                edge = warm ? child : found;                           // 0 when the window is invalid
+                const bool store = warm ? (child != 0 && child_ok) : (found != 0 && in_graph(ix, found));
+                so.put_up(out, t, nk, store ? edge : 0);
+                if (paired) so2.put_down(out2, j, nk, (found2 != 0 && in_graph(ix, found2)) ? found2 : 0);
             }
-            // ---- buckets: the k-mer's slot; a full bucket without it continues in the next one (rare at this load factor)
-            int h[M];
-#pragma unroll
-            for (int m = 0; m < M; ++m) {
-                h[m] = ka[m].x == want[m] ? 0 : ka[m].y == want[m] ? 1 : kb[m].x == want[m] ? 2 : kb[m].y == want[m] ? 3 : -1;
-                bool more = cold[m] && h[m] < 0 && ka[m].x != 0 && ka[m].y != 0 && kb[m].x != 0 && kb[m].y != 0;
-                while (more) {
-                    slot[m] += 4; if (slot[m] >= slots) slot[m] = 0;
-                    const ulonglong2 x = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot[m]));
-                    const ulonglong2 y = __ldg(reinterpret_cast<const ulonglong2*>(keys + slot[m] + 2));
-                    h[m] = x.x == want[m] ? 0 : x.y == want[m] ? 1 : y.x == want[m] ? 2 : y.y == want[m] ? 3 : -1;
-                    more = h[m] < 0 && x.x != 0 && x.y != 0 && y.x != 0 && y.y != 0;
-                }
-            }
-            uint64_t found[M];
-#pragma unroll
-            for (int m = 0; m < M; ++m) found[m] = (cold[m] && h[m] >= 0) ? __ldg(ix.kh_vals + slot[m] + h[m]) : 0u;
-            // ---- consume: the k-mer's edge, stored if it is a node of the graph
-#pragma unroll
-            for (int m = 0; m < M; ++m) {
-                const uint64_t child = adj_child(ar[m], c[m]);        // 0 unless warm (ar = 0)
-                const bool child_ok = (ar[m].y >> (8 + c[m])) & 1u;
-                edge[m] = warm[m] ? child : found[m];                  // 0 when the window is invalid
-                const bool store = warm[m] ? (child != 0 && child_ok) : (found[m] != 0 && in_graph(ix, found[m]));
-                // node ids leave in whole 32-byte sectors (slot q of the sector of out[pos]); a sector the strand shares
-                // with its neighbours gets single stores of the strand's own slots. Zeros are written too: the node
-                // arrays start zero-filled.
-                const uint64_t v = store ? edge[m] : 0;
-                uint64_t *pa = out[m] + pos;
-                const int q = (int)(((uintptr_t)pa >> 3) & 3);
-                sb0[m] = q == 0 ? v : sb0[m]; sb1[m] = q == 1 ? v : sb1[m];
-                sb2[m] = q == 2 ? v : sb2[m]; sb3[m] = q == 3 ? v : sb3[m];
-                if (pos < nk[m] && (q == 3 || pos == nk[m] - 1)) {
-                    uint64_t *sec = pa - q;
-                    if (q == 3 && pos >= 3) {
-                        reinterpret_cast<ulonglong2*>(sec)[0] = make_ulonglong2(sb0[m], sb1[m]);
-                        reinterpret_cast<ulonglong2*>(sec)[1] = make_ulonglong2(sb2[m], sb3[m]);
-                    } else {
-                        if (pos - q >= 0) sec[0] = sb0[m];
-                        if (q >= 1 && pos - q + 1 >= 0) sec[1] = sb1[m];
-                        if (q >= 2 && pos - q + 2 >= 0) sec[2] = sb2[m];
-                        if (q >= 3) sec[3] = sb3[m];
-                    }
-                }
-            }
+            if (paired) so2.put_down(out2, 0, nk, 0);                  // the probe's miss
         }
     }
 }
@@ -739,13 +817,12 @@ cudaError_t launch_subk(unsigned grid, cudaStream_t s, const SubkArgs &a, uint32
 cudaError_t launch_premap(unsigned grid, cudaStream_t s, const SeedArgs &a) { k_premap<<<grid, 256, 0, s>>>(a); return cudaGetLastError(); }
 cudaError_t launch_seed(unsigned grid, cudaStream_t s, const SeedArgs &a) { k_seed<<<grid, 128, 0, s>>>(a); return cudaGetLastError(); }
 #if !defined(MGB_WIDE_ONLY)
-// persistent grid: as many blocks as are resident at once, or fewer when the strands do not fill them
+// persistent grid: as many blocks as are resident at once, or fewer when the reads do not fill them
 cudaError_t launch_seed_hash(int num_sms, cudaStream_t s, const SeedArgs &a) {
     int per_sm = 0;
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_seed_hash, kSeedThreads, 0);
     if (e != cudaSuccess) return e;
-    const uint64_t per_block = (uint64_t)kSeedThreads * kSeedStrands;
-    const uint64_t need = ((uint64_t)a.n_reads * a.n_strands + per_block - 1) / per_block;
+    const uint64_t need = ((uint64_t)a.n_reads + kSeedThreads - 1) / kSeedThreads;     // one read per lane
     const uint64_t resident = (uint64_t)per_sm * num_sms;
     k_seed_hash<<<(unsigned)(need < resident ? need : resident), kSeedThreads, 0, s>>>(a);
     return cudaGetLastError();
@@ -802,6 +879,25 @@ __global__ void __launch_bounds__(256) k_kmer_insert(const unsigned long long *k
         uint64_t i = kh_slot_of(key, slots);
         while (atomicCAS(keys + i, 0ull, key) != 0ull) { if (++i == slots) i = 0; }
         vals[i] = (uint32_t)e;
+    }
+}
+// Reverse-complement bits of the forward adjacency records (index.cuh load_adj, y[16:21)), once the hash index is
+// complete: for every label c != '$' out of e's target node, is the reverse complement of that child's k-mer in the
+// index? A k-mer that is no valid key gets the bit too, so k_seed_hash then looks it up rather than skip it. Each
+// thread writes its own records only. `ix` carries the finished hash index.
+__global__ void __launch_bounds__(256) k_adj_rc(IndexView ix, uint2 *adj, const unsigned long long *kmer) {
+    uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint64_t nt = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t e = 1 + t; e <= ix.n; e += nt) {
+        const uint2 a = adj[e];
+        uint32_t bits = 0;
+        for (uint32_t c = 1; c < 5; ++c) {
+            const uint64_t child = adj_child(a, c);
+            if (!child) continue;
+            const unsigned long long km = kmer[child];
+            if (km == kKmerBad || kh_lookup(ix, kh_revcomp(km, ix.k))) bits |= 1u << (16 + c);
+        }
+        if (bits) adj[e].y = a.y | bits;
     }
 }
 __global__ void __launch_bounds__(256) k_radj_pack(RadjArgs a, uint32_t multi_shift) {
