@@ -150,7 +150,7 @@ struct OutAln {
 
 struct ReadStats { uint32_t num_seeds, num_extensions, num_explored_nodes, dp_columns; uint64_t dp_cells; };
 #if defined(MGB_HOST_EMU)
-extern "C" unsigned long long mgb_emu_whole_read_hits;   // host emulation (tests) only: reads answered by whole_read_exact()
+extern "C" unsigned long long mgb_emu_whole_read_hits;   // host emulation (tests) only: reads answered by exact_read_strand()
 #endif
 
 #if defined(MGB_PHASE_TIMERS) && MGB_DEVICE_CODE
@@ -3361,54 +3361,6 @@ struct ReadAligner {
         wsync();
     }
 
-    // Exact-path shortcut for the whole read (exact seeder, both strands asked for): every k-mer of one strand is in the
-    // graph and none of the other strand's. What the general code does with such a read, step by step: build_seeds
-    // gives the matching strand one seed per k-mer (num_matching = L) and the other strand none, the matching strand
-    // goes first, its first seed starts the read, extend() takes the exact-path shortcut (same conditions as there:
-    // cfg.exact_shortcut and the two score thresholds), the result enters the empty aggregator, every later seed of
-    // the strand is dropped, the other strand has nothing to extend. One alignment, {L}= along the read's own nodes,
-    // one extension, L - k + 1 seeds: written here directly. Anything else (a missing k-mer, a k-mer on the other
-    // strand, the complexity filter, min_exact_match above 1, slots too small) takes the general code.
-    MGB_HD bool whole_read_exact(bool both) {
-        const int k = (int)ix.k;
-        if (!cfg.exact_shortcut || !both || MGB_CANONICAL(cfg) || MGB_PRIMARY(ix) || L < k
-                || !cx[0].qnodes || !cx[1].qnodes || cfg.min_seed_length != ix.k || cfg.max_seed_length != ix.k
-                || !sm.lq() || L + 1 > sm.lq() || cfg.seed_complexity_filter || !(cfg.min_exact_match <= 1.0))
-            return false;
-        const int nk = L - k + 1;
-        const uint64_t *nf = cx[0].qnodes, *nr = cx[1].qnodes;
-        unsigned bits = 0;                                   // 1: a missing forward k-mer, 2: a present one; 4 / 8: reverse
-        for (int i = wlane(); i < nk; i += kWarp) bits |= (nf[i] ? 2u : 1u) | (nr[i] ? 8u : 4u);
-        bits = wreduce_or(bits);
-        int s;
-        if (bits == (2u | 4u)) s = 0;
-        else if (bits == (1u | 8u)) s = 1;
-        else return false;
-        const score_t full = cx[s].ps[0] - cx[s].ps[L] + cfg.left_end_bonus + cfg.right_end_bonus;
-        // extend(): min_path_score = max(0, min_cell_score) for a forward extension when both strands are aligned
-        // (align_strand); then the result must reach get_min_path_score() of the empty aggregator
-        if (full < imax(0, cfg.min_cell_score) || full < cfg.min_path_score) return false;
-        if ((int)caps.aln_nodes < nk || (int)caps.aln_seq < L || (int)caps.aln_cigar < 1) return false;
-        const uint64_t *qn = s ? nr : nf;
-        const AlnSlot o = m.slot(SLOT_AGG);
-        wsync();
-        for (int i = wlane(); i < nk; i += kWarp) o.nodes[i] = qn[i];
-        for (int i = wlane(); i < L; i += kWarp) o.seq[i] = cx[s].q[i];
-        o.cigar[0] = cig_pack(OP_M, L);
-        AlnHdr h;
-        h.q_len = L; h.n_nodes = nk; h.seq_len = L; h.n_cigar = 1; h.score = full; h.offset = 0;
-        h.orientation = s; h.used = 1;
-        *o.h = h;
-        wsync();
-        n_agg = 1;
-        ++cx[s].conv_epoch;                                  // set_seed() of the one extension
-        stats.num_seeds = nk; stats.num_extensions = 1;
-#if defined(MGB_HOST_EMU)
-        ++mgb_emu_whole_read_hits;
-#endif
-        return true;
-    }
-
     // whole pipeline for one read; returns the number of alignments left in SLOT_AGG.. (sorted)
     // optional: per-position index_range results of both strands (k_subk), set before run()
     const uint32_t *subk_first[2] = { nullptr, nullptr }, *subk_last[2] = { nullptr, nullptr };
@@ -3421,7 +3373,6 @@ struct ReadAligner {
         overflow = false; n_agg = 0; seed_is_query = false;
         const bool both = cfg.forward_and_reverse_complement;
         int first = 0, n_pass = 0;
-        bool early = false;
         if (act) {
         wsync();
         // per-strand context + alignment slot table (shared memory; constant indices only here)
@@ -3467,8 +3418,6 @@ struct ReadAligner {
         }
         build_psum(0);
         if (both) build_psum(1);
-        early = whole_read_exact(both);
-        if (!early) {
         if (!MGB_WIDE(ix) && sm.lay->has_prof && L + 1 <= sm.lq()) { build_prof4(0); if (both) build_prof4(1); }
         if (cfg.seed_complexity_filter) { build_lowcx(0); if (both) build_lowcx(1); }
         MGB_TOC(t_setup, 0);
@@ -3487,18 +3436,16 @@ struct ReadAligner {
             uint32_t hi = first ? bm : fm, lo = first ? fm : bm;
             n_pass = (double)lo >= (double)hi * cfg.rel_score_cutoff ? 2 : 1;
         }
-        }   // !early
         }   // act
         MGB_TOC(t_seeds, 1);
         MGB_TIC(t_align);
         for (int pass = 0; ; ++pass) {
-            const bool p_ok = act && !early && !overflow && pass < n_pass;
+            const bool p_ok = act && !overflow && pass < n_pass;
             if (!wany_full(p_ok)) break;
             align_strand(pass ? 1 - first : first, both, p_ok);
         }
         MGB_TOC(t_align, 4);
         if (!act || overflow) return 0;
-        if (early) { order[0] = 0; return 1; }
         stats.num_extensions += cx[0].num_ext + cx[1].num_ext;
         stats.num_explored_nodes += cx[0].explored_prev + cx[0].conv_n + cx[1].explored_prev + cx[1].conv_n;
         // AlignmentAggregator::get_alignments: descending LocalAlignmentLess order

@@ -684,9 +684,11 @@ int launch_prepare(const mgb_index_t *index, const Batch &b, Stream &st, int num
     return 0;
 }
 
+// summary: SeedArgs::summary (k_seed_hash writes it; nullptr on graphs without the k-mer hash index)
 int launch_seed(const mgb_index_t *index, const Batch &b, uint32_t n_strands, Stream &st, DevBufs &bufs,
-                uint64_t *n_launches = nullptr) {
-    SeedArgs a { index->view, b.cf, b.cr, b.offsets, b.koff, b.nodes_f, b.nodes_r, b.n_reads, n_strands, 0, nullptr, nullptr };
+                uint8_t *summary, uint64_t *n_launches = nullptr) {
+    SeedArgs a { index->view, b.cf, b.cr, b.offsets, b.koff, b.nodes_f, b.nodes_r, b.n_reads, n_strands, 0, nullptr, nullptr,
+                 summary };
     uint64_t items = (uint64_t)b.n_reads * n_strands;
     // first pass (k_premap): rules out the k-mers the suffix-range table has no node for; the node arrays
     // are zero-filled, so the second pass only visits what is left
@@ -723,6 +725,24 @@ int launch_seed(const mgb_index_t *index, const Batch &b, uint32_t n_strands, St
     return 0;
 }
 
+// whole-read exact answers (kernels.cuh ExactArgs) for the reads of a.list; the others are appended to a.rest
+int launch_exact_reads(const mgb_index_t *index, const ExactArgs &a, Stream &st) {
+#if defined(MGB_HOST_EMU)
+    (void)index; (void)st;
+    for (uint32_t t = 0; t < a.n_list; ++t) {
+        const uint32_t r = a.list[t];
+        uint64_t b; int L; score_t score;
+        const int s = exact_read_strand(a, a.diag, r, &b, &L, &score);
+        if (s < 0) { a.rest[(*a.n_rest)++] = r; continue; }
+        exact_read_write(a, r, b, L, s, score, *a.heap_used, 0, 1);
+        *a.heap_used += exact_read_bytes(a, L);
+    }
+#else
+    if (a.n_list) CUDA_TRY(kern_dna::launch_exact_reads(index->num_sms, st.s, a));
+#endif
+    return 0;
+}
+
 } // namespace
 
 extern "C" {
@@ -749,7 +769,7 @@ int mgb_map_to_nodes(const mgb_index_t *index, const char *seqs, const uint64_t 
         if (!rc) rc = dev_zero(b.nodes_f, (b.total_kmers + 1) * 8, st);
         if (!rc && primary) rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, st);
         if (!rc) rc = launch_prepare(index, b, st, index->num_sms);
-        if (!rc) rc = launch_seed(index, b, primary ? 2 : 1, st, bufs);
+        if (!rc) rc = launch_seed(index, b, primary ? 2 : 1, st, bufs, nullptr);
         if (!rc) rc = d2h(out_nodes, b.nodes_f, b.total_kmers * 8, st);
         if (!rc && primary) { rev.resize(b.total_kmers + 1); rc = d2h(rev.data(), b.nodes_r, b.total_kmers * 8, st); }
 #if !defined(MGB_HOST_EMU)
@@ -791,7 +811,7 @@ int mgb_map_to_nodes_strands(const mgb_index_t *index, const char *seqs, const u
         if (!rc) rc = dev_zero(b.nodes_f, (b.total_kmers + 1) * 8, st);
         if (!rc) rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, st);
         if (!rc) rc = launch_prepare(index, b, st, index->num_sms);
-        if (!rc) rc = launch_seed(index, b, 2, st, bufs);
+        if (!rc) rc = launch_seed(index, b, 2, st, bufs, nullptr);
         if (!rc) rc = d2h(out_fwd, b.nodes_f, b.total_kmers * 8, st);
         if (!rc) rc = d2h(out_rc, b.nodes_r, b.total_kmers * 8, st);
 #if !defined(MGB_HOST_EMU)
@@ -877,6 +897,14 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
         tick("setup");
         rc = upload_batch(index, seqs, offsets, n_reads, both, st, bufs, &b, &koff, &res->stats);
         tick("upload_batch (host part)");
+        // whole-read exact answers ahead of k_align (kernels.cuh ExactArgs): the configuration part of the gate. The
+        // seeding kernel of graphs with the k-mer hash index summarises what it stored per read; without it the node
+        // arrays are read instead.
+        const uint32_t k = index->view.k;
+        const bool exact_reads = dcfg.exact_shortcut && both && index->view.mode == 0 && dcfg.min_seed_length == k
+                                 && dcfg.max_seed_length == k && !dcfg.seed_complexity_filter && dcfg.min_exact_match <= 1.0;
+        uint8_t *summary = nullptr;
+        if (!rc && exact_reads && index->view.kh_slots) rc = bufs.alloc(&summary, (size_t)n_reads + 1);
         if (!rc) rc = dev_zero(b.nodes_f, (b.total_kmers + 1) * 8, st);
         if (!rc && both) rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, st);
 #if !defined(MGB_HOST_EMU)
@@ -884,7 +912,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
 #endif
         if (!rc) rc = launch_prepare(index, b, st, index->num_sms);
         res->stats.kernel_launches += 1;
-        if (!rc && map_nodes) rc = launch_seed(index, b, both ? 2 : 1, st, bufs, &res->stats.kernel_launches);
+        if (!rc && map_nodes) rc = launch_seed(index, b, both ? 2 : 1, st, bufs, summary, &res->stats.kernel_launches);
         // sub-k seeding (min_seed_length < k): the independent index_range lookups run GPU-wide first
         SubkArgs sk;
         std::memset(&sk, 0, sizeof(sk));
@@ -989,17 +1017,36 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             // output heap: generous first guess, doubled on retry passes
             uint64_t per_read = sizeof(OutAln) + 9ull * (b.L_max + 64 + index->view.k) + 4ull * 64;
             uint64_t heap_cap = (uint64_t)list.size() * per_read * dcfg.num_alternative_paths * scale + 4096;
-            char *d_arena = nullptr, *d_heap = nullptr; uint32_t *d_list = nullptr;
+            char *d_arena = nullptr, *d_heap = nullptr; uint32_t *d_list = nullptr, *d_rest = nullptr;
             unsigned long long *d_used = nullptr; unsigned int *d_next = nullptr;
             if ((rc = pass_bufs.alloc(&d_arena, stride * n_warps))) break;
             if ((rc = pass_bufs.alloc(&d_heap, heap_cap))) break;
             if ((rc = pass_bufs.alloc(&d_list, list.size()))) break;
             if ((rc = pass_bufs.alloc(&d_used, 1))) break;
-            if ((rc = pass_bufs.alloc(&d_next, 1))) break;
+            if ((rc = pass_bufs.alloc(&d_next, 2))) break;        // k_align's next read; the reads k_exact_reads leaves
+            if (exact_reads && (rc = pass_bufs.alloc(&d_rest, list.size()))) break;
             tick("pass: arena/heap alloc");
             if ((rc = h2d(d_list, list.data(), list.size() * 4, st))) break;
             if ((rc = dev_zero(d_used, 8, st))) break;
-            if ((rc = dev_zero(d_next, 4, st))) break;
+            if ((rc = dev_zero(d_next, 8, st))) break;
+            // the read-dependent part of the gate (exact_read_strand); max_len keeps what k_align's own exit required
+            ExactArgs ea;
+            std::memset(&ea, 0, sizeof(ea));
+            if (exact_reads) {
+                ea.k = k;
+                ea.end_bonus = dcfg.left_end_bonus + dcfg.right_end_bonus;
+                ea.min_score = std::max({ 0, (int)dcfg.min_cell_score, (int)dcfg.min_path_score });
+                const uint64_t max_len = std::min<uint64_t>({ lq_v > 0 ? (uint64_t)lq_v - 1 : 0, caps.aln_seq,
+                                                             (uint64_t)caps.aln_nodes + k - 1 });
+                ea.max_len = caps.aln_cigar >= 1 ? (uint32_t)max_len : 0;
+                ea.result_nodes = dcfg.result_nodes;
+                std::memcpy(ea.diag, dcfg.diag, sizeof(ea.diag));
+                ea.qf = b.qf; ea.qr = b.qr; ea.offsets = b.offsets; ea.koff = b.koff;
+                ea.nodes_f = b.nodes_f; ea.nodes_r = b.nodes_r; ea.summary = summary;
+                ea.list = d_list; ea.n_list = (uint32_t)list.size(); ea.rest = d_rest; ea.n_rest = d_next + 1;
+                ea.hdr = d_hdr; ea.heap = d_heap; ea.heap_cap = heap_cap; ea.heap_used = d_used;
+            }
+            const bool run_exact = exact_reads && ea.max_len >= k;
             AlignArgs a;
             a.ix = index->view; a.cfg = dcfg; a.caps = caps; a.lay.carve(caps); a.slay = slay;
             a.use_fast = std::getenv("MGB_TEST_NOFAST") ? 0 : 1;
@@ -1018,18 +1065,34 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             a.arena = d_arena; a.arena_stride = stride;
             a.hdr = d_hdr; a.heap = d_heap; a.heap_cap = heap_cap; a.heap_used = d_used; a.next = d_next;
             unsigned long long used = 0;
+#if !defined(MGB_HOST_EMU)
+            cudaEventRecord(ev[3], st.s);
+#endif
+            if (run_exact) {
+                // k_align takes only the reads left over; their count sizes its grid
+                if ((rc = launch_exact_reads(index, ea, st))) break;
+                uint32_t n_rest = 0;
+                if ((rc = d2h(&n_rest, d_next + 1, 4, st))) break;
+#if !defined(MGB_HOST_EMU)
+                CUDA_TRY(cudaStreamSynchronize(st.s));
+#endif
+                a.read_list = d_rest; a.n_list = n_rest;
+                res->stats.kernel_launches += 1;
+            }
 #if defined(MGB_HOST_EMU)
-            init_arena(a, d_arena);
+            if (a.n_list) init_arena(a, d_arena);
             std::vector<char> smem_emu(smem_per_warp + 64);
             const WarpMem mem_emu { d_arena, &a.lay };
             const WarpSmem sm_emu { smem_emu.data(), &a.slay };
             for (uint32_t t = 0; t < a.n_list; ++t) align_read(a, a.read_list[t], mem_emu, sm_emu, true);
             used = *d_used;
 #else
-            cudaEventRecord(ev[3], st.s);
-            CUDA_TRY(index->view.wide ? kern_any::launch_align(n_warps / (uint32_t)gpb, smem_block, st.s, a)
-                   : index->view.mode != 0 ? kern_canon::launch_align(n_warps / (uint32_t)gpb, smem_block, st.s, a)
-                                           : kern_dna::launch_align(n_warps / (uint32_t)gpb, smem_block, st.s, a));
+            if (a.n_list) {
+                const uint32_t grid = (uint32_t)(std::min<uint64_t>(n_warps, ((uint64_t)a.n_list + gpb - 1) / gpb * gpb) / gpb);
+                CUDA_TRY(index->view.wide ? kern_any::launch_align(grid, smem_block, st.s, a)
+                       : index->view.mode != 0 ? kern_canon::launch_align(grid, smem_block, st.s, a)
+                                               : kern_dna::launch_align(grid, smem_block, st.s, a));
+            }
             cudaEventRecord(ev[4], st.s);
             if ((rc = d2h(&used, d_used, 8, st))) break;
             CUDA_TRY(cudaStreamSynchronize(st.s));
@@ -1037,7 +1100,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             cudaEventRecord(ev[3], st.s);
 #endif
             tick("pass: h2d+seed+align kernels");
-            res->stats.kernel_launches += 1;
+            if (a.n_list) res->stats.kernel_launches += 1;
 #if defined(MGB_PHASE_TIMERS) && !defined(MGB_HOST_EMU)
             {
                 unsigned long long ph[8];

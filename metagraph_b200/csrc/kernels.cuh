@@ -52,6 +52,9 @@ struct SeedArgs {
     uint64_t *nodes_f, *nodes_r; uint32_t n_reads; uint32_t n_strands;
     uint32_t hinted;           // 1: k_premap ran, hint_f / hint_r hold its verdicts
     uint32_t *hint_f, *hint_r;
+    // k_seed_hash only (nullptr: not written): per read, which kinds of node id the walk stored, as ExactArgs::summary
+    // reads them (1: a 0 on the forward strand, 2: a non-zero one; 4 / 8: the same on the reverse strand; 0 if L < k)
+    uint8_t *summary;
 };
 
 MGB_HD void seed_item(const SeedArgs &a, uint64_t item) {
@@ -219,6 +222,106 @@ MGB_HD void init_arena(const AlignArgs &a, char *arena) {
         for (uint32_t i = wlane(); i < a.caps.hash_size; i += kWarp) mem.conv_slots(e)[i].epoch = 0;
     if (wlane() == 0) { mem.epoch_store()[0] = 0; mem.epoch_store()[1] = 0; }
     wsync();
+}
+
+// Whole-read exact answers (k_exact_reads, run over a pass's reads before k_align). With the exact seeder
+// (min_seed_length = max_seed_length = k) and both strands asked for, a read whose k-mers are all in the graph on one
+// strand and none on the other has one alignment: {L}= along that strand's own nodes, score Σ diag + both end bonuses,
+// L - k + 1 seeds and one extension. build_seeds would give the matching strand one seed per k-mer (num_matching = L) and
+// the other strand none; the matching strand goes first, its first seed starts the read, extend() takes the exact-path
+// shortcut (DESIGN.md §3.3), the result enters the empty aggregator and every later seed is dropped. Such a read is
+// answered here, without the aligner's set-up; every other read goes on to k_align. The host evaluates the configuration
+// part of the gate (cfg.exact_shortcut, both strands, BASIC mode, the exact seeder, no complexity filter,
+// min_exact_match <= 1) and launches nothing when it fails.
+struct ExactArgs {
+    uint32_t k;
+    int32_t end_bonus;            // left_end_bonus + right_end_bonus
+    int32_t min_score;            // max(0, min_cell_score, min_path_score): extend()'s threshold on a forward extension
+                                  // when both strands are aligned, and the empty aggregator's
+    uint32_t max_len;             // longest read answered: k_align's own exit needed both strands staged on chip
+                                  // (L + 1 <= lq) and room for L characters and L - k + 1 nodes in an alignment slot
+    uint32_t result_nodes;        // DevConfig::result_nodes: records without node ids
+    int8_t diag[128];             // DevConfig::diag
+    const char *qf, *qr; const uint64_t *offsets, *koff, *nodes_f, *nodes_r;
+    const uint8_t *summary;       // SeedArgs::summary, or nullptr: the same bits from nodes_f / nodes_r
+    const uint32_t *list; uint32_t n_list;
+    uint32_t *rest; unsigned int *n_rest;            // the reads left to k_align
+    ReadHdr *hdr; char *heap; uint64_t heap_cap; unsigned long long *heap_used;
+};
+
+// The strand (0 / 1) whose alignment answers read r, or -1; *b / *L: the read's start and length, *score: the alignment's
+// score. One lane, no collectives.
+MGB_HD int exact_read_strand(const ExactArgs &a, const int8_t *diag, uint32_t r, uint64_t *b, int *L, score_t *score) {
+    *b = a.offsets[r];
+    *L = (int)(a.offsets[r + 1] - *b);
+    const int n = *L, k = (int)a.k;
+    if (n < k || n > (int)a.max_len) return -1;
+    unsigned bits;                                       // 1: a missing forward k-mer, 2: a present one; 4 / 8: reverse
+    if (a.summary) {
+        bits = a.summary[r];
+    } else {
+        const uint64_t *nf = a.nodes_f + a.koff[r], *nr = a.nodes_r + a.koff[r];
+        bits = 0;
+        for (int i = 0; i < n - k + 1; ++i) bits |= (nf[i] ? 2u : 1u) | (nr[i] ? 8u : 4u);
+    }
+    const int s = bits == (2u | 4u) ? 0 : bits == (1u | 8u) ? 1 : -1;
+    if (s < 0) return -1;
+    // Σ diag over the strand (prepared characters are < 128), read as aligned 8-byte words (the strand buffers are padded
+    // past their end)
+    const char *q = (s ? a.qr : a.qf) + *b;
+    const uintptr_t lo = (uintptr_t)q, hi = lo + (uintptr_t)n;
+    int sum = 0;
+    for (uintptr_t w = lo & ~(uintptr_t)7; w < hi; w += 8) {
+        const unsigned long long x = *reinterpret_cast<const unsigned long long*>(w);
+        const int j0 = w < lo ? (int)(lo - w) : 0, j1 = hi - w < 8 ? (int)(hi - w) : 8;
+        for (int j = j0; j < j1; ++j) sum += diag[(x >> (8 * j)) & 0x7Fu];
+    }
+    const score_t full = sum + a.end_bonus;
+    if (full < a.min_score) return -1;
+#if defined(MGB_HOST_EMU)
+    ++mgb_emu_whole_read_hits;
+#endif
+    *score = full;
+    return s;
+}
+
+// bytes of the record: OutAln | node ids (unless result_nodes) | one CIGAR op | sequence, each part padded to 8 (align_read)
+MGB_HD uint32_t exact_read_bytes(const ExactArgs &a, int L) {
+    return (uint32_t)sizeof(OutAln) + (a.result_nodes ? 0u : 8u * (uint32_t)(L - (int)a.k + 1)) + 8u + (((uint32_t)L + 7u) & ~7u);
+}
+
+// Writes the record of read r (strand s) at heap offset `off` and the read's header, the same bytes align_read writes for
+// it, padding as zeros; a record past the end of the heap marks the read MGB_READ_OVERFLOW (the next pass retries it).
+// Lanes `lane` of `width` share the copies.
+MGB_HD void exact_read_write(const ExactArgs &a, uint32_t r, uint64_t b, int L, int s, score_t score, uint64_t off,
+                             int lane, int width) {
+    const int nk = L - (int)a.k + 1;
+    ReadHdr h;
+    h.status = MGB_READ_OK; h.n_aln = 1; h.heap_off = off;
+    h.stats.num_seeds = (uint32_t)nk; h.stats.num_extensions = 1;
+    h.stats.num_explored_nodes = 0; h.stats.dp_columns = 0; h.stats.dp_cells = 0;
+    if (off + exact_read_bytes(a, L) > a.heap_cap) {
+        h.status = MGB_READ_OVERFLOW; h.n_aln = 0; h.heap_off = 0;
+    } else {
+        char *p = a.heap + off;
+        if (lane == 0) {
+            OutAln o;
+            o.orientation = (uint32_t)s; o.score = score; o.offset = 0; o.query_begin = 0; o.query_len = (uint32_t)L;
+            o.n_nodes = (uint32_t)nk; o.seq_len = (uint32_t)L; o.n_cigar = 1;
+            *reinterpret_cast<OutAln*>(p) = o;
+        }
+        p += sizeof(OutAln);
+        if (!a.result_nodes) {
+            const uint64_t *qn = (s ? a.nodes_r : a.nodes_f) + a.koff[r];
+            for (int t = lane; t < nk; t += width) reinterpret_cast<uint64_t*>(p)[t] = qn[t];
+            p += 8ull * nk;
+        }
+        if (lane == 0) *reinterpret_cast<unsigned long long*>(p) = cig_pack(OP_M, (uint32_t)L);
+        p += 8;
+        const char *q = (s ? a.qr : a.qf) + b;
+        for (int t = lane; t < ((L + 7) & ~7); t += width) p[t] = t < L ? q[t] : 0;
+    }
+    if (lane == 0) a.hdr[r] = h;
 }
 
 // One refinement level of the suffix-range table (boss.hpp:651-655 index order: the appended
@@ -702,7 +805,7 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
         const uint64_t b = a.offsets[r];
         const int L = (int)(a.offsets[r + 1] - b);
         const int nk = L >= K ? L - K + 1 : 0;
-        if (nk == 0) continue;
+        if (nk == 0) { if (a.summary) a.summary[r] = 0; continue; }
         const uint64_t ko = a.koff[r];
         // ---- position 0 of both strands, the two lookups in flight together
         uint64_t f0, f1;
@@ -718,9 +821,11 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
         }
         const bool paired = two && ((f0 != 0) != (f1 != 0));
         const int passes = two && !paired ? 2 : 1;
+        uint32_t seen = 0;                    // SeedArgs::summary of the read: bit 0 / 1 (forward), 2 / 3 (reverse)
         for (int pass = 0; pass < passes; ++pass) {
             // the strand walked in order (the primary when paired) ...
             const bool sp = paired ? f0 == 0 : pass == 1;
+            const int sh = sp ? 2 : 0;        // its bits in `seen`; the secondary's are at 2 - sh
             CodeStream cs;
             int last_bad;
             unsigned long long key = first_kmer(cs, (sp ? a.cr : a.cf) + b, L, K, sigma, &last_bad);
@@ -728,7 +833,9 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
             uint64_t *out = (sp ? a.nodes_r : a.nodes_f) + ko;
             SectorOut so;
             so.clear();
-            so.put_up(out, 0, nk, (edge != 0 && in_graph(ix, edge)) ? edge : 0);
+            const bool store0 = edge != 0 && in_graph(ix, edge);
+            so.put_up(out, 0, nk, store0 ? edge : 0);
+            seen |= (store0 ? 2u : 1u) << sh;
             // ... and the secondary, backwards: characters L - 1 .. nk of its k-mer at nk - 1 first
             CodeStreamDown ds;
             ds.start((sp ? a.cf : a.cr) + b, paired ? L : 0);
@@ -767,11 +874,20 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
                 look2 = !(warm && child != 0 && !((ar.y >> (16 + c)) & 1u));
                 edge = warm ? child : found;                           // 0 when the window is invalid
                 const bool store = warm ? (child != 0 && child_ok) : (found != 0 && in_graph(ix, found));
-                so.put_up(out, t, nk, store ? edge : 0);
-                if (paired) so2.put_down(out2, j, nk, (found2 != 0 && in_graph(ix, found2)) ? found2 : 0);
+                so.put_up(out, t, nk, store ? edge : 0);                // (store: edge != 0)
+                seen |= (store ? 2u : 1u) << sh;
+                if (paired) {
+                    const bool store2 = found2 != 0 && in_graph(ix, found2);
+                    so2.put_down(out2, j, nk, store2 ? found2 : 0);
+                    seen |= (store2 ? 2u : 1u) << (2 - sh);
+                }
             }
-            if (paired) so2.put_down(out2, 0, nk, 0);                  // the probe's miss
+            if (paired) {
+                so2.put_down(out2, 0, nk, 0);                          // the probe's miss
+                seen |= 1u << (2 - sh);
+            }
         }
+        if (a.summary) a.summary[r] = (uint8_t)seen;
     }
 }
 #endif // !MGB_WIDE_ONLY
@@ -853,6 +969,74 @@ __global__ void __launch_bounds__(256) k_prepare(PrepArgs a) {
     uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) / kWarp;
     uint32_t nwarps = (gridDim.x * blockDim.x) / kWarp;
     for (uint32_t r = warp; r < a.n_reads; r += nwarps) prepare_read(a, r);
+}
+
+// Whole-read exact answers for the reads of a.list, a tile of kExactThreads reads per block and round. Each thread
+// decides for one read (exact_read_strand: its loads are independent of the other reads', so a warp has 32 reads' loads
+// in flight); a block prefix sum of the record sizes gives the answered reads one heap allocation per tile, and the
+// others one append to a.rest. Then each warp writes its answered records one after the other, 32 lanes per record.
+// Persistent grid. No index structure is read.
+static constexpr int kExactThreads = 256;
+__global__ void __launch_bounds__(kExactThreads) k_exact_reads(const __grid_constant__ ExactArgs a) {
+    constexpr int kWarps = kExactThreads / 32;
+    __shared__ int8_t diag[128];
+    __shared__ unsigned long long s_off[kWarps];        // per warp: heap offset of its first record
+    __shared__ uint32_t s_bytes[kWarps], s_left[kWarps], s_slot[kWarps];
+    for (int i = threadIdx.x; i < 128; i += kExactThreads) diag[i] = a.diag[i];
+    __syncthreads();
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const unsigned below = (1u << lane) - 1u;
+    for (uint64_t base = (uint64_t)blockIdx.x * kExactThreads; base < a.n_list; base += (uint64_t)gridDim.x * kExactThreads) {
+        const uint64_t t = base + threadIdx.x;
+        uint32_t r = 0; uint64_t b = 0; int L = 0, s = -1; score_t score = 0;
+        if (t < a.n_list) {
+            r = a.list[t];
+            s = exact_read_strand(a, diag, r, &b, &L, &score);
+        }
+        const uint32_t bytes = s >= 0 ? exact_read_bytes(a, L) : 0u;
+        uint32_t inc = bytes;                                          // inclusive prefix sum over the warp
+        #pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t o = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += o; }
+        const unsigned left = __ballot_sync(0xffffffffu, t < a.n_list && s < 0);
+        if (lane == 31) s_bytes[w] = inc;
+        if (lane == 0) s_left[w] = (uint32_t)__popc(left);
+        __syncthreads();
+        if (w == 0) {                                                  // the same over the warps, one atomic each
+            const uint32_t v = lane < kWarps ? s_bytes[lane] : 0u, c = lane < kWarps ? s_left[lane] : 0u;
+            uint32_t vi = v, ci = c;
+            #pragma unroll
+            for (int d = 1; d < kWarps; d <<= 1) {
+                const uint32_t ov = __shfl_up_sync(0xffffffffu, vi, d), oc = __shfl_up_sync(0xffffffffu, ci, d);
+                if (lane >= d) { vi += ov; ci += oc; }
+            }
+            const uint32_t tv = __shfl_sync(0xffffffffu, vi, kWarps - 1), tc = __shfl_sync(0xffffffffu, ci, kWarps - 1);
+            unsigned long long off = 0; unsigned int slot = 0;
+            if (lane == 0) {
+                if (tv) off = atomicAdd(a.heap_used, (unsigned long long)tv);
+                if (tc) slot = atomicAdd(a.n_rest, tc);
+            }
+            off = __shfl_sync(0xffffffffu, off, 0); slot = __shfl_sync(0xffffffffu, slot, 0);
+            if (lane < kWarps) { s_off[lane] = off + (vi - v); s_slot[lane] = slot + (ci - c); }
+        }
+        __syncthreads();
+        if ((left >> lane) & 1u) a.rest[s_slot[w] + __popc(left & below)] = r;
+        const unsigned long long my_off = s_off[w] + (inc - bytes);
+        for (unsigned todo = __ballot_sync(0xffffffffu, s >= 0); todo; todo &= todo - 1) {
+            const int j = __ffs(todo) - 1;
+            exact_read_write(a, __shfl_sync(0xffffffffu, r, j), __shfl_sync(0xffffffffu, (unsigned long long)b, j),
+                             __shfl_sync(0xffffffffu, L, j), __shfl_sync(0xffffffffu, s, j),
+                             __shfl_sync(0xffffffffu, score, j), __shfl_sync(0xffffffffu, my_off, j), lane, 32);
+        }
+    }
+}
+cudaError_t launch_exact_reads(int num_sms, cudaStream_t s, const ExactArgs &a) {
+    int per_sm = 0;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_exact_reads, kExactThreads, 0);
+    if (e != cudaSuccess) return e;
+    const uint64_t need = ((uint64_t)a.n_list + kExactThreads - 1) / kExactThreads;
+    const uint64_t resident = (uint64_t)per_sm * num_sms;
+    k_exact_reads<<<(unsigned)(need < resident ? need : resident), kExactThreads, 0, s>>>(a);
+    return cudaGetLastError();
 }
 // round r (0-based) brings character k - 3 - r of every edge's k-mer to c_nxt[e]; kmer_shift = 2 * (k - 3 - r)
 __global__ void __launch_bounds__(256) k_radj_gather(RadjArgs a, int kmer_shift) {
