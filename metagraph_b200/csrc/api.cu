@@ -288,6 +288,92 @@ struct mgb_results {
     mgb_stats_t stats;
 };
 
+#if !defined(MGB_HOST_EMU)
+// Path layout of a graph with the k-mer hash index (IndexView::pl_*, kernels.cuh k_path_*), from the per-edge k-mers
+// of the hash build. Skipped, leaving the seeding walk as it is without it, when the device memory is not there (it
+// keeps the same 16 GB for the aligner's working memory as the hash index) or MGB_NO_PATH_INDEX is set.
+static int build_path_layout(mgb_index *idx, const unsigned long long *kmer) {
+    const uint64_t n = idx->view.n;
+    if (std::getenv("MGB_NO_PATH_INDEX") || n >= (1ull << 31)) return MGB_OK;
+    size_t free_b = 0, total_b = 0;
+    cudaMemGetInfo(&free_b, &total_b);
+    // pred + jump during the build; pl_pos stays, and the positions take about 4.5 bytes per edge
+    if ((double)free_b < 1.2 * 16.5 * (n + 1) || (double)free_b - 8.6 * (n + 1) < 16e9) return MGB_OK;
+    kern_dna::PathArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.ix = idx->view; a.kmer = kmer;
+    struct Counters { unsigned long long total; unsigned int count; };
+    Counters *ctr = nullptr;
+    auto drop = [&]() {
+        cudaGetLastError();
+        cudaFree(a.pred); cudaFree(a.jump); cudaFree(a.node); cudaFree(a.text); cudaFree(a.rc); cudaFree(a.stop); cudaFree(ctr);
+        return MGB_OK;
+    };
+    if (cudaMalloc((void**)&a.pred, (n + 1) * 4) != cudaSuccess || cudaMalloc((void**)&a.jump, (n + 1) * 8) != cudaSuccess
+            || cudaMalloc((void**)&ctr, sizeof(Counters)) != cudaSuccess)
+        return drop();
+    a.total = &ctr->total; a.count = &ctr->count;
+    cudaError_t e = cudaMemset(a.pred, 0xFF, (n + 1) * 4);
+    if (e == cudaSuccess) e = cudaMemset(ctr, 0, sizeof(Counters));
+    const unsigned grid = (unsigned)idx->num_sms * 16;
+    auto check = [&](const char *what) -> int {
+        if (e == cudaSuccess) e = cudaGetLastError();
+        if (e == cudaSuccess) return MGB_OK;
+        drop();
+        return fail(MGB_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+    };
+    // *count after one launch of kernel f
+    auto counted = [&](void (*f)(kern_dna::PathArgs)) -> unsigned {
+        unsigned c = 0;
+        if (e == cudaSuccess) e = cudaMemset(a.count, 0, 4);
+        if (e == cudaSuccess) { f<<<grid, 256>>>(a); e = cudaGetLastError(); }
+        if (e == cudaSuccess) e = cudaMemcpy(&c, a.count, 4, cudaMemcpyDeviceToHost);
+        return c;
+    };
+    auto rank = [&]() { while (e == cudaSuccess && counted(kern_dna::k_path_jump)) {} };
+    kern_dna::k_path_pred<<<grid, 256>>>(a);
+    kern_dna::k_path_link<<<grid, 256>>>(a);
+    rank();
+    const unsigned cycle_nodes = counted(kern_dna::k_path_cycle_init);
+    if (cycle_nodes) {
+        for (unsigned w = 1; ; w *= 2) {               // the smallest node over windows of 2w >= every cycle's length
+            kern_dna::k_path_cycle_min<<<grid, 256>>>(a);
+            if (w >= cycle_nodes) break;
+        }
+        kern_dna::k_path_cycle_cut<<<grid, 256>>>(a);
+        rank();
+    }
+    kern_dna::k_path_heads<<<grid, 256>>>(a);
+    unsigned long long used = 0;
+    if (e == cudaSuccess) e = cudaMemcpy(&used, a.total, 8, cudaMemcpyDeviceToHost);
+    if (int rc = check("path layout")) return rc;
+    const uint64_t n_pos = ((used + 63) & ~63ull) + kPlPad;
+    if (n_pos >= (1ull << 32)) return drop();
+    cudaMemGetInfo(&free_b, &total_b);
+    const uint64_t bytes = n_pos * 4 + n_pos / 4 + 2 * (n_pos / 8);
+    if ((double)free_b < 1.2 * bytes || cudaMalloc((void**)&a.node, n_pos * 4) != cudaSuccess
+            || cudaMalloc((void**)&a.text, n_pos / 4) != cudaSuccess || cudaMalloc((void**)&a.rc, n_pos / 8) != cudaSuccess
+            || cudaMalloc((void**)&a.stop, n_pos / 8) != cudaSuccess)
+        return drop();
+    e = cudaMemset(a.node, 0, n_pos * 4);
+    if (e == cudaSuccess) e = cudaMemset(a.text, 0, n_pos / 4);
+    if (e == cudaSuccess) e = cudaMemset(a.rc, 0, n_pos / 8);
+    if (e == cudaSuccess) e = cudaMemset(a.stop, 0xFF, n_pos / 8);
+    if (e == cudaSuccess) kern_dna::k_path_place<<<grid, 256>>>(a);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (int rc = check("path layout")) return rc;
+    cudaFree(a.jump); cudaFree(ctr);
+    idx->bufs.push_back(a.pred); idx->bufs.push_back(a.node); idx->bufs.push_back(a.text); idx->bufs.push_back(a.rc);
+    idx->bufs.push_back(a.stop);
+    idx->device_bytes += (n + 1) * 4 + bytes;
+    idx->view.pl_pos = a.pred; idx->view.pl_node = a.node;
+    idx->view.pl_text = reinterpret_cast<const unsigned long long*>(a.text);
+    idx->view.pl_rc = a.rc; idx->view.pl_stop = a.stop;
+    idx->view.pl_n = n_pos;
+    return MGB_OK;
+}
+#endif
+
 extern "C" {
 
 const char* mgb_last_error(void) { return g_err.c_str(); }
@@ -523,9 +609,9 @@ int mgb_index_create(const uint8_t *W, const uint8_t *last, uint64_t n_plus_1, c
         }
         if (e == cudaSuccess) e = cudaGetLastError();
         if (e == cudaSuccess) e = cudaDeviceSynchronize();
-        cudaFree(bwd_arr); cudaFree(c0); cudaFree(c1); cudaFree(multi); cudaFree(kmer);
+        cudaFree(bwd_arr); cudaFree(c0); cudaFree(c1); cudaFree(multi);
         if (e != cudaSuccess) {
-            cudaFree(radj); cudaFree(kh_keys); cudaFree(kh_vals);
+            cudaFree(kmer); cudaFree(radj); cudaFree(kh_keys); cudaFree(kh_vals);
             return fail(MGB_ERR_CUDA, std::string("radj / k-mer hash build: ") + cudaGetErrorString(e));
         }
         idx->bufs.push_back(radj);
@@ -535,7 +621,10 @@ int mgb_index_create(const uint8_t *W, const uint8_t *last, uint64_t n_plus_1, c
             idx->bufs.push_back(kh_keys); idx->bufs.push_back(kh_vals);
             idx->device_bytes += kh_slots * 12;
             idx->view.kh_keys = kh_keys; idx->view.kh_vals = kh_vals; idx->view.kh_slots = kh_slots;
+            rc = build_path_layout(idx.get(), kmer);
         }
+        cudaFree(kmer);
+        if (rc) return rc;
     }
 #endif
     *out = idx.release();
@@ -1013,6 +1102,8 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             }
             if (n_warps64 > ((uint64_t)list.size() + gpb - 1) / gpb * gpb) n_warps64 = ((uint64_t)list.size() + gpb - 1) / gpb * gpb;
             uint32_t n_warps = (uint32_t)n_warps64;
+            if (dbg_time) std::fprintf(stderr, "[mgb] k_align grid: %u lane groups (%llu resident)\n", n_warps,
+                                       (unsigned long long)index->num_sms * blocks_per_sm * gpb);
 #endif
             // output heap: generous first guess, doubled on retry passes
             uint64_t per_read = sizeof(OutAln) + 9ull * (b.L_max + 64 + index->view.k) + 4ull * 64;

@@ -40,6 +40,8 @@ static constexpr int kBlkEdges = 64;
 static constexpr int kBlkWords = 16;
 static constexpr int kSelLastRate = 64;
 static constexpr int kSelWRate = 32;
+static constexpr uint32_t kPlNone = 0xFFFFFFFFu;    // IndexView::pl_pos of an edge that is not a DBG node
+static constexpr uint64_t kPlPad = 256;             // filler positions after the last path (a multiple of 64)
 
 struct IndexView {
     const uint32_t *blocks;     // nblk * 16 words
@@ -57,6 +59,23 @@ struct IndexView {
     const unsigned long long *kh_keys;
     const uint32_t *kh_vals;
     uint64_t kh_slots;
+    // Path layout (graphs with the k-mer hash index; pl_n == 0: absent). The DBG nodes are covered by disjoint paths
+    // (each step from a node to its child), laid out one after another in a position space of pl_n positions, with k - 1
+    // filler positions after every path (k_path_* in kernels.cuh builds it):
+    //   pl_node[p]  the node whose k-mer starts at position p, 0 at a filler position
+    //   pl_text     the characters of the positions, 2 bits each (position i in bits 2i.. of the packed words, as the
+    //               hash keys); the k-mer of pl_node[p] is pl_text[p .. p + k)
+    //   pl_rc       1 bit per position: the reverse complement of pl_node[p]'s k-mer is in the hash index (the meaning
+    //               of the adjacency records' bits 16..20)
+    //   pl_stop     1 bit per position: pl_node[p] == 0
+    //   pl_pos[e]   the position of edge e, kPlNone unless e is a DBG node
+    // The arrays end with at least kPlPad filler positions, so readers may run ahead of a path's end.
+    const uint32_t *pl_node;
+    const uint32_t *pl_pos;
+    const unsigned long long *pl_text;
+    const uint32_t *pl_rc;
+    const uint32_t *pl_stop;
+    uint64_t pl_n;
     uint64_t n;                 // number of edges (ids 1..n)
     uint32_t nblk;
     uint32_t k;                 // DBG k; BOSS node length = k - 1

@@ -775,6 +775,36 @@ struct SectorOut {
     }
 };
 
+// A walk along the path layout (IndexView::pl_*): the character, reverse-complement and stop bits of position q, read
+// sequentially, each array by the aligned word that holds q. Words are loaded only when q enters them; the filler
+// padding at the end of the layout keeps that inside the arrays. The node ids are not read here: k_seed_hash copies the
+// run a whole warp at a time once the walk leaves it.
+struct PathWalk {
+    uint32_t q;                   // position of the k-mer the next step would reach
+    bool on;                      // still on the path
+    unsigned long long tw;        // pl_text word holding position q + k - 1 (the last character of q's k-mer)
+    uint32_t rw, sw;              // pl_rc / pl_stop words holding q
+    MGB_D void load(const IndexView &ix, bool all) {
+        const uint32_t qt = q + ix.k - 1;
+        if (all || (qt & 31) == 0) tw = __ldg(ix.pl_text + (qt >> 5));
+        if (all || (q & 31) == 0) { rw = __ldg(ix.pl_rc + (q >> 5)); sw = __ldg(ix.pl_stop + (q >> 5)); }
+    }
+    // the walk's k-mer is the one of edge e (stored, so a DBG node): start after its position, if it has one
+    MGB_D void start(const IndexView &ix, uint64_t e, bool stored) {
+        const uint32_t p = stored && ix.pl_n ? __ldg(ix.pl_pos + e) : kPlNone;
+        on = p != kPlNone;
+        q = p + 1;
+        tw = 0; rw = 0; sw = ~0u;
+        if (on) load(ix, true);
+    }
+    // the next k-mer, whose last character is c (valid), is the one at q
+    MGB_D bool next_is(const IndexView &ix, uint32_t c) const {
+        return on && ((tw >> (2 * ((q + ix.k - 1) & 31))) & 3u) == c - 1 && !((sw >> (q & 31)) & 1u);
+    }
+    MGB_D bool rc() const { return (rw >> (q & 31)) & 1u; }
+    MGB_D void step(const IndexView &ix) { ++q; load(ix, false); }
+};
+
 // BOSS::map_to_edges (boss.cpp:996-1045) on graphs with the k-mer hash index (DNA block layout, k <= 31), one read per
 // lane. A strand walked in order costs one load per k-mer: the adjacency record of the previous k-mer's edge while the
 // walk is warm (boss.cpp:1024-1043), the k-mer's bucket (+ the value on a hit) when it is cold (map_to_edge,
@@ -790,6 +820,14 @@ struct SectorOut {
 // own characters, read backwards. Its first k-mer (position 0) is the probe's miss. If both probes hit (CANONICAL-mode
 // graphs, regions stored in both orientations) or neither does (an error in the first k-mer), the strands are walked
 // one after the other. (c2 prepare + seed: 14.8 ms -> 7.2 ms, DESIGN.md §3.2.)
+//
+// With the path layout, the strand walked in order starts at its probe's position on the path (PathWalk) and stays on the
+// path while each next character is the path's and the path goes on: k-mer t is then the string stored at q, so its node
+// id is pl_node[q] and pl_rc[q] stands in for the adjacency record's reverse-complement bit. Such a step loads nothing
+// but the layout's character and bit words in order (one per 32 steps); when the secondary needs no lookup either it
+// skips the lookup code altogether. The run's node ids are copied at the end of the pass, by the warp together. At the
+// first mismatch, invalid character or path end the walk goes on as above from the last node on the path, and does not
+// return to it. (c2 k_seed_hash: 6.0 ms -> 2.85 ms, DESIGN.md §3.2.)
 //
 // Steps are written with selects rather than branches: lanes in different regimes issue together. Persistent grid:
 // lane t of n_lanes takes the reads t + n_lanes * round.
@@ -836,6 +874,8 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
             const bool store0 = edge != 0 && in_graph(ix, edge);
             so.put_up(out, 0, nk, store0 ? edge : 0);
             seen |= (store0 ? 2u : 1u) << sh;
+            PathWalk pw;
+            pw.start(ix, edge, store0 && nk > 1);
             // ... and the secondary, backwards: characters L - 1 .. nk of its k-mer at nk - 1 first
             CodeStreamDown ds;
             ds.start((sp ? a.cf : a.cr) + b, paired ? L : 0);
@@ -856,12 +896,23 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
                 if (c < 1 || c >= sigma) last_bad = t + K - 1;
                 key = (key >> 2) | ((unsigned long long)((c - 1) & 3u) << top);
                 const bool ok = last_bad < t;                          // a k-mer without an invalid character
-                const bool warm = ok && edge != 0, cold = ok && edge == 0;
+                // on the path: the k-mer t - 1 is the one at q - 1, so k-mer t is the one at q if its last character is
+                // q's and q is on the same path. Leaving it, the walk goes on from the last node on it.
+                const bool path = ok && pw.next_is(ix, c);
+                if (pw.on && !path) { if (ok) edge = __ldg(ix.pl_node + pw.q - 1); pw.on = false; }
+                const bool warm = ok && edge != 0 && !path, cold = ok && edge == 0;
                 const int j = nk - t;
                 const uint32_t c2 = ds.next();
                 if (c2 < 1 || c2 >= sigma) bad2 = j;
                 key2 = ((key2 << 2) | ((c2 - 1) & 3u)) & mask;
                 const bool cold2 = paired && look2 && bad2 >= j + K;
+                if (path && !cold2) {                                  // no lookup on either strand: the short way
+                    look2 = pw.rc();
+                    pw.step(ix);
+                    seen |= 2u << sh;
+                    if (paired) { so2.put_down(out2, j, nk, 0); seen |= 1u << (2 - sh); }
+                    continue;
+                }
                 uint2 ar = make_uint2(0u, 0u);
                 if (warm) ar = load_adj(ix, edge);
                 KhProbe p, p2;
@@ -871,11 +922,16 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
                 // ---- consume: the k-mers' edges, stored if they are nodes of the graph
                 const uint64_t child = adj_child(ar, c);              // 0 unless warm (ar = 0)
                 const bool child_ok = (ar.y >> (8 + c)) & 1u;
-                look2 = !(warm && child != 0 && !((ar.y >> (16 + c)) & 1u));
-                edge = warm ? child : found;                           // 0 when the window is invalid
-                const bool store = warm ? (child != 0 && child_ok) : (found != 0 && in_graph(ix, found));
-                so.put_up(out, t, nk, store ? edge : 0);                // (store: edge != 0)
-                seen |= (store ? 2u : 1u) << sh;
+                look2 = path ? pw.rc() : !(warm && child != 0 && !((ar.y >> (16 + c)) & 1u));
+                if (path) {
+                    pw.step(ix);                                       // stored by the copy below
+                    seen |= 2u << sh;
+                } else {
+                    edge = warm ? child : found;                       // 0 when the window is invalid
+                    const bool store = warm ? (child != 0 && child_ok) : (found != 0 && in_graph(ix, found));
+                    so.put_up(out, t, nk, store ? edge : 0);            // (store: edge != 0)
+                    seen |= (store ? 2u : 1u) << sh;
+                }
                 if (paired) {
                     const bool store2 = found2 != 0 && in_graph(ix, found2);
                     so2.put_down(out2, j, nk, store2 ? found2 : 0);
@@ -885,6 +941,20 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
             if (paired) {
                 so2.put_down(out2, 0, nk, 0);                          // the probe's miss
                 seen |= 1u << (2 - sh);
+            }
+            // ---- the path run: k-mers 0 .. t of a lane that took t steps on the path are pl_node[p .. q) (p: the
+            // position of the probe's node, loaded again), copied by the lanes here together, 32 node ids per
+            // instruction. The copy comes after the lane's own stores: SectorOut may have written stale slots of the
+            // run's sectors.
+            const uint32_t from = pw.q != kPlNone + 1 ? __ldg(ix.pl_pos + (sp ? f1 : f0)) : pw.q;
+            const unsigned grp = __activemask();
+            const int width = __popc(grp), rank = __popc(grp & ((1u << (threadIdx.x & 31)) - 1u));
+            __syncwarp(grp);
+            for (unsigned todo = __ballot_sync(grp, pw.q - from > 1); todo; todo &= todo - 1) {
+                const int src = __ffs(todo) - 1;
+                uint64_t *dst = reinterpret_cast<uint64_t*>(__shfl_sync(grp, (unsigned long long)out, src));
+                const uint32_t f = __shfl_sync(grp, from, src), len = __shfl_sync(grp, pw.q - from, src);
+                for (uint32_t i = rank; i < len; i += width) dst[i] = __ldg(ix.pl_node + f + i);
             }
         }
         if (a.summary) a.summary[r] = (uint8_t)seen;
@@ -1084,6 +1154,144 @@ __global__ void __launch_bounds__(256) k_adj_rc(IndexView ix, uint2 *adj, const 
         if (bits) adj[e].y = a.y | bits;
     }
 }
+
+// Path layout (IndexView::pl_*), built once the hash index is complete. Its nodes are the DBG nodes the seeding walk
+// stores (in_graph, a k-mer without '$'). A node whose target has exactly one such child links to it; a child that several
+// nodes link to keeps the smallest of them, the others end their paths. Cycles (tandem repeats shorter than k, circular
+// inputs) are cut at their smallest node. Positions come from pointer jumping over `jump`, one word per edge:
+//   0                          not a DBG node
+//   next | dist << 32          not done: `next` is dist steps ahead on the path
+//   tail | dist << 32 | kJDone done: the path's last node is dist steps ahead (k_path_heads then puts the tail's
+//                              position in place of its own id, dist 0)
+// Cycle nodes never get done; k_path_cycle_* then hold (next | smallest node seen << 32) instead. Edge ids are < 2^31.
+struct PathArgs {
+    IndexView ix;                        // with the hash index
+    const unsigned long long *kmer;      // per edge (RadjArgs::kmer)
+    uint32_t *pred;                      // per edge: the node linking to it, kPlNone if none; k_path_place: pl_pos
+    unsigned long long *jump;            // per edge, as above
+    uint32_t *node; unsigned int *text, *rc, *stop;           // pl_node / pl_text / pl_rc cleared, pl_stop all
+                                                              // ones (k_path_place)
+    unsigned long long *total;           // positions handed out (k_path_heads)
+    unsigned int *count;                 // nodes that got done in a round / cycle nodes
+};
+static constexpr unsigned long long kJDone = 1ull << 63;
+MGB_D bool path_node(const PathArgs &a, uint64_t e) { return in_graph(a.ix, e) && a.kmer[e] != kKmerBad; }
+// the child that DBG node e links to if it is the only one, else 0
+MGB_D uint64_t path_child(const PathArgs &a, uint64_t e) {
+    const uint2 ar = a.ix.adj[e];
+    const uint32_t ok = (ar.y >> 8) & 31u;
+    if (popc32(ok) != 1) return 0;
+    const uint64_t c = adj_child(ar, (uint32_t)ffs32(ok) - 1);
+    return c && a.kmer[c] != kKmerBad ? c : 0;
+}
+MGB_D void count_warp(unsigned int *count, bool p) {
+    const unsigned m = __ballot_sync(0xffffffffu, p);
+    if (m && (threadIdx.x & 31) == __ffs(m) - 1) atomicAdd(count, (unsigned)__popc(m));
+}
+#define MGB_EDGE_LOOP(e, n) \
+    for (uint64_t e = 1 + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e <= (n); e += (uint64_t)gridDim.x * blockDim.x)
+__global__ void __launch_bounds__(256) k_path_pred(PathArgs a) {
+    MGB_EDGE_LOOP(e, a.ix.n) {
+        if (!path_node(a, e)) continue;
+        const uint64_t c = path_child(a, e);
+        if (c) atomicMin(a.pred + c, (uint32_t)e);
+    }
+}
+__global__ void __launch_bounds__(256) k_path_link(PathArgs a) {
+    MGB_EDGE_LOOP(e, a.ix.n) {
+        unsigned long long j = 0;
+        if (path_node(a, e)) {
+            const uint64_t c = path_child(a, e);
+            j = c && a.pred[c] == (uint32_t)e ? (1ull << 32) | c : kJDone | e;
+        }
+        a.jump[e] = j;
+    }
+}
+// One round of pointer jumping, in place: a word read from another node is a valid (next, dist) pair whether or not that
+// node has jumped in this round yet. *count: the nodes that got done. (The block-uniform loop keeps the ballot whole.)
+__global__ void __launch_bounds__(256) k_path_jump(PathArgs a) {
+    const uint64_t nt = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t base = (uint64_t)blockIdx.x * blockDim.x; base < a.ix.n; base += nt) {
+        const uint64_t e = 1 + base + threadIdx.x;
+        bool done = false;
+        if (e <= a.ix.n) {
+            const unsigned long long x = a.jump[e];
+            if (x && !(x & kJDone)) {
+                const unsigned long long y = a.jump[(uint32_t)x];
+                const unsigned long long d = ((x >> 32) + (y >> 32)) & 0x7FFFFFFFull;   // (cycle nodes: wraps, unused)
+                a.jump[e] = (y & (kJDone | 0xFFFFFFFFull)) | (d << 32);
+                done = (y & kJDone) != 0;
+            }
+        }
+        count_warp(a.count, done);
+    }
+}
+// the nodes left undone are on cycles: each starts with itself as the smallest node seen; *count: how many
+__global__ void __launch_bounds__(256) k_path_cycle_init(PathArgs a) {
+    const uint64_t nt = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t base = (uint64_t)blockIdx.x * blockDim.x; base < a.ix.n; base += nt) {
+        const uint64_t e = 1 + base + threadIdx.x;
+        bool cyc = false;
+        if (e <= a.ix.n) {
+            const unsigned long long x = a.jump[e];
+            cyc = x && !(x & kJDone);
+            if (cyc) a.jump[e] = (e << 32) | path_child(a, e);
+        }
+        count_warp(a.count, cyc);
+    }
+}
+// one doubling round of the smallest node over the cycle ahead
+__global__ void __launch_bounds__(256) k_path_cycle_min(PathArgs a) {
+    MGB_EDGE_LOOP(e, a.ix.n) {
+        const unsigned long long x = a.jump[e];
+        if (!x || (x & kJDone)) continue;
+        const unsigned long long y = a.jump[(uint32_t)x];
+        const unsigned long long m = (x >> 32) < (y >> 32) ? (x >> 32) : (y >> 32);
+        a.jump[e] = (m << 32) | (y & 0xFFFFFFFFull);
+    }
+}
+// the cycle node whose child is the cycle's smallest node becomes a tail, the smallest node a head
+__global__ void __launch_bounds__(256) k_path_cycle_cut(PathArgs a) {
+    MGB_EDGE_LOOP(e, a.ix.n) {
+        const unsigned long long x = a.jump[e];
+        if (!x || (x & kJDone)) continue;
+        const uint64_t c = path_child(a, e);
+        if (c == (x >> 32)) { a.jump[e] = kJDone | e; a.pred[c] = kPlNone; }
+        else a.jump[e] = (1ull << 32) | c;
+    }
+}
+// every head takes the positions of its path and the k - 1 filler positions after it, and leaves the tail's position in
+// the tail's word
+__global__ void __launch_bounds__(256) k_path_heads(PathArgs a) {
+    MGB_EDGE_LOOP(e, a.ix.n) {
+        if (a.pred[e] != kPlNone) continue;
+        const unsigned long long x = a.jump[e];
+        if (!x) continue;
+        const uint64_t d = (x >> 32) & 0x7FFFFFFFull;
+        const unsigned long long base = atomicAdd(a.total, (unsigned long long)(d + a.ix.k));
+        a.jump[(uint32_t)x] = kJDone | ((base + d) & 0xFFFFFFFFull);
+    }
+}
+// pl_pos, pl_node, pl_text (every node its first character, a tail all k), pl_rc and pl_stop
+__global__ void __launch_bounds__(256) k_path_place(PathArgs a) {
+    const int K = (int)a.ix.k;
+    MGB_EDGE_LOOP(e, a.ix.n) {
+        const unsigned long long x = a.jump[e];
+        if (!x) { a.pred[e] = kPlNone; continue; }
+        const uint64_t d = (x >> 32) & 0x7FFFFFFFull;
+        const uint64_t pos = d == 0 ? (uint32_t)x : (uint32_t)a.jump[(uint32_t)x] - d;
+        a.pred[e] = (uint32_t)pos;
+        a.node[pos] = (uint32_t)e;
+        atomicAnd(a.stop + (pos >> 5), ~(1u << (pos & 31)));
+        const unsigned long long km = a.kmer[e];
+        for (int i = 0; i < (d == 0 ? K : 1); ++i) {
+            const uint64_t q = pos + i;
+            atomicOr(a.text + (q >> 4), (unsigned)((km >> (2 * i)) & 3u) << (2 * (q & 15)));
+        }
+        if (kh_lookup(a.ix, kh_revcomp(km, a.ix.k))) atomicOr(a.rc + (pos >> 5), 1u << (pos & 31));
+    }
+}
+#undef MGB_EDGE_LOOP
 __global__ void __launch_bounds__(256) k_radj_pack(RadjArgs a, uint32_t multi_shift) {
     uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     uint64_t nt = (uint64_t)gridDim.x * blockDim.x;
