@@ -151,6 +151,22 @@ struct OutAln {
 struct ReadStats { uint32_t num_seeds, num_extensions, num_explored_nodes, dp_columns; uint64_t dp_cells; };
 #if defined(MGB_HOST_EMU)
 extern "C" unsigned long long mgb_emu_whole_read_hits;   // host emulation (tests) only: reads answered by exact_read_strand()
+// host emulation (tests) only: how often the aligner leaves its on-chip working set, so that a test can show which of
+// these paths its inputs reach. The order is part of the test interface (tests/parity_common.py EMU_PATHS).
+enum EmuPath : int {
+    EMU_QUEUE_MIGRATE,        // heap_push: the best-first queue moves to the arena
+    EMU_NN_MIGRATE,           // nn_push: the next-nodes list moves to the arena
+    EMU_COLUMN_MIGRATE,       // extend_ins_end: an on-chip column moves to arena scratch mid-column
+    EMU_ARENA_COLUMN,         // a column (root or child) created in arena scratch: wider than the on-chip buffers
+    EMU_UNSTAGED_READ,        // a read whose strands are not staged on chip (L + 1 > lq)
+    EMU_GENERAL_COLUMN,       // a child column computed by the general path
+    EMU_READ_OVERFLOW,        // a read marked MGB_READ_OVERFLOW (retried with a larger arena)
+    EMU_N_PATHS
+};
+extern "C" unsigned long long mgb_emu_path_hits[EMU_N_PATHS];
+#define MGB_EMU_HIT(path) __atomic_fetch_add(&mgb_emu_path_hits[path], 1ull, __ATOMIC_RELAXED)
+#else
+#define MGB_EMU_HIT(path) ((void)0)
 #endif
 
 #if defined(MGB_PHASE_TIMERS) && MGB_DEVICE_CODE
@@ -1731,6 +1747,7 @@ struct ReadAligner {
     MGB_HD void heap_push(int &n, HeapItem it) {
         if (n >= hp_cap) {
             if (hp == m.heap()) { overflow = true; return; }
+            MGB_EMU_HIT(EMU_QUEUE_MIGRATE);
             for (int t = wlane(); t < n; t += kWarp) m.heap()[t] = hp[t];
             wsync();
             hp = m.heap(); hp_cap = caps.max_cols;
@@ -1765,6 +1782,7 @@ struct ReadAligner {
     MGB_HD void nn_push(int &n, HeapItem it) {
         if (n >= np_cap) {
             if (np == m.next_nodes()) { overflow = true; return; }
+            MGB_EMU_HIT(EMU_NN_MIGRATE);
             for (int t = wlane(); t < n; t += kWarp) m.next_nodes()[t] = np[t];
             wsync();
             np = m.next_nodes(); np_cap = caps.max_cols;
@@ -1814,6 +1832,7 @@ struct ReadAligner {
         if (size + cnt + 5 > sc.cap) {
             Scratch big;                               // only an on-chip scratch can be too small
             if (!sc.on_chip || !scratch_arena(max_size, &big)) { overflow = true; return size; }
+            MGB_EMU_HIT(EMU_COLUMN_MIGRATE);
             for (int t = wlane(); t < size + 5 && t < sc.cap; t += kWarp) {
                 big.S[t] = sc.S[t]; big.E[t] = sc.E[t]; big.F[t] = sc.F[t];
             }
@@ -2100,7 +2119,7 @@ struct ReadAligner {
             Scratch sc;
             bool have_sc = true;
             if (1 + 8 <= sm.bmax()) sc = scratch_smem(0);
-            else have_sc = scratch_arena(wlen + 1, &sc);
+            else { have_sc = scratch_arena(wlen + 1, &sc); MGB_EMU_HIT(EMU_ARENA_COLUMN); }
             if (have_sc) {
                 for (int t = wlane(); t < 1 + 5; t += kWarp) { sc.S[t] = kNinf; sc.E[t] = kNinf; sc.F[t] = kNinf; }
                 wsync();
@@ -2420,6 +2439,7 @@ struct ReadAligner {
             }
             // ---- general path: columns of any width, S | E | F in the table
             MGB_COUNT(6);
+            MGB_EMU_HIT(EMU_GENERAL_COLUMN);
             if (par_fmt == FMT_COMPACT && pb >= 0) {
                 // the backtrack compares the F of a general-path column with its parent's (:976-997): write the
                 // parent's F (still on chip) into the space its compact record reserves for it
@@ -2432,7 +2452,7 @@ struct ReadAligner {
             }
             Scratch sc;
             if (size0 + 8 <= sm.bmax()) { sc = scratch_smem(cb); if (cb) res1 = -1; else res0 = -1; }
-            else if (!scratch_arena(wlen + 1 - begin, &sc)) continue;
+            else { MGB_EMU_HIT(EMU_ARENA_COLUMN); if (!scratch_arena(wlen + 1 - begin, &sc)) continue; }
             // DPTColumn::create: everything (incl. padding) = ninf (extender.cpp:389-410)
             for (int j = wlane(); j < size0 + 5; j += kWarp) { sc.S[j] = kNinf; sc.E[j] = kNinf; sc.F[j] = kNinf; }
             wsync();
@@ -3395,7 +3415,7 @@ struct ReadAligner {
             if (L + 1 <= sm.lq()) {
                 for (int i = wlane(); i < L; i += kWarp) { sm.q0()[i] = qf[i]; sm.q1()[i] = qr[i]; }
                 c0.q = sm.q0(); c1.q = sm.q1(); c0.ps = sm.psum0(); c1.ps = sm.psum1();
-            }
+            } else MGB_EMU_HIT(EMU_UNSTAGED_READ);
             sm.ctx()[0] = c0; sm.ctx()[1] = c1;
         }
         wsync();

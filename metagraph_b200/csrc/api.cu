@@ -1223,7 +1223,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             const uint32_t heap_id = (uint32_t)res->heaps.size() - 1;
             for (uint32_t r : list) {
                 const ReadHdr &h = hdr_host[r];
-                if (h.status == MGB_READ_OVERFLOW) { retry.push_back(r); continue; }
+                if (h.status == MGB_READ_OVERFLOW) { MGB_EMU_HIT(EMU_READ_OVERFLOW); retry.push_back(r); continue; }
                 res->stats.num_seeds += h.stats.num_seeds;
                 res->stats.num_extensions += h.stats.num_extensions;
                 res->stats.num_explored_nodes += h.stats.num_explored_nodes;
@@ -1283,7 +1283,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
 
 static std::atomic<uint32_t> g_max_pieces{0};      // 0 = automatic
 #if defined(MGB_HOST_EMU)
-extern "C" { unsigned long long mgb_emu_whole_read_hits = 0; }
+extern "C" { unsigned long long mgb_emu_whole_read_hits = 0; unsigned long long mgb_emu_path_hits[EMU_N_PATHS] = {}; }
 #endif
 
 extern "C" {

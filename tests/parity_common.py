@@ -112,6 +112,23 @@ def whole_read_hits(lib):
         return None
 
 
+# the aligner's spill / migration sites the host-emulation build counts (align_core.cuh EmuPath, same order)
+EMU_PATHS = ("queue_migrate", "nn_migrate", "column_migrate", "arena_column", "unstaged_read", "general_column",
+             "read_overflow")
+
+
+def path_hits(lib):
+    """test counters of the host-emulation build by path name (None for the product library)"""
+    import ctypes
+    from metagraph_b200 import _lib
+    L = _lib.load_library(lib)
+    try:
+        hits = (ctypes.c_ulonglong * len(EMU_PATHS)).in_dll(L, "mgb_emu_path_hits")
+    except ValueError:
+        return None
+    return dict(zip(EMU_PATHS, hits))
+
+
 def exact_shortcut_case(lib, seed, k, cfg, nseq=3, G=3000, nreads=80, L=90):
     """Reads that match a path of the graph exactly (the exact-path shortcut of the extender applies to them) on a
     graph with variants and a tandem repeat, mixed with reads carrying errors; kernels (shortcut on) == oracle, and
@@ -705,3 +722,154 @@ RANDOM_CASES = [
     # large enough for the device-refined suffix-range levels (s > 8)
     (12, 31, 400000, 30, 150, 0.02, lambda k: cli_defaults(k, min_seed_length=31, max_seed_length=31), False, 1),
 ]
+
+
+# Inputs that push k_align out of its on-chip working set, one per path (align_core.cuh): DP columns wider than the
+# on-chip column buffers (created in arena scratch, or moved there mid-column by extend_ins_end), reads not staged on
+# chip, the best-first queue and the next-nodes list moving to the arena, reads that overflow their arena and are retried
+# with a larger one. The copies between the two places are warp-cooperative, so only the device can show a race in them;
+# the host emulation shows that each input reaches its path (PRESSURE_TARGETS, path_hits).
+PRESSURE_INPUTS = ("insertions", "insertions_cheap_gaps", "wide_band", "queue", "retry")
+PRESSURE_TARGETS = {
+    "insertions": ("column_migrate", "arena_column"),
+    "insertions_cheap_gaps": ("column_migrate", "arena_column"),
+    "wide_band": ("arena_column", "unstaged_read"),
+    "queue": ("queue_migrate", "nn_migrate"),
+    "retry": ("read_overflow",),
+}
+
+
+def _random_seq(rng, n):
+    return "".join(np.array(list("ACGT"))[rng.integers(0, 4, n)])
+
+
+def pressure_input(name):
+    """(k, graph sequences, reads, config) of one of PRESSURE_INPUTS"""
+    if name in ("insertions", "insertions_cheap_gaps"):
+        # 300 bp windows with 40 bp of random sequence inserted in the middle or put in place of the last 20 bp: under a
+        # large x-drop the insertion runs of extend_ins_end grow a column past the on-chip buffers while it is computed
+        rng = np.random.default_rng(301)
+        k = 15
+        genome = _random_seq(rng, 5000)
+        reads = []
+        for i in range(40):
+            p = int(rng.integers(0, len(genome) - 300))
+            w, ins = genome[p:p + 300], _random_seq(rng, 40)
+            r = w[:150] + ins + w[150:] if i % 2 else w[:280] + ins
+            reads.append(revcomp(r) if i % 3 == 0 else r)
+        kw = dict(xdrop=1000) if name == "insertions" else dict(xdrop=300, gap_opening_penalty=-2, gap_extension_penalty=-1)
+        return k, [genome], reads, cli_defaults(k, min_exact_match=0.0, **kw)
+    if name == "wide_band":
+        # no x-drop: a column spans the whole read. Reads of 249 .. 600 bp: the on-chip buffers are capped at 256 cells
+        # and a batch with a read over 511 bp stages no query on chip (lq = 0)
+        rng = np.random.default_rng(302)
+        k = 13
+        genome = _random_seq(rng, 1500)
+        reads = []
+        for i in range(10):
+            L = 600 if i == 0 else 249 if i == 1 else int(rng.integers(249, 601))
+            p = int(rng.integers(0, len(genome) - L))
+            r = mutate(rng, genome[p:p + L], 0.03)
+            reads.append(revcomp(r) if i % 2 else r)
+        return k, [genome], reads, struct_defaults()
+    if name == "queue":
+        # tandem repeats on a low-complexity graph, three alternative paths and a large node budget: many columns wait in
+        # the queue (and tie for the next-nodes list) at once, more than the on-chip queue holds
+        rng = np.random.default_rng(303)
+        k = 11
+        base = lowcx_genome(rng, 4000)
+        unit = _random_seq(rng, 7)
+        seqs = [base, base[:600] + unit * 30 + base[600:1400], mutate(rng, base[2000:3500], 0.03)]
+        reads = []
+        for i in range(30):
+            s_ = seqs[i % 3]
+            p = int(rng.integers(0, len(s_) - 150))
+            r = mutate(rng, s_[p:p + 150], 0.04)
+            reads.append(revcomp(r) if i % 2 else r)
+        reads.append(base[580:600] + unit * 14 + base[600:620])
+        cfg = cli_defaults(k, min_seed_length=8, num_alternative_paths=3, max_nodes_per_seq_char=50.0, xdrop=60,
+                           min_exact_match=0.0, rel_score_cutoff=0.0)
+        return k, seqs, reads, cfg
+    if name == "retry":
+        # low-complexity sequence (homopolymers, short tandem repeats) with every seed kept, sub-k seeds, a large x-drop
+        # and node budget: about half the reads from it explore more columns than their arena holds at scale 1 and are
+        # retried with a larger one; the reads from the unique sequence in the same batch are not
+        rng = np.random.default_rng(304)
+        k = 15
+        seqs = [lowcx_genome(rng, 3000), _random_seq(rng, 2000)]
+        reads = []
+        for i in range(30):
+            s_, L = (seqs[0], 150) if i % 2 == 0 else (seqs[1], 110)
+            p = int(rng.integers(0, len(s_) - L))
+            r = mutate(rng, s_[p:p + L], 0.03)
+            reads.append(revcomp(r) if i % 3 == 0 else r)
+        cfg = cli_defaults(k, min_seed_length=6, max_num_seeds_per_locus=SIZE_MAX, max_nodes_per_seq_char=20.0,
+                           xdrop=100, min_exact_match=0.0)
+        return k, seqs, reads, cfg
+    raise ValueError(name)
+
+
+_pressure_expected = {}
+
+
+def pressure_case(lib, name):
+    """Runs the pressure input `name` through the library: lines == oracle (node paths included). Returns the run's
+    statistics and, on the host emulation, how often it took each path (path_hits; None on the device). The index is
+    built inside the call, so index-side knobs set in the environment apply."""
+    k, seqs, reads, cfg = pressure_input(name)
+    if name not in _pressure_expected:
+        _pressure_expected[name] = O.OracleGraph(k, seqs).align_tsv(cfg, reads, with_nodes=True)
+    exp = _pressure_expected[name]
+    idx = DBGSuccinctIndex(BOSSTable.from_sequences(k, seqs, lib=lib), lib=lib)
+    h0 = path_hits(lib)
+    got, stats = run_lines(idx, cfg, reads)
+    h1 = path_hits(lib)
+    idx.close()
+    bad = [i for i in range(len(reads)) if exp[i] != got[i]]
+    assert not bad, (name, bad[:3], exp[bad[0]][:300], got[bad[0]][:300])
+    return stats, None if h0 is None else {p: h1[p] - h0[p] for p in EMU_PATHS}
+
+
+# Knobs of api.cu that move k_align's on-chip limits or switch a path off (name, environment). Where a column, the queue
+# or a query strand lives must change neither the lines nor the DP: every run equals the oracle, and its DP_COUNTERS
+# equal those of the default run. The host chooses the smallest column buffer as 64 cells (the register path of the
+# extender needs 40); a small queue or staging limit only makes the checks on every push and every read (n >= hp_cap,
+# L + 1 <= lq) fire earlier. The k-mer hash and path index exist on the device only.
+SPILL_KNOBS = (
+    ("default", {}),
+    ("bmax64", {"MGB_TEST_BMAX": "64"}),
+    ("lq0", {"MGB_TEST_LQ": "0"}),
+    ("lq_split", {"MGB_TEST_LQ": None}),                                 # pressure_lq_split: some reads staged, some not
+    ("hcap1", {"MGB_TEST_HCAP": "1"}),
+    ("hcap4", {"MGB_TEST_HCAP": "4"}),
+    ("nofast", {"MGB_TEST_NOFAST": "1"}),                                # no register path: every column general
+    ("nosubk", {"MGB_TEST_NOSUBK": "1"}),                                # sub-k seeds (min_seed_length < k) in k_align
+    ("nopremap", {"MGB_TEST_NOPREMAP": "1", "MGB_NO_KMER_HASH": "1"}),   # premap runs only without the k-mer hash
+    ("no_path_index", {"MGB_NO_PATH_INDEX": "1"}),
+    ("wide", {"MGB_TEST_WIDE": "1"}),                                    # the alphabet-generic index layout
+    ("pieces3", {"MGB_TEST_PIECES": "3"}),                               # retried reads in several pieces and heaps
+)
+DP_COUNTERS = ("num_seeds", "num_extensions", "num_explored_nodes", "dp_cells", "dp_columns")
+
+
+def pressure_lq_split(name):
+    """a staging limit (multiple of 16) that stages some reads of the input on chip and leaves others in global memory"""
+    lens = [len(r) for r in pressure_input(name)[2]]
+    fits = [lq for lq in range(16, 1024, 16) if min(lens) + 1 <= lq < max(lens) + 1]
+    assert fits, (name, min(lens), max(lens))
+    return fits[len(fits) // 2]
+
+
+def pressure_knob_matrix(lib, name, monkeypatch, knobs=SPILL_KNOBS):
+    """Runs the pressure input `name` under every knob: lines == oracle, DP counters == the default run's. Returns
+    {knob: (statistics, path hits)}; path hits are None on the device."""
+    out = {}
+    for knob, env in knobs:
+        with monkeypatch.context() as mp:
+            for var, val in env.items():
+                mp.setenv(var, str(pressure_lq_split(name)) if val is None else val)
+            out[knob] = pressure_case(lib, name)
+        base = out[knobs[0][0]][0]
+        diff = {c: (base[c], out[knob][0][c]) for c in DP_COUNTERS if out[knob][0][c] != base[c]}
+        assert not diff, (name, knob, diff)
+    return out

@@ -114,10 +114,14 @@ def test_seed_complexity_filter_emu():
 
 
 def test_c1_shape_emu():
-    """configs[0] shape: transcripts aligned to their own k=12 graph, ragged lengths up to 2.5 kbp
-    (longer than the on-chip column buffers: the arena scratch and unstaged-query paths run)."""
+    """configs[0] shape: transcripts aligned to their own k=12 graph, ragged lengths up to 2.5 kbp. The batch holds
+    reads over 511 bp, so no read is staged on chip; at the CLI's x-drop every DP column still fits the on-chip
+    buffers (the arena-column paths are reached by the pressure inputs, test_pressure_inputs_reach_their_paths_emu)."""
+    h0 = P.path_hits(EMU)
     n, full = P.c1_case(EMU, 10, 2500)
+    h1 = P.path_hits(EMU)
     assert full >= n - 2
+    assert h1["unstaged_read"] - h0["unstaged_read"] >= n
 
 
 def test_c1_transcripts_subset_emu():
@@ -227,3 +231,27 @@ def test_bad_min_cell_score_emu():
         O.OracleGraph(3, []).align_tsv(cfg, ["ACGT"])
     B200Aligner(idx, struct_defaults(score_matrix=dna_scoring_matrix(2, -1, -2)))   # the same graph with a sane config
     idx.close()
+
+
+@pytest.mark.parametrize("name", P.PRESSURE_INPUTS)
+def test_pressure_inputs_reach_their_paths_emu(name):
+    """Each pressure input reaches the spill / migration / retry path it is built for (the emulation counts the
+    aligner's sites), and the emulation equals the oracle on it. test_spill_paths_gpu.py runs the same bytes on the
+    device, where the lanes of a warp share the copies to the arena."""
+    stats, hits = P.pressure_case(EMU, name)
+    for path in P.PRESSURE_TARGETS[name]:
+        assert hits[path] > 0, (name, path, hits)
+    if name == "retry":
+        assert 0 < stats["num_reads_retried"] < len(P.pressure_input(name)[2]), stats
+
+
+@pytest.mark.parametrize("name", P.PRESSURE_INPUTS)
+def test_spill_knobs_emu(name, monkeypatch):
+    """The knob matrix of test_spill_paths_gpu.py on the emulation: every run equals the oracle and the default run's
+    DP counters, and the knobs that move an on-chip limit reach the path they move it to."""
+    hits = {knob: h for knob, (_, h) in P.pressure_knob_matrix(EMU, name, monkeypatch).items()}
+    assert hits["bmax64"]["arena_column"] > 0
+    assert 0 < hits["lq_split"]["unstaged_read"] < hits["lq0"]["unstaged_read"]
+    if name in ("queue", "retry"):                # the insertion and wide-band inputs never queue two columns
+        assert hits["hcap1"]["queue_migrate"] > hits["hcap4"]["queue_migrate"] > hits["default"]["queue_migrate"]
+        assert hits["nofast"]["general_column"] > hits["default"]["general_column"]

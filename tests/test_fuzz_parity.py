@@ -59,3 +59,13 @@ def test_fuzz_large_k_emu(k):
     for seed, mode in ((k, "basic"), (k + 1, "canonical"), (k + 2, "primary")):
         bad, info = P.fuzz_case(EMU, seed, canonical=mode == "canonical", primary=mode == "primary", k=k)
         assert not bad, (k, seed, mode, info)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("k", [47, 64, 84])
+def test_fuzz_large_k_gpu(k):
+    """test_fuzz_large_k_emu on the device: the 256-bit-key instantiations of k_seed / k_align (kern_any), in BASIC,
+    CANONICAL and PRIMARY mode."""
+    for seed, mode in ((k, "basic"), (k + 1, "canonical"), (k + 2, "primary")):
+        bad, info = P.fuzz_case(None, seed, canonical=mode == "canonical", primary=mode == "primary", k=k)
+        assert not bad, (k, seed, mode, info)

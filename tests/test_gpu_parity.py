@@ -52,6 +52,17 @@ def test_generic_layout_on_dna_gpu(monkeypatch):
         P.random_case(LIB, seed, k, G, n, L, rate, cfgf(k), mask, nseq)
 
 
+def test_general_path_gpu(monkeypatch):
+    """With the extender's register path switched off every column goes through the general path (S | E | F table
+    format), with all 32 lanes sharing a column: the goldens, MT and the first random cases still equal the oracle."""
+    monkeypatch.setenv("MGB_TEST_NOFAST", "1")
+    P.check_goldens(LIB)
+    P.check_mt(LIB, True)
+    for case in P.RANDOM_CASES[:5]:
+        seed, k, G, n, L, rate, cfgf, mask, nseq = case
+        P.random_case(LIB, seed, k, G, n, L, rate, cfgf(k), mask, nseq)
+
+
 def test_seed_complexity_filter_gpu():
     """seed complexity filter on (CLI default): kernels vs oracle on low-complexity inputs."""
     for seed, k, exact in ((31, 15, False), (32, 21, True), (33, 31, False)):
