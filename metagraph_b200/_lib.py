@@ -51,7 +51,7 @@ _libs = {}
 
 
 def load_library(path=None):
-    # MGB_LIB: another build of the same library (e.g. a different lane-group width), for probes
+    # MGB_LIB: another build of the same library (e.g. one with phase timers), for probes
     path = os.path.abspath(path or os.environ.get("MGB_LIB") or DEFAULT_LIB)
     if path in _libs:
         return _libs[path]

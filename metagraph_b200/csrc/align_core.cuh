@@ -187,10 +187,9 @@ enum { SLOT_SEED = 0, SLOT_TMP = 1, SLOT_EXT = 2, SLOT_BWD = 2 + kMaxAlt, SLOT_A
 // ------------------------------------------------------------------------------------
 MGB_HOSTDEV size_t align_up(size_t x) { return (x + 15) & ~(size_t)15; }
 
-// State handed to / taken back from the extender's chain loop (ReadAligner::chain_loop, run out of line by
-// chain_entry): the extension's constants, the column that is the sole candidate, and the running values.
+// State handed to / taken back from the extender's chain loop (ReadAligner::chain_loop, run by chain_entry in
+// an aligner of its own): the extension's constants, the column that is the sole candidate, and the running values.
 struct ChainIO {
-    bool active;                 // this lane group takes part (the groups of a warp call together)
     int e, rc, start, wlen, seed_off_m1, sh_offset, seed_seq_len, force_fixed, seed_is_query;
     score_t partial_sum_offset;
     const char *seed_seq; const uint64_t *seed_nodes; uint64_t seed_node0;
@@ -205,9 +204,7 @@ struct ChainIO {
     uint64_t dp_cells; uint32_t dp_columns;
 };
 struct WarpMem; struct WarpSmem;
-#if MGB_DEVICE_CODE && defined(MGB_CHAIN_NOINLINE)
-static __device__ __noinline__
-#elif MGB_DEVICE_CODE
+#if MGB_DEVICE_CODE
 static __device__ __forceinline__
 #else
 static inline
@@ -215,7 +212,7 @@ static inline
 void chain_entry(const IndexView &ix, const DevConfig &cfg, const Caps &caps, const WarpMem &m, const WarpSmem &sm, int L,
                  ChainIO *io);
 
-// Regions of a lane group's arena as BYTE OFFSETS from its base. The layout is the same for every group, so it is
+// Regions of a warp's arena as BYTE OFFSETS from its base. The layout is the same for every warp, so it is
 // computed once on the host and travels in the kernel parameters (constant bank): a region's address is
 // base + constant, no pointer table has to live in registers or on the stack.
 struct WarpLayout {
@@ -227,7 +224,7 @@ struct WarpLayout {
     // seed complexity filter: 3-mer codes / equal-3-mer masks (scratch) and, per strand, the largest start of a
     // low-complexity 3-mer interval ending at or before each 3-mer (see build_lowcx)
     uint64_t lc_word, lc_eq, lc_max[2];
-    uint64_t epoch_store;   // conv-table epochs survive across the reads a group processes
+    uint64_t epoch_store;   // conv-table epochs survive across the reads a warp processes
     uint64_t total;
 
     MGB_HOSTDEV size_t carve(const Caps &c) {
@@ -295,8 +292,8 @@ struct WarpMem {
     MGB_HD uint32_t* epoch_store() const { return (uint32_t*)(base + lay->epoch_store); }
 };
 
-// Per-group on-chip working set (shared memory on the device, a heap block in the host emulation), again as
-// offsets from the group's base: two DP column buffers (parent / child ping-pong), the query strands and their
+// Per-warp on-chip working set (shared memory on the device, a heap block in the host emulation), again as
+// offsets from the warp's base: two DP column buffers (parent / child ping-pong), the query strands and their
 // suffix sums, the best-first queue and the outgoing-edge scratch.
 struct SmemLayout {
     int bmax, lq, hcap;       // column buffer cells; staged query capacity in characters (0: not staged); queue entries
@@ -1907,7 +1904,7 @@ struct ReadAligner {
     // --------------------------------------------------------------------------------
     struct RegCol { score_t S[kCPL], E[kCPL], F[kCPL]; uint8_t fl[kCPL]; };
 
-    // value of cell `idx` of a lane-distributed array, broadcast to the group
+    // value of cell `idx` of a lane-distributed array, broadcast to the warp
     MGB_HD static score_t cell_bcast(const score_t (&v)[kCPL], int idx) {
         score_t x = v[0];
 #if MGB_DEVICE_CODE
@@ -1916,23 +1913,17 @@ struct ReadAligner {
         for (int c = 1; c < kCPL; ++c) if ((idx & (kCPL - 1)) == c) x = v[c];
         return wbcast(x, idx / kCPL);
     }
-    // dst[j] = v[j - j0] for the lane's cells j < limit; on the device dst + j0 is aligned to kCPL cells and
-    // limit is a multiple of 8
+    // dst[j] = v[j - j0] for the lane's cells j < limit
     MGB_HD static void store_cells(score_t *dst, int j0, const score_t (&v)[kCPL], int limit) {
 #if MGB_DEVICE_CODE
-        if (j0 >= limit) return;
-        if constexpr (kCPL == 1) dst[j0] = v[0];
-        else if constexpr (kCPL == 2) *reinterpret_cast<int2*>(dst + j0) = make_int2(v[0], v[1]);
-        else *reinterpret_cast<int4*>(dst + j0) = make_int4(v[0], v[1], v[2], v[3]);
+        if (j0 < limit) dst[j0] = v[0];
 #else
         for (int c = 0; c < kCPL && j0 + c < limit; ++c) dst[j0 + c] = v[c];
 #endif
     }
     MGB_HD static void store_flags(uint8_t *dst, int j0, const uint8_t (&v)[kCPL]) {
 #if MGB_DEVICE_CODE
-        if constexpr (kCPL == 1) dst[j0] = v[0];
-        else if constexpr (kCPL == 2) *reinterpret_cast<uint16_t*>(dst + j0) = (uint16_t)(v[0] | (v[1] << 8));
-        else *reinterpret_cast<uint32_t*>(dst + j0) = v[0] | (v[1] << 8) | (v[2] << 16) | ((uint32_t)v[3] << 24);
+        dst[j0] = v[0];
 #else
         for (int c = 0; c < kCPL; ++c) dst[j0 + c] = v[c];
 #endif
@@ -2034,13 +2025,10 @@ struct ReadAligner {
     // The reference's nested loops (queue rounds -> next_nodes -> outgoing edges) run here as ONE loop whose
     // iteration creates one child column: `t >= n_out` means "take the next parent off the queue".
     // --------------------------------------------------------------------------------
-    // Lock-step over the lane groups of a warp (kWarp < 32): every lane of the warp calls extend() (`act` tells
-    // whether this group has an extension to run) and the column loop runs while ANY group has work, so the
-    // groups execute it together, one child column per iteration each, instead of drifting apart.
-    MGB_HD int extend(int e, int seed_slot, score_t min_path_score, bool force_fixed_seed, int out_base, bool act) {
+    MGB_HD int extend(int e, int seed_slot, score_t min_path_score, bool force_fixed_seed, int out_base) {
         const int s = e;                                 // query strand of this extender
         const AlnSlot seed = m.slot(seed_slot);
-        AlnHdr sh = AlnHdr();
+        const AlnHdr sh = *seed.h;
         bool rc = false;
         const int K = ix.k;
         const score_t xdrop = cfg.xdrop;
@@ -2057,9 +2045,8 @@ struct ReadAligner {
         uint32_t cells_limit = 0;
         score_t min_cell_score = 0, best_score = 0;
         int heap_n = 0, nn_n = 0;
-        bool go = act;
+        bool go = sh.used;                                // nothing to extend from a seed slot that was dropped
         if (go) {
-            sh = *seed.h;
             rc = !MGB_CANONICAL(cfg) && cx[e].rc;        // the RCDBG view is never used on CANONICAL / PRIMARY graphs
             ++cx[e].num_ext;
             min_path_score = imax(0, min_path_score);
@@ -2157,48 +2144,43 @@ struct ReadAligner {
         const score_t *parS = nullptr, *parF = nullptr;
         uint8_t par_fmt = FMT_FULL;
 
-        while (true) {
-            const bool mine = go && !overflow && !finished;
-            if (!wany_full(mine)) break;
+        while (go && !overflow && !finished) {
             // ---------------- chain: the column just committed is the only candidate (:477-504 would push it and
             // pop it again), sits in an on-chip buffer and its band under the current cutoff is known. In a
-            // linear stretch of the graph every column is like that: chain_loop() (out of line, so that its
-            // code is compact and its registers its own) creates such columns one after the other until
-            // something unusual turns up, which it leaves to the general code below.
+            // linear stretch of the graph every column is like that: chain_loop() (run by chain_entry, with the
+            // running values handed over in a ChainIO) creates such columns one after the other until something
+            // unusual turns up, which it leaves to the general code below.
             {
-                const bool chain = mine && reg_path && chain_ok && t >= n_out && heap_n == 0 && nn_n == 1
+                const bool chain = reg_path && chain_ok && t >= n_out && heap_n == 0 && nn_n == 1
                                    && np[0].idx == last_idx && last_band_valid && last_band_cutoff == cutoff
                                    && (res0 == (int)last_idx || res1 == (int)last_idx);
-                if (wany_full(chain)) {
+                if (chain) {
                     ChainIO io;
-                    io.active = chain;
                     io.e = e; io.rc = rc; io.start = start; io.wlen = wlen; io.seed_off_m1 = seed_off_m1;
                     io.sh_offset = (int)sh.offset; io.seed_seq_len = seed_seq_len; io.force_fixed = force_fixed_seed;
                     io.seed_is_query = seed_is_query; io.partial_sum_offset = partial_sum_offset;
                     io.seed_seq = seed_seq; io.seed_nodes = seed.nodes; io.seed_node0 = seed_node0; io.cells_limit = cells_limit;
                     io.ci = last_idx; io.c_node = last_col.node; io.c_offset = last_col.offset; io.c_trim = last_col.trim;
                     io.c_bm = last_band_mask; io.c_pb = res1 == (int)last_idx ? 1 : 0;
-                    io.cur_it = chain ? np[0] : HeapItem();
+                    io.cur_it = np[0];
                     io.cutoff = cutoff; io.best_score = best_score; io.min_cell_score = min_cell_score;
                     io.table_size_bytes = table_size_bytes; io.n_cols = n_cols; io.cells_used = cells_used;
                     io.pf_node = pf_node; io.pf_adj = pf_adj;
                     io.stop = 0; io.overflow = false; io.dp_cells = 0; io.dp_columns = 0;
                     chain_entry(ix, cfg, caps, m, sm, L, &io);
-                    if (chain) {
-                        cutoff = io.cutoff; best_score = io.best_score; min_cell_score = io.min_cell_score;
-                        table_size_bytes = io.table_size_bytes; n_cols = io.n_cols; cells_used = io.cells_used;
-                        pf_node = io.pf_node; pf_adj = io.pf_adj;
-                        stats.dp_cells += io.dp_cells; stats.dp_columns += io.dp_columns;
-                        if (io.overflow) overflow = true;
-                        // the general code finds: an empty queue (stop 1), or column ci as the one entry of
-                        // next_nodes (stop 2); its register copy is re-read from the table, its band re-computed
-                        if (io.stop == 1) nn_n = 0; else { np[0] = io.cur_it; nn_n = 1; }
-                        last_idx = 0xffffffffu; last_band_valid = false;
-                        res0 = io.c_pb == 0 ? (int)io.ci : -1; res1 = io.c_pb == 1 ? (int)io.ci : -1;
-                    }
+                    cutoff = io.cutoff; best_score = io.best_score; min_cell_score = io.min_cell_score;
+                    table_size_bytes = io.table_size_bytes; n_cols = io.n_cols; cells_used = io.cells_used;
+                    pf_node = io.pf_node; pf_adj = io.pf_adj;
+                    stats.dp_cells += io.dp_cells; stats.dp_columns += io.dp_columns;
+                    if (io.overflow) overflow = true;
+                    // the general code finds: an empty queue (stop 1), or column ci as the one entry of
+                    // next_nodes (stop 2); its register copy is re-read from the table, its band re-computed
+                    if (io.stop == 1) nn_n = 0; else { np[0] = io.cur_it; nn_n = 1; }
+                    last_idx = 0xffffffffu; last_band_valid = false;
+                    res0 = io.c_pb == 0 ? (int)io.ci : -1; res1 = io.c_pb == 1 ? (int)io.ci : -1;
                 }
             }
-            if (!mine || overflow) continue;
+            if (overflow) continue;
             if (t >= n_out) {
                 // ---------------- next parent: queue round / next_nodes (:477-504) ----------------
                 if (!nn_n) {
@@ -2539,8 +2521,8 @@ struct ReadAligner {
     }
 
     // The extender's chain loop (see extend()): one child column per iteration of the column that is the sole
-    // candidate, registers only, no queue traffic. It runs out of line (chain_entry), where the kernel parameters
-    // are reached through generic pointers, so everything it reads more than once is copied into locals first.
+    // candidate, registers only, no queue traffic. It runs in an aligner of its own (chain_entry) and takes the
+    // running values from io, where it leaves them again; everything it reads more than once is copied into locals first.
     // Leaves with io.stop = 1 (the extension is over: nothing is left in the queue) or 2 (column io.ci stays the
     // sole candidate and the general code expands it: several children, a column too wide for the register path,
     // a seed node missing from the graph, a convergence-table entry that has to move, ...).
@@ -2577,7 +2559,6 @@ struct ReadAligner {
         const int Lq = L;
         const int j0 = wlane() * kCPL;
 
-        bool chain = io.active;
         uint32_t ci = io.ci; uint64_t c_node = io.c_node;
         int c_offset = io.c_offset, c_trim = io.c_trim, c_pb = io.c_pb;
         uint32_t c_bm = io.c_bm;
@@ -2592,217 +2573,211 @@ struct ReadAligner {
         int stop = 0;
         bool ovf = false;
 
-        while (wany_full(chain)) {
-            if (!chain) continue;
-            do {
-                if (c_maxval < best_score) {
-                    if ((double)ncols / wlen >= cfg.max_nodes_per_seq_char) { stop = 1; break; }      // global_xdrop
-                    if ((double)table_bytes / 1000000 > cfg.max_ram_per_alignment) { stop = 1; break; }
-                }
-                if (!c_bm) { stop = 1; break; }                    // no band: no children
-                const int begin = ffs32(c_bm) - 1 + c_trim;
-                const int prev_end = 32 - clz32(c_bm) + c_trim;
-                const int noff = c_offset + 1;
-                const uint32_t seed_pos = (uint32_t)(noff - sh_offset);
-                const bool in_seed = seed_pos < (uint32_t)seed_seq_len;
-                uint64_t cnode; uint32_t code; uint8_t ch;
-                // call_outgoing (:330-387), a single plain child
-                if (in_seed && (noff < K || force_fixed)) {
-                    cnode = noff < K ? seed_node0 : seed_nodes[noff - K + 1];
-                    if (!cnode) { stop = 2; break; }               // (fixed seed: a node the graph does not have)
-                    ch = (uint8_t)seed_seq[seed_pos];
-                    code = seed_is_q ? qcodes[start + seed_pos] : cfg.code_of[ch];
-                } else if (!rc) {
-                    const uint2 a = c_node == pfn ? pfa : adj[c_node];
-                    const uint32_t all = a.y & 31u, ok = a.x ? ((a.y >> 8) & 30u) : 0u;
-                    if (!ok) { cols[ci].is_tip = 1; stop = 1; break; }
-                    if (ok & (ok - 1u)) { stop = 2; break; }
-                    code = (uint32_t)ffs32(ok) - 1;
-                    cnode = (uint64_t)a.x - popc32(all) + 1 + popc32(all & ((1u << code) - 1u));
-                    ch = (uint8_t)(letters >> (8 * (code - 1)));
-                } else {
-                    // RCDBG::call_outgoing_kmers through the reverse adjacency records, single incoming edge
-                    const uint2 rr = radj[c_node];
-                    if ((rr.y >> 3) & 1u) { stop = 2; break; }     // several incoming edges
-                    const uint64_t edge = rr.x;
-                    uint32_t c = 0;
-                    if (edge != 0 && edge <= n_edges && (!valid || ((valid[edge >> 5] >> (edge & 31)) & 1u)))
-                        c = radj[edge].y & 7u;
-                    if (!c) { cols[ci].is_tip = 1; stop = 1; break; }   // no incoming k-mer, or its first character is '$'
-                    code = sigma - c;                                   // complement
-                    ch = (uint8_t)(letters >> (8 * (code - 1)));
-                    cnode = edge;
-                }
-                if (code < 1 || code > 4) { stop = 2; break; }
-                if (ch >= 'a' && ch <= 'z') ch -= 32;              // toupper (:564)
-                if (ncols >= max_cols) { ovf = true; stop = 1; break; }
-                const int size0 = imin(prev_end, wlen) + 1 - begin;
-                const int n = prev_end - begin;
-                if (n > 28 || size0 > 27) { stop = 2; break; }
-                // requests whose latency overlaps the DP below: the child's adjacency record, its convergence slot
-                if (!rc) { pfn = cnode; pfa = adj[cnode]; }
-                const uint64_t key = cnode + (rc ? n_edges : 0);
-                uint32_t hp = ((uint32_t)key * 0x9E3779B1u) ^ ((uint32_t)(key >> 32) * 0x85EBCA77u);
-                hp = (hp ^ (hp >> 15)) & hash_mask;
-                ConvSlot sl = cslots[hp];
+        while (!stop) {                                    // every exit sets stop
+            if (c_maxval < best_score) {
+                if ((double)ncols / wlen >= cfg.max_nodes_per_seq_char) { stop = 1; break; }      // global_xdrop
+                if ((double)table_bytes / 1000000 > cfg.max_ram_per_alignment) { stop = 1; break; }
+            }
+            if (!c_bm) { stop = 1; break; }                    // no band: no children
+            const int begin = ffs32(c_bm) - 1 + c_trim;
+            const int prev_end = 32 - clz32(c_bm) + c_trim;
+            const int noff = c_offset + 1;
+            const uint32_t seed_pos = (uint32_t)(noff - sh_offset);
+            const bool in_seed = seed_pos < (uint32_t)seed_seq_len;
+            uint64_t cnode; uint32_t code; uint8_t ch;
+            // call_outgoing (:330-387), a single plain child
+            if (in_seed && (noff < K || force_fixed)) {
+                cnode = noff < K ? seed_node0 : seed_nodes[noff - K + 1];
+                if (!cnode) { stop = 2; break; }               // (fixed seed: a node the graph does not have)
+                ch = (uint8_t)seed_seq[seed_pos];
+                code = seed_is_q ? qcodes[start + seed_pos] : cfg.code_of[ch];
+            } else if (!rc) {
+                const uint2 a = c_node == pfn ? pfa : adj[c_node];
+                const uint32_t all = a.y & 31u, ok = a.x ? ((a.y >> 8) & 30u) : 0u;
+                if (!ok) { cols[ci].is_tip = 1; stop = 1; break; }
+                if (ok & (ok - 1u)) { stop = 2; break; }
+                code = (uint32_t)ffs32(ok) - 1;
+                cnode = (uint64_t)a.x - popc32(all) + 1 + popc32(all & ((1u << code) - 1u));
+                ch = (uint8_t)(letters >> (8 * (code - 1)));
+            } else {
+                // RCDBG::call_outgoing_kmers through the reverse adjacency records, single incoming edge
+                const uint2 rr = radj[c_node];
+                if ((rr.y >> 3) & 1u) { stop = 2; break; }     // several incoming edges
+                const uint64_t edge = rr.x;
+                uint32_t c = 0;
+                if (edge != 0 && edge <= n_edges && (!valid || ((valid[edge >> 5] >> (edge & 31)) & 1u)))
+                    c = radj[edge].y & 7u;
+                if (!c) { cols[ci].is_tip = 1; stop = 1; break; }   // no incoming k-mer, or its first character is '$'
+                code = sigma - c;                                   // complement
+                ch = (uint8_t)(letters >> (8 * (code - 1)));
+                cnode = edge;
+            }
+            if (code < 1 || code > 4) { stop = 2; break; }
+            if (ch >= 'a' && ch <= 'z') ch -= 32;              // toupper (:564)
+            if (ncols >= max_cols) { ovf = true; stop = 1; break; }
+            const int size0 = imin(prev_end, wlen) + 1 - begin;
+            const int n = prev_end - begin;
+            if (n > 28 || size0 > 27) { stop = 2; break; }
+            // requests whose latency overlaps the DP below: the child's adjacency record, its convergence slot
+            if (!rc) { pfn = cnode; pfa = adj[cnode]; }
+            const uint64_t key = cnode + (rc ? n_edges : 0);
+            uint32_t hp = ((uint32_t)key * 0x9E3779B1u) ^ ((uint32_t)(key >> 32) * 0x85EBCA77u);
+            hp = (hp ^ (hp >> 15)) & hash_mask;
+            ConvSlot sl = cslots[hp];
 
-                const score_t *pS = buf0 + (size_t)c_pb * 3 * bmax + (begin - c_trim);
-                const int prof_base = start + begin;
-                const int sh = 8 * ((int)code - 1);
-                RegCol r;
-                const int size = reg_column([&](int j) { const int x = prof_base + j;
-                                                         return x <= Lq ? (int)(int8_t)(p4[x] >> sh) : 0; },
-                                            pS, pS + 2 * bmax, n, size0, wlen + 1 - begin, 0, noff > 1, cutoff, go, ge,
-                                            ge_shift, r);
-                if (size < 0) { stop = 2; break; }
-                // per-column scan (:643-669)
-                const int diag_i = noff - seed_off_m1;
-                score_t mn = 0x7fffffff, bs = INT32_MIN;
+            const score_t *pS = buf0 + (size_t)c_pb * 3 * bmax + (begin - c_trim);
+            const int prof_base = start + begin;
+            const int sh = 8 * ((int)code - 1);
+            RegCol r;
+            const int size = reg_column([&](int j) { const int x = prof_base + j;
+                                                     return x <= Lq ? (int)(int8_t)(p4[x] >> sh) : 0; },
+                                        pS, pS + 2 * bmax, n, size0, wlen + 1 - begin, 0, noff > 1, cutoff, go, ge,
+                                        ge_shift, r);
+            if (size < 0) { stop = 2; break; }
+            // per-column scan (:643-669)
+            const int diag_i = noff - seed_off_m1;
+            score_t mn = 0x7fffffff, bs = INT32_MIN;
 #if MGB_DEVICE_CODE
 #pragma unroll
 #endif
-                for (int c = 0; c < kCPL; ++c) {
-                    const bool cell = j0 + c < size;
-                    const score_t v = r.S[c];
-                    if (cell && v != kNinf) mn = imin(mn, v);
-                    if (cell) bs = imax(bs, v);
+            for (int c = 0; c < kCPL; ++c) {
+                const bool cell = j0 + c < size;
+                const score_t v = r.S[c];
+                if (cell && v != kNinf) mn = imin(mn, v);
+                if (cell) bs = imax(bs, v);
+            }
+            const score_t col_min = wreduce_min(mn);
+            const score_t max_val = wreduce_max(bs);
+            int bkey = 0x7fffffff; bool he = false;            // (distance to the diagonal, row) of the best cell
+            score_t ext_cut = 0;
+            if (!in_seed) ext_cut = (score_t)((double)best_score * rsc + pso);
+#if MGB_DEVICE_CODE
+#pragma unroll
+#endif
+            for (int c = 0; c < kCPL; ++c) {
+                const int j = j0 + c;
+                const bool cell = j < size;
+                if (cell && r.S[c] == max_val) bkey = imin(bkey, (iabs(j + begin - diag_i) << 5) | j);
+                if (!in_seed && cell && r.S[c] + ps[start + begin + j] >= ext_cut) he = true;
+            }
+            const int max_pos = (wreduce_min(bkey) & 31) + begin;
+            // ---- convergence filter, first half (update_seed_filter, :100-156): find the node's entry. Cases
+            // that move data around are left to the general code before anything has been written
+            const int s_first = begin ? 0 : 1;
+            const int qstart = start + begin - (begin ? 1 : 0);
+            const int n_pass = size - s_first;
+            bool hit = false;
+            {
+                uint32_t probes = 0;
+                while (sl.epoch == epoch && sl.key != key && probes < hash_size) { hp = (hp + 1) & hash_mask; sl = cslots[hp]; ++probes; }
+                hit = sl.epoch == epoch && sl.key == key;
+            }
+            int new_end = 0;
+            if (!hit) {
+                const int seg_start = imax(0, qstart - 8);
+                const int seg_cap = imin(Lq + 1, qstart + n_pass + 8) - seg_start;
+                if (conv_n >= max_conv_entries || 2 * (conv_n + 1) > hash_size || conv_used + seg_cap > max_conv_cells) {
+                    stop = 2; break;                           // (the general code reports the overflow)
                 }
-                const score_t col_min = wreduce_min(mn);
-                const score_t max_val = wreduce_max(bs);
-                int bkey = 0x7fffffff; bool he = false;            // (distance to the diagonal, row) of the best cell
-                score_t ext_cut = 0;
-                if (!in_seed) ext_cut = (score_t)((double)best_score * rsc + pso);
+                sl.key = key; sl.epoch = epoch; sl.start = qstart; sl.size = n_pass;
+                sl.seg_start = seg_start; sl.seg_cap = seg_cap; sl.seg_off = conv_used;
+            } else {
+                // the node was met before (seed columns share the seed's node): only the in-place cases -- the
+                // passed range overlaps the stored one and ends at or after its end, inside the segment
+                new_end = imax(qstart + n_pass, sl.start + sl.size);
+                if (qstart < sl.start || qstart >= sl.start + sl.size || new_end > sl.seg_start + sl.seg_cap) {
+                    stop = 2; break;
+                }
+            }
+
+            const uint32_t cap_before = t_cap;
+            if (ncols + 1 > t_cap) t_cap = t_cap ? 2 * t_cap : 1;
+            made_cells += size; ++made;
+            min_cell_score = imin(min_cell_score, col_min);
+            if (!in_seed && (max_val < cutoff || !wballot(he))) { stop = 1; break; }   // pop(table.size() - 1)
+
+            table_bytes += 136ull * (t_cap - cap_before) + 3ull * vec_capacity(size0, size) * 4;
+            if ((int64_t)max_val - cutoff > xdrop) cutoff = max_val - xdrop;
+            best_score = imax(best_score, max_val);
+            if (cused > cells_limit) { ovf = true; stop = 1; break; }
+            // ---- commit: DP table (compact format, whole 32-byte sectors) and the on-chip child buffer
+            const int capr = capr_of(size);
+            const uint32_t off = (cused + 7u) & ~7u;
+            cused = off + 2 * capr + 8;
+            score_t *dst = cells + off;
+            score_t *cb_S = buf0 + (size_t)(1 - c_pb) * 3 * bmax;
+            store_cells(dst, j0, r.S, capr);
+            store_flags(reinterpret_cast<uint8_t*>(dst + capr), j0, r.fl);
+            store_cells(cb_S, j0, r.S, 32); store_cells(cb_S + 2 * bmax, j0, r.F, 32);
+            ColMeta col;
+            col.node = cnode; col.parent = ci; col.c = ch;
+            col.offset = noff; col.max_pos = max_pos; col.trim = begin; col.score = 0;
+            col.is_tip = 0; col.started = 0; col.fmt = FMT_COMPACT; col.pad0 = col.pad1 = 0;
+            col.size = size; col.cells_off = off;
+            const uint32_t idx = ncols;
+            cols[ncols++] = col;
+            uint32_t bits = 0;
+#if MGB_DEVICE_CODE
+#pragma unroll
+#endif
+            for (int c = 0; c < kCPL; ++c) if (j0 + c < size && r.S[c] >= cutoff) bits |= 1u << c;
+            const uint32_t bm_new = kCPL == 32 ? bits : wreduce_or(bits << (j0 & 31));
+
+            // ---- convergence filter, second half
+            score_t converged;
+            score_t *c0 = ccells + sl.seg_off + (qstart - s_first - sl.seg_start);              // indexed by cell
+            if (!hit) {
+                conv_used += sl.seg_cap; ++conv_n;
+                cslots[hp] = sl;
+                score_t mx = kNinf;
 #if MGB_DEVICE_CODE
 #pragma unroll
 #endif
                 for (int c = 0; c < kCPL; ++c) {
                     const int j = j0 + c;
-                    const bool cell = j < size;
-                    if (cell && r.S[c] == max_val) bkey = imin(bkey, (iabs(j + begin - diag_i) << 5) | j);
-                    if (!in_seed && cell && r.S[c] + ps[start + begin + j] >= ext_cut) he = true;
+                    if (j >= s_first && j < size) { c0[j] = r.S[c]; mx = imax(mx, r.S[c]); }
                 }
-                const int max_pos = (wreduce_min(bkey) & 31) + begin;
-                // ---- convergence filter, first half (update_seed_filter, :100-156): find the node's entry. Cases
-                // that move data around are left to the general code before anything has been written
-                const int s_first = begin ? 0 : 1;
-                const int qstart = start + begin - (begin ? 1 : 0);
-                const int n_pass = size - s_first;
-                bool hit = false;
-                {
-                    uint32_t probes = 0;
-                    while (sl.epoch == epoch && sl.key != key && probes < hash_size) { hp = (hp + 1) & hash_mask; sl = cslots[hp]; ++probes; }
-                    hit = sl.epoch == epoch && sl.key == key;
-                }
-                int new_end = 0;
-                if (!hit) {
-                    const int seg_start = imax(0, qstart - 8);
-                    const int seg_cap = imin(Lq + 1, qstart + n_pass + 8) - seg_start;
-                    if (conv_n >= max_conv_entries || 2 * (conv_n + 1) > hash_size || conv_used + seg_cap > max_conv_cells) {
-                        stop = 2; break;                           // (the general code reports the overflow)
-                    }
-                    sl.key = key; sl.epoch = epoch; sl.start = qstart; sl.size = n_pass;
-                    sl.seg_start = seg_start; sl.seg_cap = seg_cap; sl.seg_off = conv_used;
-                } else {
-                    // the node was met before (seed columns share the seed's node): only the in-place cases -- the
-                    // passed range overlaps the stored one and ends at or after its end, inside the segment
-                    new_end = imax(qstart + n_pass, sl.start + sl.size);
-                    if (qstart < sl.start || qstart >= sl.start + sl.size || new_end > sl.seg_start + sl.seg_cap) {
-                        stop = 2; break;
-                    }
-                }
-
-                const uint32_t cap_before = t_cap;
-                if (ncols + 1 > t_cap) t_cap = t_cap ? 2 * t_cap : 1;
-                made_cells += size; ++made;
-                min_cell_score = imin(min_cell_score, col_min);
-                if (!in_seed && (max_val < cutoff || !wballot(he))) { stop = 1; break; }   // pop(table.size() - 1)
-
-                table_bytes += 136ull * (t_cap - cap_before) + 3ull * vec_capacity(size0, size) * 4;
-                if ((int64_t)max_val - cutoff > xdrop) cutoff = max_val - xdrop;
-                best_score = imax(best_score, max_val);
-                if (cused > cells_limit) { ovf = true; stop = 1; break; }
-                // ---- commit: DP table (compact format, whole 32-byte sectors) and the on-chip child buffer
-                const int capr = capr_of(size);
-                const uint32_t off = (cused + 7u) & ~7u;
-                cused = off + 2 * capr + 8;
-                score_t *dst = cells + off;
-                score_t *cb_S = buf0 + (size_t)(1 - c_pb) * 3 * bmax;
-                store_cells(dst, j0, r.S, capr);
-                store_flags(reinterpret_cast<uint8_t*>(dst + capr), j0, r.fl);
-                store_cells(cb_S, j0, r.S, 32); store_cells(cb_S + 2 * bmax, j0, r.F, 32);
-                ColMeta col;
-                col.node = cnode; col.parent = ci; col.c = ch;
-                col.offset = noff; col.max_pos = max_pos; col.trim = begin; col.score = 0;
-                col.is_tip = 0; col.started = 0; col.fmt = FMT_COMPACT; col.pad0 = col.pad1 = 0;
-                col.size = size; col.cells_off = off;
-                const uint32_t idx = ncols;
-                cols[ncols++] = col;
-                uint32_t bits = 0;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-                for (int c = 0; c < kCPL; ++c) if (j0 + c < size && r.S[c] >= cutoff) bits |= 1u << c;
-                const uint32_t bm_new = kCPL == 32 ? bits : wreduce_or(bits << (j0 & 31));
-
-                // ---- convergence filter, second half
-                score_t converged;
-                score_t *c0 = ccells + sl.seg_off + (qstart - s_first - sl.seg_start);              // indexed by cell
-                if (!hit) {
-                    conv_used += sl.seg_cap; ++conv_n;
+                converged = wreduce_max(mx);
+            } else {
+                const int old_end = sl.start + sl.size;
+                if (new_end > old_end) {                       // vec.resize(n, ninf)
+                    score_t *cseg = ccells + sl.seg_off;
+                    for (int p = old_end + wlane(); p < new_end; p += kWarp) cseg[p - sl.seg_start] = kNinf;
+                    sl.size = new_end - sl.start;
                     cslots[hp] = sl;
-                    score_t mx = kNinf;
+                    wsync();
+                }
+                score_t max_changed = kNinf;
 #if MGB_DEVICE_CODE
 #pragma unroll
 #endif
-                    for (int c = 0; c < kCPL; ++c) {
-                        const int j = j0 + c;
-                        if (j >= s_first && j < size) { c0[j] = r.S[c]; mx = imax(mx, r.S[c]); }
-                    }
-                    converged = wreduce_max(mx);
-                } else {
-                    const int old_end = sl.start + sl.size;
-                    if (new_end > old_end) {                       // vec.resize(n, ninf)
-                        score_t *cseg = ccells + sl.seg_off;
-                        for (int p = old_end + wlane(); p < new_end; p += kWarp) cseg[p - sl.seg_start] = kNinf;
-                        sl.size = new_end - sl.start;
-                        cslots[hp] = sl;
-                        wsync();
-                    }
-                    score_t max_changed = kNinf;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-                    for (int c = 0; c < kCPL; ++c) {
-                        const int j = j0 + c;
-                        if (j >= s_first && j < size) {
-                            score_t vj = c0[j];
-                            if ((double)r.S[c] > (double)vj * rsc) {
-                                vj = imax(vj, r.S[c]);
-                                c0[j] = vj;
-                                max_changed = imax(max_changed, vj);
-                            }
+                for (int c = 0; c < kCPL; ++c) {
+                    const int j = j0 + c;
+                    if (j >= s_first && j < size) {
+                        score_t vj = c0[j];
+                        if ((double)r.S[c] > (double)vj * rsc) {
+                            vj = imax(vj, r.S[c]);
+                            c0[j] = vj;
+                            max_changed = imax(max_changed, vj);
                         }
                     }
-                    converged = wreduce_max(max_changed);
                 }
-                wsync();
-                // the new column becomes the parent
-                ci = idx; c_node = cnode; c_offset = noff; c_trim = begin; c_bm = bm_new; c_pb = 1 - c_pb;
-                c_maxval = max_val;
-                cur_it.score = converged; cur_it.neg_off_diag = -iabs(max_pos - diag_i); cur_it.idx = idx;
-                cur_it.max_score = max_val;
-                if (converged == kNinf) { stop = 1; break; }
-            } while (false);
-            if (stop) chain = false;
+                converged = wreduce_max(max_changed);
+            }
+            wsync();
+            // the new column becomes the parent
+            ci = idx; c_node = cnode; c_offset = noff; c_trim = begin; c_bm = bm_new; c_pb = 1 - c_pb;
+            c_maxval = max_val;
+            cur_it.score = converged; cur_it.neg_off_diag = -iabs(max_pos - diag_i); cur_it.idx = idx;
+            cur_it.max_score = max_val;
+            if (converged == kNinf) { stop = 1; break; }
         }
-        if (io.active) {
-            tc.table_cap = t_cap; tc.conv_n = conv_n; tc.conv_cells_used = conv_used;
-            io.ci = ci; io.c_pb = c_pb; io.cur_it = cur_it;
-            io.cutoff = cutoff; io.best_score = best_score; io.min_cell_score = min_cell_score;
-            io.table_size_bytes = table_bytes; io.n_cols = ncols; io.cells_used = cused;
-            io.pf_node = pfn; io.pf_adj = pfa;
-            io.stop = stop; io.overflow = ovf; io.dp_cells = made_cells; io.dp_columns = made;
-        }
+        tc.table_cap = t_cap; tc.conv_n = conv_n; tc.conv_cells_used = conv_used;
+        io.ci = ci; io.c_pb = c_pb; io.cur_it = cur_it;
+        io.cutoff = cutoff; io.best_score = best_score; io.min_cell_score = min_cell_score;
+        io.table_size_bytes = table_bytes; io.n_cols = ncols; io.cells_used = cused;
+        io.pf_node = pfn; io.pf_adj = pfa;
+        io.stop = stop; io.overflow = ovf; io.dp_cells = made_cells; io.dp_columns = made;
     }
 
     long long phase_cycles[8] = {0,0,0,0,0,0,0,0};   // MGB_PHASE_TIMERS: setup, seeds, fwd loop, backtrack, rest
@@ -3178,64 +3153,48 @@ struct ReadAligner {
     // Seeds of query strand s, in order (dbg_aligner.cpp:360-384 align_core when `both` is false,
     // :657-736 aln_both otherwise: forward extension, then backward extension of left-clipped
     // results through the reverse-complement graph view).
-    // Lock-step over the lane groups of a warp: the loops below that end in the extender run while ANY group of
-    // the warp has work (wany_full) and `act` / `seed_ok` / `ext_ok` say whether THIS group takes part, so that
-    // all lanes of the warp enter the extender's column loop together (see extend()).
-    MGB_HD void align_strand(int s, bool both, bool act) {
+    MGB_HD void align_strand(int s, bool both) {
         const int fe = s, be = 1 - s;
-        int n_seeds_s = 0; SeedRec *seeds_s = nullptr; bool implicit = false;
         const int nk = L >= (int)ix.k ? L - (int)ix.k + 1 : 0;
-        int i = 0;
-        if (act) {
-            cx[fe].rc = 0;
-            if (both) cx[be].rc = MGB_CANONICAL(cfg) ? 0 : 1;     // use_rcdbg (dbg_aligner.cpp:646-650)
-            n_seeds_s = cx[s].n_seeds;
-            seeds_s = cx[s].seeds;
-            implicit = cx[s].implicit_seeds != 0;
-            stats.num_seeds += n_seeds_s;
-            if (!n_seeds_s) act = false;
-            else if (implicit) i = mask_next(cx[s].mask, nk, 0, true);
-        }
+        cx[fe].rc = 0;
+        if (both) cx[be].rc = MGB_CANONICAL(cfg) ? 0 : 1;     // use_rcdbg (dbg_aligner.cpp:646-650)
+        const int n_seeds_s = cx[s].n_seeds;
+        SeedRec *seeds_s = cx[s].seeds;
+        const bool implicit = cx[s].implicit_seeds != 0;
+        stats.num_seeds += n_seeds_s;
+        if (!n_seeds_s) return;
+        int i = implicit ? mask_next(cx[s].mask, nk, 0, true) : 0;
         while (true) {
-            // next live seed of this group (dead ones are skipped here so that a group never idles on them)
-            if (act && !implicit) while (i < n_seeds_s && !seeds_s[i].alive) ++i;
-            const bool seed_ok = act && !overflow && (implicit ? i < nk : i < n_seeds_s);
-            if (!wany_full(seed_ok)) break;
-            score_t mps_fwd = 0;
-            if (seed_ok) {
-                SeedRec sd;
-                if (implicit) {
-                    sd.clip = i; sd.len = ix.k; sd.offset = 0; sd.n_nodes = 1; sd.node0 = cx[s].qnodes[i];
-                    sd.alive = 1; sd.pad = 0;
-                } else {
-                    sd = seeds_s[i];
-                }
-                seed_to_slot(SLOT_SEED, s, sd);
-                seed_is_query = true;
-                mps_fwd = both ? cfg.min_cell_score : get_min_path_score();
+            // next live seed
+            if (!implicit) while (i < n_seeds_s && !seeds_s[i].alive) ++i;
+            if (overflow || (implicit ? i >= nk : i >= n_seeds_s)) break;
+            SeedRec sd;
+            if (implicit) {
+                sd.clip = i; sd.len = ix.k; sd.offset = 0; sd.n_nodes = 1; sd.node0 = cx[s].qnodes[i];
+                sd.alive = 1; sd.pad = 0;
+            } else {
+                sd = seeds_s[i];
             }
+            seed_to_slot(SLOT_SEED, s, sd);
+            seed_is_query = true;
+            const score_t mps_fwd = both ? cfg.min_cell_score : get_min_path_score();
             // One call site for both kinds of extension (the forward one, then the backward ones it
             // spawns): the extender is by far the largest piece of code and must exist once.
-            int n_rc = 0, it = 0;
-            while (true) {
-                const bool it_ok = seed_ok && !overflow && it <= n_rc;
-                if (!wany_full(it_ok)) break;
-                bool ext_ok = it_ok;
-                if (ext_ok) {
-                    if (it == 0) {
-                        set_seed(fe);
-                    } else if (!m.slot(SLOT_EXT + it - 1).h->used) {
-                        ext_ok = false;
-                    } else {
-                        // align_core(ManualSeeder(rc_of_alignments), bwd_extender, ..., force_fixed_seed = true)
-                        set_seed(be);
-                        seed_is_query = false;
-                    }
-                }
+            // A backward seed dropped by an earlier backward extension stays in its slot, unused: extend() does
+            // nothing for it.
+            int n_rc = 0;
+            for (int it = 0; !overflow && it <= n_rc; ++it) {
                 const int r = it - 1;
+                const bool ext_ok = it == 0 || m.slot(SLOT_EXT + r).h->used;
+                if (it == 0) {
+                    set_seed(fe);
+                } else if (ext_ok) {
+                    // align_core(ManualSeeder(rc_of_alignments), bwd_extender, ..., force_fixed_seed = true)
+                    set_seed(be);
+                    seed_is_query = false;
+                }
                 const int n_ext = extend(it ? be : fe, it ? SLOT_EXT + r : SLOT_SEED,
-                                         (ext_ok && it) ? get_min_path_score() : mps_fwd, it != 0, it ? SLOT_BWD : SLOT_EXT,
-                                         ext_ok);
+                                         (ext_ok && it) ? get_min_path_score() : mps_fwd, it != 0, it ? SLOT_BWD : SLOT_EXT);
                 // results of this extension: one loop (and one agg_add site: the aggregator's comparison
                 // code is large) for the forward case (aggregate, then reverse-complement the clipped
                 // ones for the backward pass) and the backward case (reverse-complement back, then aggregate)
@@ -3292,9 +3251,8 @@ struct ReadAligner {
                             a.h->used = 0;
                     }
                 }
-                if (it_ok) ++it;
             }
-            if (seed_ok && !overflow && shortcut_hit) {
+            if (!overflow && shortcut_hit) {
                 // exact-path shortcut: the extension it replaces covers every later seed of the strand (their last
                 // node and position lie on the matched path with at least the seed's score, DESIGN.md)
                 wsync();
@@ -3309,7 +3267,7 @@ struct ReadAligner {
                 }
                 shortcut_hit = false;
                 wsync();
-            } else if (seed_ok && !overflow) {
+            } else if (!overflow) {
                 // later seeds already covered by this extension are dropped (:731-734, :379-382);
                 // independent probes, one seed per lane
                 wsync();
@@ -3344,7 +3302,7 @@ struct ReadAligner {
                 }
                 wsync();
             }
-            if (seed_ok) i = implicit ? mask_next(cx[s].mask, nk, i + 1, true) : i + 1;
+            i = implicit ? mask_next(cx[s].mask, nk, i + 1, true) : i + 1;
         }
     }
 
@@ -3385,15 +3343,12 @@ struct ReadAligner {
     // optional: per-position index_range results of both strands (k_subk), set before run()
     const uint32_t *subk_first[2] = { nullptr, nullptr }, *subk_last[2] = { nullptr, nullptr };
     const uint8_t *subk_len[2] = { nullptr, nullptr };
-    // `act`: this lane group has a read (the groups of a warp call run() together, see align_strand / extend)
-    MGB_HD int run(bool act, int L_, const char *qf, const char *qr, const uint8_t *cf, const uint8_t *cr,
+    MGB_HD int run(int L_, const char *qf, const char *qr, const uint8_t *cf, const uint8_t *cr,
                    const uint64_t *nf, const uint64_t *nr, int *order) {
         MGB_TIC(t_setup);
         L = L_;
         overflow = false; n_agg = 0; seed_is_query = false;
         const bool both = cfg.forward_and_reverse_complement;
-        int first = 0, n_pass = 0;
-        if (act) {
         wsync();
         // per-strand context + alignment slot table (shared memory; constant indices only here)
         {
@@ -3448,7 +3403,7 @@ struct ReadAligner {
             if (overflow) break;
             if ((double)L * cfg.min_exact_match > (double)cx[s].num_matching) { cx[s].n_seeds = 0; cx[s].num_matching = 0; }
         }
-        n_pass = 1;
+        int first = 0, n_pass = 1;
         if (both) {
             // the strand with more exact-match bases first; the other only if it is close (:738-755)
             uint32_t fm = cx[0].num_matching, bm = cx[1].num_matching;
@@ -3456,16 +3411,12 @@ struct ReadAligner {
             uint32_t hi = first ? bm : fm, lo = first ? fm : bm;
             n_pass = (double)lo >= (double)hi * cfg.rel_score_cutoff ? 2 : 1;
         }
-        }   // act
         MGB_TOC(t_seeds, 1);
         MGB_TIC(t_align);
-        for (int pass = 0; ; ++pass) {
-            const bool p_ok = act && !overflow && pass < n_pass;
-            if (!wany_full(p_ok)) break;
-            align_strand(pass ? 1 - first : first, both, p_ok);
-        }
+        for (int pass = 0; !overflow && pass < n_pass; ++pass)
+            align_strand(pass ? 1 - first : first, both);
         MGB_TOC(t_align, 4);
-        if (!act || overflow) return 0;
+        if (overflow) return 0;
         stats.num_extensions += cx[0].num_ext + cx[1].num_ext;
         stats.num_explored_nodes += cx[0].explored_prev + cx[0].conv_n + cx[1].explored_prev + cx[1].conv_n;
         // AlignmentAggregator::get_alignments: descending LocalAlignmentLess order
@@ -3481,9 +3432,7 @@ struct ReadAligner {
     }
 };
 
-#if MGB_DEVICE_CODE && defined(MGB_CHAIN_NOINLINE)
-static __device__ __noinline__
-#elif MGB_DEVICE_CODE
+#if MGB_DEVICE_CODE
 static __device__ __forceinline__
 #else
 static inline

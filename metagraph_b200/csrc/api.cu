@@ -1050,7 +1050,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             if (pass == 6) { rc = fail(MGB_ERR_OVERFLOW, "a read exceeded the largest per-read work arena"); break; }
             Caps caps = choose_caps(b.L_max, dcfg, index->view.k, scale);
             size_t stride = arena_bytes(caps);
-            // on-chip working set per lane group: the column buffers hold the widest column the x-drop band
+            // on-chip working set per warp: the column buffers hold the widest column the x-drop band
             // allows (choose_caps' estimate; at least 64 cells, the register path of the extender needs 40) of
             // reads up to 248 bp; wider columns spill to the arena scratch
             uint64_t band_est = (uint64_t)b.L_max + 9;
@@ -1071,7 +1071,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             uint32_t n_warps = 1;
 #else
             int blocks_per_sm = 0;
-            const size_t smem_block = smem_per_warp * kern_dna::kGroupsPerBlock;
+            const size_t smem_block = smem_per_warp * kern_dna::kWarpsPerBlock;
             {
                 // driver queries serialise against running work: ask once per shared-memory size
                 static std::mutex occ_mu;
@@ -1091,19 +1091,19 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
                 } else blocks_per_sm = it->second;
             }
             if (blocks_per_sm < 1) blocks_per_sm = 1;
-            const uint64_t gpb = kern_dna::kGroupsPerBlock;       // lane groups (reads in flight) per block
-            uint64_t n_warps64 = (uint64_t)index->num_sms * blocks_per_sm * gpb;
+            const uint64_t wpb = kern_dna::kWarpsPerBlock;        // warps (reads in flight) per block
+            uint64_t n_warps64 = (uint64_t)index->num_sms * blocks_per_sm * wpb;
             if (stride * n_warps64 > pass_bufs.capacity_of_next()) {
                 size_t free_b = 0, total_b = 0;
                 cudaMemGetInfo(&free_b, &total_b);
                 uint64_t mem_warps = (uint64_t)(free_b * 0.6 + pass_bufs.capacity_of_next()) / (stride ? stride : 1);
-                if (mem_warps < gpb) mem_warps = gpb;
-                if (n_warps64 > mem_warps) n_warps64 = mem_warps / gpb * gpb;
+                if (mem_warps < wpb) mem_warps = wpb;
+                if (n_warps64 > mem_warps) n_warps64 = mem_warps / wpb * wpb;
             }
-            if (n_warps64 > ((uint64_t)list.size() + gpb - 1) / gpb * gpb) n_warps64 = ((uint64_t)list.size() + gpb - 1) / gpb * gpb;
+            if (n_warps64 > ((uint64_t)list.size() + wpb - 1) / wpb * wpb) n_warps64 = ((uint64_t)list.size() + wpb - 1) / wpb * wpb;
             uint32_t n_warps = (uint32_t)n_warps64;
-            if (dbg_time) std::fprintf(stderr, "[mgb] k_align grid: %u lane groups (%llu resident)\n", n_warps,
-                                       (unsigned long long)index->num_sms * blocks_per_sm * gpb);
+            if (dbg_time) std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident)\n", n_warps,
+                                       (unsigned long long)index->num_sms * blocks_per_sm * wpb);
 #endif
             // output heap: generous first guess, doubled on retry passes
             uint64_t per_read = sizeof(OutAln) + 9ull * (b.L_max + 64 + index->view.k) + 4ull * 64;
@@ -1175,11 +1175,11 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             std::vector<char> smem_emu(smem_per_warp + 64);
             const WarpMem mem_emu { d_arena, &a.lay };
             const WarpSmem sm_emu { smem_emu.data(), &a.slay };
-            for (uint32_t t = 0; t < a.n_list; ++t) align_read(a, a.read_list[t], mem_emu, sm_emu, true);
+            for (uint32_t t = 0; t < a.n_list; ++t) align_read(a, a.read_list[t], mem_emu, sm_emu);
             used = *d_used;
 #else
             if (a.n_list) {
-                const uint32_t grid = (uint32_t)(std::min<uint64_t>(n_warps, ((uint64_t)a.n_list + gpb - 1) / gpb * gpb) / gpb);
+                const uint32_t grid = (uint32_t)(std::min<uint64_t>(n_warps, ((uint64_t)a.n_list + wpb - 1) / wpb * wpb) / wpb);
                 CUDA_TRY(index->view.wide ? kern_any::launch_align(grid, smem_block, st.s, a)
                        : index->view.mode != 0 ? kern_canon::launch_align(grid, smem_block, st.s, a)
                                                : kern_dna::launch_align(grid, smem_block, st.s, a));

@@ -30,20 +30,14 @@ namespace mgb {
 typedef int32_t score_t;
 static constexpr score_t kNinf = INT32_MIN + 100;   // aligner_config.hpp:31
 
-// A read is aligned by a GROUP of kWarp consecutive lanes (MGB_GROUP_WIDTH = 32, 16 or 8; one warp holds
-// 32 / kWarp groups that work on different reads and may diverge from each other: every collective
-// names its group's lanes only). "Scalar" values are uniform within a group. kCPL = 32 / kWarp is the
-// number of DP cells a lane owns in the register path of the extender (a column of up to 32 cells).
-#ifndef MGB_GROUP_WIDTH
-#define MGB_GROUP_WIDTH 32
-#endif
+// A read is aligned by one warp of kWarp lanes; "scalar" values are uniform within the warp. The host
+// emulation is a one-lane warp. kCPL is the number of DP cells a lane owns in the register path of the
+// extender (a column of up to 32 cells): 1 on the device, 32 in the emulation.
 #if MGB_DEVICE_CODE
-static constexpr int kWarp = MGB_GROUP_WIDTH;
-static_assert(kWarp == 32 || kWarp == 16 || kWarp == 8, "MGB_GROUP_WIDTH must be 32, 16 or 8");
-static constexpr int kCPL = 32 / kWarp;
+static constexpr int kWarp = 32;
+static constexpr int kCPL = 1;
 MGB_D int wlane() { return threadIdx.x & (kWarp - 1); }
-MGB_D unsigned wshift() { return kWarp == 32 ? 0u : (threadIdx.x & 31u & ~(unsigned)(kWarp - 1)); }
-MGB_D unsigned wmask() { return kWarp == 32 ? 0xffffffffu : (((1u << (kWarp & 31)) - 1u) << wshift()); }
+MGB_D unsigned wmask() { return 0xffffffffu; }
 MGB_D void wsync() { __syncwarp(wmask()); }
 template <class T> MGB_D T wbcast(T v, int src) { return __shfl_sync(wmask(), v, src, kWarp); }
 MGB_D uint64_t wbcast64(uint64_t v, int src) {
@@ -55,11 +49,8 @@ MGB_D int wreduce_max(int v) { return __reduce_max_sync(wmask(), v); }
 MGB_D int wreduce_min(int v) { return __reduce_min_sync(wmask(), v); }
 MGB_D int wreduce_add(int v) { return __reduce_add_sync(wmask(), v); }
 MGB_D unsigned wreduce_or(unsigned v) { return __reduce_or_sync(wmask(), v); }
-MGB_D unsigned wballot(bool p) {
-    const unsigned b = __ballot_sync(wmask(), p);
-    return kWarp == 32 ? b : ((b >> wshift()) & ((1u << (kWarp & 31)) - 1u));
-}
-// inclusive prefix max over the lanes of the group
+MGB_D unsigned wballot(bool p) { return __ballot_sync(wmask(), p); }
+// inclusive prefix max over the lanes of the warp
 MGB_D int wscan_max(int v) {
 #pragma unroll
     for (int d = 1; d < kWarp; d <<= 1) {
@@ -68,7 +59,7 @@ MGB_D int wscan_max(int v) {
     }
     return v;
 }
-// inclusive prefix sum over the lanes of the group
+// inclusive prefix sum over the lanes of the warp
 MGB_D int wscan_add(int v) {
 #pragma unroll
     for (int d = 1; d < kWarp; d <<= 1) {
@@ -81,9 +72,6 @@ MGB_D int wshfl_up1(int v, int fill) {
     int o = __shfl_up_sync(wmask(), v, 1, kWarp);
     return wlane() == 0 ? fill : o;
 }
-// true if `p` holds for any lane group of the warp (p is uniform within a group). The loops around the
-// extender's column loop run in lock-step over the groups of a warp: every lane of the warp must call this.
-MGB_D bool wany_full(bool p) { return kWarp == 32 ? p : (__any_sync(0xffffffffu, p) != 0); }
 MGB_D int popc32(uint32_t x) { return __popc(x); }
 MGB_D int ffs32(uint32_t x) { return __ffs(x); }            // 1-based, 0 if none
 MGB_D int clz32(uint32_t x) { return __clz(x); }
@@ -106,7 +94,6 @@ inline int wreduce_min(int v) { return v; }
 inline int wreduce_add(int v) { return v; }
 inline unsigned wreduce_or(unsigned v) { return v; }
 inline int wscan_add(int v) { return v; }
-inline bool wany_full(bool p) { return p; }
 inline unsigned wballot(bool p) { return p ? 1u : 0u; }
 inline int wscan_max(int v) { return v; }
 inline int wshfl_up1(int, int fill) { return fill; }

@@ -126,8 +126,8 @@ MGB_HD void subk_item(const SubkArgs &a, uint32_t r, uint32_t s, uint32_t chunk)
 
 struct AlignArgs {
     IndexView ix; DevConfig cfg; Caps caps;
-    WarpLayout lay;             // arena regions of a lane group (offsets)
-    SmemLayout slay;            // on-chip working set of a lane group (offsets)
+    WarpLayout lay;             // arena regions of a warp (offsets)
+    SmemLayout slay;            // on-chip working set of a warp (offsets)
     int use_fast;               // 0 disables the register fast path (test knob)
     unsigned long long *phase_out;   // MGB_PHASE_TIMERS builds: cycles per phase (setup, seeds, fwd, backtrack, align total)
     const char *qf, *qr; const uint8_t *cf, *cr; const uint64_t *offsets, *koff;
@@ -140,24 +140,22 @@ struct AlignArgs {
     unsigned int *next;
 };
 
-// `act`: this lane group has a read; a group without one still walks through the lock-step loops of the
-// aligner (the lane groups of a warp run them together)
-MGB_HD void align_read(const AlignArgs &a, uint32_t r, const WarpMem &mem, const WarpSmem &sm, bool act) {
+// aligns read r with the warp's arena and on-chip working set and writes its record and alignments
+MGB_HD void align_read(const AlignArgs &a, uint32_t r, const WarpMem &mem, const WarpSmem &sm) {
     ReadAligner al(a.ix, a.cfg, a.caps, mem, sm);
     al.use_fast = a.use_fast != 0;
-    const uint64_t b = act ? a.offsets[r] : 0;
-    const int L = act ? (int)(a.offsets[r + 1] - b) : 0;
+    const uint64_t b = a.offsets[r];
+    const int L = (int)(a.offsets[r + 1] - b);
     int order[kMaxAlt];
     const bool has_k = L >= (int)a.ix.k;
     if (a.sub_len_f) {
         al.subk_first[0] = a.sub_first_f + b; al.subk_last[0] = a.sub_last_f + b; al.subk_len[0] = a.sub_len_f + b;
         if (a.sub_len_r) { al.subk_first[1] = a.sub_first_r + b; al.subk_last[1] = a.sub_last_r + b; al.subk_len[1] = a.sub_len_r + b; }
     }
-    const uint64_t ko = (act && has_k) ? a.koff[r] : 0;
-    int n = al.run(act, L, a.qf + b, a.qr + b, a.cf + b, a.cr + b,
+    const uint64_t ko = has_k ? a.koff[r] : 0;
+    int n = al.run(L, a.qf + b, a.qr + b, a.cf + b, a.cr + b,
                    has_k ? a.nodes_f + ko : nullptr,
                    has_k && a.cfg.forward_and_reverse_complement ? a.nodes_r + ko : nullptr, order);
-    if (!act) return;
 #if defined(MGB_PHASE_TIMERS) && MGB_DEVICE_CODE
     if (wlane() == 0 && a.phase_out) {
         for (int p = 0; p < 8; ++p) atomicAdd((unsigned long long*)a.phase_out + p, (unsigned long long)al.phase_cycles[p]);
@@ -508,7 +506,7 @@ __global__ void __launch_bounds__(128) k_subk(SubkArgs a, uint32_t chunks_per_st
     }
 }
 
-// one lane group per read strand
+// one warp per read strand
 __global__ void __launch_bounds__(256) k_premap(SeedArgs a) {
     const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / kWarp;
     const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) / kWarp;
@@ -971,24 +969,23 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
 #define MGB_ALIGN_THREADS 128
 #endif
 static constexpr int kAlignThreads = MGB_ALIGN_THREADS;
-static constexpr int kGroupsPerBlock = kAlignThreads / kWarp;   // reads in flight per block of k_align
-// one lane group (kWarp lanes, common.cuh) per read; kAlignThreads / kWarp groups per block
+static constexpr int kWarpsPerBlock = kAlignThreads / kWarp;   // reads in flight per block of k_align
+// one warp per read
 __global__ void __launch_bounds__(kAlignThreads, MGB_ALIGN_MIN_BLOCKS) k_align(const __grid_constant__ AlignArgs a) {
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) / kWarp;
     char *arena = a.arena + (size_t)warp * a.arena_stride;
     extern __shared__ __align__(16) char smem_raw[];
     char *smem = smem_raw + (threadIdx.x / kWarp) * a.slay.total;
     init_arena(a, arena);
-    // the group's arena and on-chip working set: base + offsets from the kernel parameters
+    // the warp's arena and on-chip working set: base + offsets from the kernel parameters
     const WarpMem mem { arena, &a.lay };
     const WarpSmem sm { smem, &a.slay };
     while (true) {
         unsigned int t = 0;
         if (wlane() == 0) t = atomicAdd(a.next, 1u);
         t = wbcast(t, 0);
-        const bool have = t < a.n_list;
-        if (!wany_full(have)) break;
-        align_read(a, have ? a.read_list[t] : 0u, mem, sm, have);
+        if (t >= a.n_list) break;
+        align_read(a, a.read_list[t], mem, sm);
     }
 }
 

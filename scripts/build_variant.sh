@@ -1,6 +1,6 @@
 #!/bin/bash
 # builds metagraph_b200/_lib/libmgb_<tag>.so with extra nvcc flags (probes of kernel variants; select with MGB_LIB)
-#   scripts/build_variant.sh gw16 -DMGB_GROUP_WIDTH=16
+#   scripts/build_variant.sh timers -DMGB_PHASE_TIMERS
 set -e
 tag=$1; shift
 cd "$(dirname "$0")/.."
