@@ -164,6 +164,11 @@ uint64_t mgo_boss_succ_last(void *g, uint64_t i) { return static_cast<DBGSuccinc
 uint64_t mgo_boss_rank_W(void *g, uint64_t i, int c) { return static_cast<DBGSuccinct*>(g)->boss.rank_W(i, c); }
 uint64_t mgo_boss_rank_last(void *g, uint64_t i) { return static_cast<DBGSuccinct*>(g)->boss.rank_last(i); }
 uint64_t mgo_boss_select_last(void *g, uint64_t i) { return static_cast<DBGSuccinct*>(g)->boss.select_last(i); }
+// 1 if the source node of edge i has a single incoming edge (BOSS::is_single_incoming(bwd(i), last character))
+uint64_t mgo_boss_is_single_incoming(void *g, uint64_t i) {
+    auto &b = static_cast<DBGSuccinct*>(g)->boss;
+    return b.is_single_incoming(b.bwd(i), b.get_node_last_value(i)) ? 1 : 0;
+}
 void mgo_node_sequence(void *g, uint64_t node, char *out) {
     std::string s = static_cast<DBGSuccinct*>(g)->get_node_sequence(node);
     std::memcpy(out, s.data(), s.size());

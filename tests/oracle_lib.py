@@ -42,7 +42,7 @@ def lib():
         L.mgo_call_outgoing.restype = i
         L.mgo_call_outgoing.argtypes = [vp, u64, i, vp, vp]
         for f in ("mgo_boss_fwd", "mgo_boss_bwd", "mgo_boss_pred_last", "mgo_boss_succ_last",
-                  "mgo_boss_rank_last", "mgo_boss_select_last"):
+                  "mgo_boss_rank_last", "mgo_boss_select_last", "mgo_boss_is_single_incoming"):
             getattr(L, f).restype = u64
             getattr(L, f).argtypes = [vp, u64]
         for f in ("mgo_boss_pick_edge", "mgo_boss_rank_W"):

@@ -8,6 +8,7 @@ import dataclasses
 import numpy as np
 import pytest
 
+import index_tables as IT
 import oracle_lib as O
 import parity_common as P
 from metagraph_b200.aligner import B200Aligner, BOSSTable, DBGSuccinctIndex, format_alignment
@@ -49,8 +50,11 @@ class Case:
         else:
             monkeypatch.setenv("MGB_NO_KMER_HASH", "1")
         W, last, F, _ = self.g.arrays()
-        idx = DBGSuccinctIndex(BOSSTable(self.k, W, last, F))
+        boss = BOSSTable(self.k, W, last, F)
+        idx = DBGSuccinctIndex(boss)
         monkeypatch.delenv("MGB_NO_KMER_HASH", raising=False)
+        if hashed:
+            IT.assert_hashed(idx, boss)
         return idx
 
     def is_exact(self, r):

@@ -3,6 +3,7 @@ map_to_nodes, on reads whose strands run side by side in one lane with different
 import numpy as np
 import pytest
 
+import index_tables as IT
 import oracle_lib as O
 import parity_common as P
 from metagraph_b200.aligner import BOSSTable, DBGSuccinctIndex
@@ -47,7 +48,9 @@ def test_hashed_map_to_nodes_gpu(k, primary):
     if primary:
         g.set_mode(2)
     W, last, F, _ = g.arrays()
-    idx = DBGSuccinctIndex(BOSSTable(k, W, last, F), mode=2 if primary else 0)
+    boss = BOSSTable(k, W, last, F)
+    idx = DBGSuccinctIndex(boss, mode=2 if primary else 0)
+    IT.assert_hashed(idx, boss)
     reads = mixed_reads(rng, seqs, k, 1001)
     got = idx.map_to_nodes_sequentially(reads)
     bad = [i for i, (r, n) in enumerate(zip(reads, got)) if list(n) != list(g.map_to_nodes(r))]

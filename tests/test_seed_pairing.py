@@ -8,6 +8,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import index_tables as IT
 import oracle_lib as O
 import parity_common as P
 from metagraph_b200.aligner import BOSSTable, DBGSuccinctIndex
@@ -82,7 +83,9 @@ def test_map_to_nodes_strands_gpu(graph):
         graph_seqs = contigs
     g = O.OracleGraph(k, graph_seqs, mask=False)
     W, last, F, _ = g.arrays()
-    idx = DBGSuccinctIndex(BOSSTable(k, W, last, F))
+    boss = BOSSTable(k, W, last, F)
+    idx = DBGSuccinctIndex(boss)
+    IT.assert_hashed(idx, boss)
     reads = mixed_reads(rng, contigs, k, 1001) + role_reads(rng, contigs, k)
     fwd, rev = idx.map_to_nodes_strands(reads)
     idx.close()
