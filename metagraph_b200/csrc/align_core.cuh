@@ -151,6 +151,7 @@ struct OutAln {
 struct ReadStats { uint32_t num_seeds, num_extensions, num_explored_nodes, dp_columns; uint64_t dp_cells; };
 #if defined(MGB_HOST_EMU)
 extern "C" unsigned long long mgb_emu_whole_read_hits;   // host emulation (tests) only: reads answered by exact_read_strand()
+extern "C" unsigned long long mgb_emu_path_read_hits;    // ... and by exact_path_strand()
 // host emulation (tests) only: how often the aligner leaves its on-chip working set, so that a test can show which of
 // these paths its inputs reach. The order is part of the test interface (tests/parity_common.py EMU_PATHS).
 enum EmuPath : int {

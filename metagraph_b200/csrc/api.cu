@@ -773,11 +773,13 @@ int launch_prepare(const mgb_index_t *index, const Batch &b, Stream &st, int num
     return 0;
 }
 
-// summary: SeedArgs::summary (k_seed_hash writes it; nullptr on graphs without the k-mer hash index)
+// summary: SeedArgs::summary (k_seed_hash writes it; nullptr on graphs without the k-mer hash index); list / n_list:
+// SeedArgs::list (k_seed_hash only)
 int launch_seed(const mgb_index_t *index, const Batch &b, uint32_t n_strands, Stream &st, DevBufs &bufs,
-                uint8_t *summary, uint64_t *n_launches = nullptr) {
+                uint8_t *summary, uint64_t *n_launches = nullptr, const uint32_t *list = nullptr,
+                const unsigned int *n_list = nullptr) {
     SeedArgs a { index->view, b.cf, b.cr, b.offsets, b.koff, b.nodes_f, b.nodes_r, b.n_reads, n_strands, 0, nullptr, nullptr,
-                 summary };
+                 summary, list, n_list };
     uint64_t items = (uint64_t)b.n_reads * n_strands;
     // first pass (k_premap): rules out the k-mers the suffix-range table has no node for; the node arrays
     // are zero-filled, so the second pass only visits what is left
@@ -796,7 +798,12 @@ int launch_seed(const mgb_index_t *index, const Batch &b, uint32_t n_strands, St
     (void)st;
     if (premap)
         for (uint64_t it = 0; it < items; ++it) premap_item(a, (uint32_t)(it / n_strands), (uint32_t)(it % n_strands));
-    for (uint64_t it = 0; it < items; ++it) seed_item(a, it);
+    if (list) {
+        for (uint32_t t = 0; t < *n_list; ++t)
+            for (uint32_t s = 0; s < n_strands; ++s) seed_item(a, (uint64_t)list[t] * n_strands + s);
+    } else {
+        for (uint64_t it = 0; it < items; ++it) seed_item(a, it);
+    }
 #else
     if (!items) return 0;
     if (premap) {
@@ -818,7 +825,8 @@ int launch_seed(const mgb_index_t *index, const Batch &b, uint32_t n_strands, St
 int launch_exact_reads(const mgb_index_t *index, const ExactArgs &a, Stream &st) {
 #if defined(MGB_HOST_EMU)
     (void)index; (void)st;
-    for (uint32_t t = 0; t < a.n_list; ++t) {
+    const uint32_t n_list = a.n_list_dev ? *a.n_list_dev : a.n_list;
+    for (uint32_t t = 0; t < n_list; ++t) {
         const uint32_t r = a.list[t];
         uint64_t b; int L; score_t score;
         const int s = exact_read_strand(a, a.diag, r, &b, &L, &score);
@@ -828,6 +836,29 @@ int launch_exact_reads(const mgb_index_t *index, const ExactArgs &a, Stream &st)
     }
 #else
     if (a.n_list) CUDA_TRY(kern_dna::launch_exact_reads(index->num_sms, st.s, a));
+#endif
+    return 0;
+}
+
+// whole-read exact answers from the raw reads (kernels.cuh PrepExactArgs), in place of launch_prepare; the reads left
+// over are prepared and listed in a.list
+int launch_prepare_exact(const mgb_index_t *index, const PrepExactArgs &a, Stream &st) {
+#if defined(MGB_HOST_EMU)
+    (void)index; (void)st;
+    for (uint32_t r = 0; r < a.prep.n_reads; ++r) {
+        uint64_t b; int L; uint32_t p; score_t score;
+        int s = exact_path_strand(a, r, &b, &L, &p, &score);
+        const uint64_t off = *a.ex.heap_used;
+        if (s >= 0) {
+            *a.ex.heap_used += exact_read_bytes(a.ex, L);
+            if (off + exact_read_bytes(a.ex, L) > a.ex.heap_cap) s = -1;
+        }
+        if (s >= 0) { exact_path_write(a, r, b, L, s, p, score, off, 0, 1); continue; }
+        a.list[(*a.n_list)++] = r;
+        prepare_read(a.prep, r);
+    }
+#else
+    if (a.prep.n_reads) CUDA_TRY(kern_dna::launch_prepare_exact(index->num_sms, st.s, a));
 #endif
     return 0;
 }
@@ -996,12 +1027,73 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
         if (!rc && exact_reads && index->view.kh_slots) rc = bufs.alloc(&summary, (size_t)n_reads + 1);
         if (!rc) rc = dev_zero(b.nodes_f, (b.total_kmers + 1) * 8, st);
         if (!rc && both) rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, st);
+        ReadHdr *d_hdr = nullptr;
+        if (!rc) rc = bufs.alloc(&d_hdr, (size_t)n_reads + 1);
+        // query length k_align stages on chip (0: none; MGB_TEST_LQ: test knob that forces the unstaged path)
+        const int lq = b.L_max + 1 <= 512 ? (int)((b.L_max + 1 + 15) & ~15u) : 0;
+        int lq_v = lq;
+        if (const char *e = std::getenv("MGB_TEST_LQ")) lq_v = std::atoi(e);
+        // output heap of a pass over n reads: generous first guess, doubled on retry passes (MGB_TEST_HEAP0: test knob,
+        // pass 0's capacity in bytes)
+        auto heap_cap_of = [&](uint64_t n, uint32_t scale) {
+            const uint64_t per_read = sizeof(OutAln) + 9ull * (b.L_max + 64 + index->view.k) + 4ull * 64;
+            uint64_t cap = n * per_read * dcfg.num_alternative_paths * scale + 4096;
+            if (const char *e = std::getenv("MGB_TEST_HEAP0")) if (scale == 1) cap = std::min<uint64_t>(cap, std::atoll(e));
+            return cap;
+        };
+        // longest read with a whole-read exact answer: k_align's own exit needed both strands staged on chip
+        // (L + 1 <= lq) and room for L characters and L - k + 1 nodes in an alignment slot
+        auto exact_max_len = [&](const Caps &caps) -> uint32_t {
+            const uint64_t max_len = std::min<uint64_t>({ lq_v > 0 ? (uint64_t)lq_v - 1 : 0, caps.aln_seq,
+                                                         (uint64_t)caps.aln_nodes + k - 1 });
+            return caps.aln_cigar >= 1 ? (uint32_t)max_len : 0;
+        };
+        auto exact_args = [&](const Caps &caps, ExactArgs *ea) {
+            std::memset(ea, 0, sizeof(*ea));
+            ea->k = k;
+            ea->end_bonus = dcfg.left_end_bonus + dcfg.right_end_bonus;
+            ea->min_score = std::max({ 0, (int)dcfg.min_cell_score, (int)dcfg.min_path_score });
+            ea->max_len = exact_max_len(caps);
+            ea->result_nodes = dcfg.result_nodes;
+            std::memcpy(ea->diag, dcfg.diag, sizeof(ea->diag));
+            ea->qf = b.qf; ea->qr = b.qr; ea->offsets = b.offsets; ea->koff = b.koff;
+            ea->nodes_f = b.nodes_f; ea->nodes_r = b.nodes_r; ea->summary = summary;
+            ea->hdr = d_hdr;
+        };
+        // Whole-read exact answers from the raw reads, in place of k_prepare (kernels.cuh PrepExactArgs), on graphs with
+        // the k-mer hash index and the path layout: the reads left over are prepared, seeded and go on as before. Pass 0's
+        // heap, its counters and the list exist before the kernel runs; pass 0 below takes them over.
+        // MGB_TEST_NO_PREPARE_EXACT: test knob, the route off.
+        PrepExactArgs pa;
+        std::memset(&pa, 0, sizeof(pa));
+        unsigned int *next0 = nullptr;      // k_align's next read, the reads k_exact_reads leaves, the length of pa.list
+        uint32_t *rest0 = nullptr;
+        const bool prep_exact = !rc && exact_reads && index->view.kh_slots && index->view.pl_n
+                                && exact_max_len(choose_caps(b.L_max, dcfg, k, 1)) >= k
+                                && !std::getenv("MGB_TEST_NO_PREPARE_EXACT");
+        if (prep_exact) {
+            pa.ix = index->view;
+            pa.prep = PrepArgs { b.seqs, b.offsets, b.n_reads, b.qf, b.qr, b.cf, b.cr, {0} };
+            std::memcpy(pa.prep.code_of, index->at.code_of, sizeof(pa.prep.code_of));
+            exact_args(choose_caps(b.L_max, dcfg, k, 1), &pa.ex);
+            pa.ex.heap_cap = heap_cap_of(n_reads, 1);
+            if (!rc) rc = bufs.alloc(&pa.ex.heap, pa.ex.heap_cap);
+            if (!rc) rc = bufs.alloc(&pa.ex.heap_used, 1);
+            if (!rc) rc = bufs.alloc(&next0, 4);
+            if (!rc) rc = bufs.alloc(&pa.list, (size_t)n_reads + 1);
+            if (!rc) rc = bufs.alloc(&rest0, (size_t)n_reads + 1);
+            if (!rc) rc = dev_zero(pa.ex.heap_used, 8, st);
+            if (!rc) rc = dev_zero(next0, 16, st);
+            pa.n_list = next0 + 2;
+        }
 #if !defined(MGB_HOST_EMU)
         cudaEventRecord(ev[1], st.s);
 #endif
-        if (!rc) rc = launch_prepare(index, b, st, index->num_sms);
+        if (!rc) rc = prep_exact ? launch_prepare_exact(index, pa, st) : launch_prepare(index, b, st, index->num_sms);
         res->stats.kernel_launches += 1;
-        if (!rc && map_nodes) rc = launch_seed(index, b, both ? 2 : 1, st, bufs, summary, &res->stats.kernel_launches);
+        if (!rc && map_nodes)
+            rc = launch_seed(index, b, both ? 2 : 1, st, bufs, summary, &res->stats.kernel_launches,
+                             prep_exact ? pa.list : nullptr, prep_exact ? pa.n_list : nullptr);
         // sub-k seeding (min_seed_length < k): the independent index_range lookups run GPU-wide first
         SubkArgs sk;
         std::memset(&sk, 0, sizeof(sk));
@@ -1038,8 +1130,6 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
 #if !defined(MGB_HOST_EMU)
         cudaEventRecord(ev[2], st.s);
 #endif
-        ReadHdr *d_hdr = nullptr;
-        if (!rc) rc = bufs.alloc(&d_hdr, (size_t)n_reads + 1);
 
         // align passes: all reads with scale 1, overflowed reads again with larger arenas
         std::vector<uint32_t> list(n_reads);
@@ -1057,12 +1147,10 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             if (dcfg.gap_ext < 0 && dcfg.xdrop < (1 << 20))
                 band_est = std::min<uint64_t>(band_est, 2ull * (dcfg.xdrop / (-dcfg.gap_ext)) + 16 + 8);
             const int bmax = band_est <= 256 ? std::max(64, (int)((band_est + 31) & ~31ull)) : 256;
-            const int lq = b.L_max + 1 <= 512 ? (int)((b.L_max + 1 + 15) & ~15u) : 0;
             int hcap = 16;
-            // test knobs: force the spill paths (arena scratch, queue migration, unstaged query)
-            int bmax_v = bmax, lq_v = lq;
+            // test knobs: force the spill paths (arena scratch, queue migration)
+            int bmax_v = bmax;
             if (const char *e = std::getenv("MGB_TEST_BMAX")) bmax_v = std::atoi(e);
-            if (const char *e = std::getenv("MGB_TEST_LQ")) lq_v = std::atoi(e);
             if (const char *e = std::getenv("MGB_TEST_HCAP")) hcap = std::atoi(e);
             SmemLayout slay;
             const size_t smem_per_warp = slay.carve(bmax_v, lq_v, hcap, !index->view.wide);
@@ -1105,37 +1193,35 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             if (dbg_time) std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident)\n", n_warps,
                                        (unsigned long long)index->num_sms * blocks_per_sm * wpb);
 #endif
-            // output heap: generous first guess, doubled on retry passes
-            uint64_t per_read = sizeof(OutAln) + 9ull * (b.L_max + 64 + index->view.k) + 4ull * 64;
-            uint64_t heap_cap = (uint64_t)list.size() * per_read * dcfg.num_alternative_paths * scale + 4096;
+            // pass 0 after k_prepare_exact: its heap, counters and list of reads left over are in place already
+            const bool listed = pass == 0 && prep_exact;
+            const uint64_t heap_cap = listed ? pa.ex.heap_cap : heap_cap_of(list.size(), scale);
             char *d_arena = nullptr, *d_heap = nullptr; uint32_t *d_list = nullptr, *d_rest = nullptr;
             unsigned long long *d_used = nullptr; unsigned int *d_next = nullptr;
             if ((rc = pass_bufs.alloc(&d_arena, stride * n_warps))) break;
-            if ((rc = pass_bufs.alloc(&d_heap, heap_cap))) break;
-            if ((rc = pass_bufs.alloc(&d_list, list.size()))) break;
-            if ((rc = pass_bufs.alloc(&d_used, 1))) break;
-            if ((rc = pass_bufs.alloc(&d_next, 2))) break;        // k_align's next read; the reads k_exact_reads leaves
-            if (exact_reads && (rc = pass_bufs.alloc(&d_rest, list.size()))) break;
+            if (listed) {
+                d_heap = pa.ex.heap; d_list = pa.list; d_used = pa.ex.heap_used; d_next = next0; d_rest = rest0;
+            } else {
+                if ((rc = pass_bufs.alloc(&d_heap, heap_cap))) break;
+                if ((rc = pass_bufs.alloc(&d_list, list.size()))) break;
+                if ((rc = pass_bufs.alloc(&d_used, 1))) break;
+                if ((rc = pass_bufs.alloc(&d_next, 2))) break;    // k_align's next read; the reads k_exact_reads leaves
+                if (exact_reads && (rc = pass_bufs.alloc(&d_rest, list.size()))) break;
+            }
             tick("pass: arena/heap alloc");
-            if ((rc = h2d(d_list, list.data(), list.size() * 4, st))) break;
-            if ((rc = dev_zero(d_used, 8, st))) break;
-            if ((rc = dev_zero(d_next, 8, st))) break;
+            if (!listed) {
+                if ((rc = h2d(d_list, list.data(), list.size() * 4, st))) break;
+                if ((rc = dev_zero(d_used, 8, st))) break;
+                if ((rc = dev_zero(d_next, 8, st))) break;
+            }
             // the read-dependent part of the gate (exact_read_strand); max_len keeps what k_align's own exit required
             ExactArgs ea;
             std::memset(&ea, 0, sizeof(ea));
             if (exact_reads) {
-                ea.k = k;
-                ea.end_bonus = dcfg.left_end_bonus + dcfg.right_end_bonus;
-                ea.min_score = std::max({ 0, (int)dcfg.min_cell_score, (int)dcfg.min_path_score });
-                const uint64_t max_len = std::min<uint64_t>({ lq_v > 0 ? (uint64_t)lq_v - 1 : 0, caps.aln_seq,
-                                                             (uint64_t)caps.aln_nodes + k - 1 });
-                ea.max_len = caps.aln_cigar >= 1 ? (uint32_t)max_len : 0;
-                ea.result_nodes = dcfg.result_nodes;
-                std::memcpy(ea.diag, dcfg.diag, sizeof(ea.diag));
-                ea.qf = b.qf; ea.qr = b.qr; ea.offsets = b.offsets; ea.koff = b.koff;
-                ea.nodes_f = b.nodes_f; ea.nodes_r = b.nodes_r; ea.summary = summary;
-                ea.list = d_list; ea.n_list = (uint32_t)list.size(); ea.rest = d_rest; ea.n_rest = d_next + 1;
-                ea.hdr = d_hdr; ea.heap = d_heap; ea.heap_cap = heap_cap; ea.heap_used = d_used;
+                exact_args(caps, &ea);
+                ea.list = d_list; ea.n_list = (uint32_t)list.size(); ea.n_list_dev = listed ? pa.n_list : nullptr;
+                ea.rest = d_rest; ea.n_rest = d_next + 1;
+                ea.heap = d_heap; ea.heap_cap = heap_cap; ea.heap_used = d_used;
             }
             const bool run_exact = exact_reads && ea.max_len >= k;
             AlignArgs a;
@@ -1162,12 +1248,14 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             if (run_exact) {
                 // k_align takes only the reads left over; their count sizes its grid
                 if ((rc = launch_exact_reads(index, ea, st))) break;
-                uint32_t n_rest = 0;
-                if ((rc = d2h(&n_rest, d_next + 1, 4, st))) break;
+                uint32_t n_rest[2] = { 0, 0 };          // and after k_prepare_exact, the length of its list
+                if ((rc = d2h(n_rest, d_next + 1, listed ? 8 : 4, st))) break;
 #if !defined(MGB_HOST_EMU)
                 CUDA_TRY(cudaStreamSynchronize(st.s));
 #endif
-                a.read_list = d_rest; a.n_list = n_rest;
+                if (listed && dbg_time)
+                    std::fprintf(stderr, "[mgb] reads %u+%u k_prepare_exact answered %u\n", lo, n_reads, n_reads - n_rest[1]);
+                a.read_list = d_rest; a.n_list = n_rest[0];
                 res->stats.kernel_launches += 1;
             }
 #if defined(MGB_HOST_EMU)
@@ -1283,7 +1371,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
 
 static std::atomic<uint32_t> g_max_pieces{0};      // 0 = automatic
 #if defined(MGB_HOST_EMU)
-extern "C" { unsigned long long mgb_emu_whole_read_hits = 0; unsigned long long mgb_emu_path_hits[EMU_N_PATHS] = {}; }
+extern "C" { unsigned long long mgb_emu_whole_read_hits = 0, mgb_emu_path_read_hits = 0; unsigned long long mgb_emu_path_hits[EMU_N_PATHS] = {}; }
 #endif
 
 extern "C" {

@@ -55,6 +55,9 @@ struct SeedArgs {
     // k_seed_hash only (nullptr: not written): per read, which kinds of node id the walk stored, as ExactArgs::summary
     // reads them (1: a 0 on the forward strand, 2: a non-zero one; 4 / 8: the same on the reverse strand; 0 if L < k)
     uint8_t *summary;
+    // k_seed_hash only: the reads to seed, list[0 .. *n_list) (built on the device by k_prepare_exact); nullptr: all
+    // n_reads reads
+    const uint32_t *list; const unsigned int *n_list;
 };
 
 MGB_HD void seed_item(const SeedArgs &a, uint64_t item) {
@@ -243,6 +246,7 @@ struct ExactArgs {
     const char *qf, *qr; const uint64_t *offsets, *koff, *nodes_f, *nodes_r;
     const uint8_t *summary;       // SeedArgs::summary, or nullptr: the same bits from nodes_f / nodes_r
     const uint32_t *list; uint32_t n_list;
+    const unsigned int *n_list_dev;                  // non-null: the list's length is *n_list_dev (<= n_list)
     uint32_t *rest; unsigned int *n_rest;            // the reads left to k_align
     ReadHdr *hdr; char *heap; uint64_t heap_cap; unsigned long long *heap_used;
 };
@@ -288,11 +292,13 @@ MGB_HD uint32_t exact_read_bytes(const ExactArgs &a, int L) {
     return (uint32_t)sizeof(OutAln) + (a.result_nodes ? 0u : 8u * (uint32_t)(L - (int)a.k + 1)) + 8u + (((uint32_t)L + 7u) & ~7u);
 }
 
-// Writes the record of read r (strand s) at heap offset `off` and the read's header, the same bytes align_read writes for
-// it, padding as zeros; a record past the end of the heap marks the read MGB_READ_OVERFLOW (the next pass retries it).
-// Lanes `lane` of `width` share the copies.
-MGB_HD void exact_read_write(const ExactArgs &a, uint32_t r, uint64_t b, int L, int s, score_t score, uint64_t off,
-                             int lane, int width) {
+// The one layout of a whole-read exact answer ({L}= along strand s, L - k + 1 nodes): writes the record of read r at heap
+// offset `off` and the read's header, the same bytes align_read writes for it, padding as zeros; a record past the end
+// of the heap marks the read MGB_READ_OVERFLOW (the next pass retries it). node(t) / chr(t): the strand's node id t and
+// prepared character t. Lanes `lane` of `width` share the copies.
+template <class Node, class Chr>
+MGB_HD void exact_record_write(const ExactArgs &a, uint32_t r, int L, int s, score_t score, uint64_t off, Node node, Chr chr,
+                               int lane, int width) {
     const int nk = L - (int)a.k + 1;
     ReadHdr h;
     h.status = MGB_READ_OK; h.n_aln = 1; h.heap_off = off;
@@ -310,16 +316,202 @@ MGB_HD void exact_read_write(const ExactArgs &a, uint32_t r, uint64_t b, int L, 
         }
         p += sizeof(OutAln);
         if (!a.result_nodes) {
-            const uint64_t *qn = (s ? a.nodes_r : a.nodes_f) + a.koff[r];
-            for (int t = lane; t < nk; t += width) reinterpret_cast<uint64_t*>(p)[t] = qn[t];
+            for (int t = lane; t < nk; t += width) reinterpret_cast<uint64_t*>(p)[t] = node(t);
             p += 8ull * nk;
         }
         if (lane == 0) *reinterpret_cast<unsigned long long*>(p) = cig_pack(OP_M, (uint32_t)L);
         p += 8;
-        const char *q = (s ? a.qr : a.qf) + b;
-        for (int t = lane; t < ((L + 7) & ~7); t += width) p[t] = t < L ? q[t] : 0;
+        for (int t = lane; t < ((L + 7) & ~7); t += width) p[t] = t < L ? chr(t) : 0;
     }
     if (lane == 0) a.hdr[r] = h;
+}
+
+// exact_record_write from the seeding kernel's node arrays and the prepared strands
+MGB_HD void exact_read_write(const ExactArgs &a, uint32_t r, uint64_t b, int L, int s, score_t score, uint64_t off,
+                             int lane, int width) {
+    const uint64_t *qn = (s ? a.nodes_r : a.nodes_f) + a.koff[r];
+    const char *q = (s ? a.qr : a.qf) + b;
+    exact_record_write(a, r, L, s, score, off, [qn](int t) { return qn[t]; }, [q](int t) { return q[t]; }, lane, width);
+}
+
+#if MGB_DEVICE_CODE
+// One k-mer lookup in the hash index (kh_lookup) in three parts, so that a lane keeps several in flight: issue() loads
+// the k-mer's bucket (nothing when `on` is false), find() settles it (a full bucket without the k-mer continues in the
+// next one, rare at this load factor), value() loads the edge (0: not in the graph).
+struct KhProbe {
+    unsigned long long want;
+    uint64_t slot;
+    ulonglong2 ka, kb;
+    int h;
+    MGB_D void issue(const IndexView &ix, unsigned long long key, bool on) {
+        want = key | (1ull << 63);
+        slot = kh_slot_of(want, ix.kh_slots);
+        ka = make_ulonglong2(0ull, 0ull); kb = ka;
+        if (on) {
+            ka = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot));
+            kb = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot + 2));
+        }
+    }
+    MGB_D void find(const IndexView &ix) {
+        h = ka.x == want ? 0 : ka.y == want ? 1 : kb.x == want ? 2 : kb.y == want ? 3 : -1;
+        bool more = h < 0 && ka.x != 0 && ka.y != 0 && kb.x != 0 && kb.y != 0;     // never when not issued
+        while (more) {
+            slot += 4; if (slot >= ix.kh_slots) slot = 0;
+            const ulonglong2 x = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot));
+            const ulonglong2 y = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot + 2));
+            h = x.x == want ? 0 : x.y == want ? 1 : y.x == want ? 2 : y.y == want ? 3 : -1;
+            more = h < 0 && x.x != 0 && x.y != 0 && y.x != 0 && y.y != 0;
+        }
+    }
+    MGB_D uint64_t value(const IndexView &ix) const { return h >= 0 ? __ldg(ix.kh_vals + slot + h) : 0u; }
+};
+#endif
+
+// Whole-read exact answers straight from the raw characters (k_prepare_exact, in place of k_prepare): a read is answered
+// here only if
+//   1. k <= L <= max_len, and every character is A, C, G or T (after sanitize_char);
+//   2. of the position-0 k-mers of the two strands exactly one is in the hash index (the primary strand), its edge is
+//      in_graph and has a place p on the path layout;
+//   3. pl_text[p .. p + L) is the primary strand, no pl_stop bit is set in [p, p + L - k + 1) and no pl_rc bit in the same
+//      range;
+//   4. Σ diag over the primary strand plus both end bonuses >= min_score.
+// k_seed_hash would then walk the read paired (2), and the primary's walk would stay on the path to the end (3: each next
+// character is the path's, the path goes on): it stores pl_node[p .. p + nk) on the primary. Every secondary k-mer is the
+// reverse complement of a primary k-mer (1: no invalid window) whose pl_rc bit is 0, so its lookup misses and it stores 0.
+// So exact_read_strand would take the primary with the same score (4), and the record is exact_record_write's with
+// node ids pl_node[p + t]. Every other read is prepared as by prepare_read and seeded; k_exact_reads still answers the
+// exact ones among them (across a path end, with a pl_rc bit set, ...). DESIGN.md §3.3.
+struct PrepExactArgs {
+    IndexView ix;                // with the k-mer hash index and the path layout
+    PrepArgs prep;                // the raw reads, and the strand buffers of the reads left over
+    ExactArgs ex;                 // k, end_bonus, min_score, max_len, result_nodes, diag; hdr and the heap
+    uint32_t *list; unsigned int *n_list;            // the reads left over (prepared, to be seeded)
+};
+
+MGB_HD unsigned long long ldg64(const unsigned long long *p) {
+#if MGB_DEVICE_CODE
+    return __ldg(p);
+#else
+    return *p;
+#endif
+}
+// 2-bit code of an A/C/G/T byte, upper or lower case (A 0, C 1, G 2, T 3); *ok is cleared for any other byte
+MGB_HD uint32_t acgt_code(uint32_t ch, bool *ok) {
+    const uint32_t u = ch & 0xDFu;
+    *ok = *ok && ch < 128 && (u == 'A' || u == 'C' || u == 'G' || u == 'T');
+    return ((u >> 1) ^ (u >> 2)) & 3u;
+}
+// Σ diag over the characters whose 2-bit codes are given, from the four diag values packed one byte each
+MGB_HD int diag_of(uint32_t dg4, uint32_t code) { return (int)(int8_t)(uint8_t)(dg4 >> (8 * code)); }
+
+// The primary strand (0 / 1) of read r if the read is answered here (conditions above), else -1; *b / *L: the read's
+// start and length, *pos: its place p on the path, *score: the alignment's score. One lane, no collectives. The raw
+// characters are read as aligned 8-byte words (the buffer is padded past its end).
+MGB_HD int exact_path_strand(const PrepExactArgs &a, uint32_t r, uint64_t *b, int *L, uint32_t *pos, score_t *score) {
+    const IndexView &ix = a.ix;
+    *b = a.prep.offsets[r];
+    *L = (int)(a.prep.offsets[r + 1] - *b);
+    const int n = *L, K = (int)a.ex.k;
+    if (n < K || n > (int)a.ex.max_len) return -1;
+    const uintptr_t lo = (uintptr_t)(a.prep.seqs + *b), hi = lo + (uintptr_t)n;
+    // ---- the position-0 k-mers of both strands: characters [0, k) forward, [L - k, L) backwards and complemented
+    bool ok = true;
+    unsigned long long kf = 0, kr = 0;
+    {
+        const uintptr_t e = lo + (uintptr_t)K;
+        for (uintptr_t w = lo & ~(uintptr_t)7; w < e; w += 8) {
+            const unsigned long long x = ldg64(reinterpret_cast<const unsigned long long*>(w));
+            const int j0 = w < lo ? (int)(lo - w) : 0, j1 = e - w < 8 ? (int)(e - w) : 8;
+            for (int j = j0; j < j1; ++j) kf |= (unsigned long long)acgt_code((uint32_t)(x >> (8 * j)) & 0xFFu, &ok) << (2 * (w + j - lo));
+        }
+        const uintptr_t s0 = hi - (uintptr_t)K;
+        for (uintptr_t w = s0 & ~(uintptr_t)7; w < hi; w += 8) {
+            const unsigned long long x = ldg64(reinterpret_cast<const unsigned long long*>(w));
+            const int j0 = w < s0 ? (int)(s0 - w) : 0, j1 = hi - w < 8 ? (int)(hi - w) : 8;
+            for (int j = j0; j < j1; ++j)        // raw position i is reverse-strand position L - 1 - i
+                kr |= (unsigned long long)(3u - acgt_code((uint32_t)(x >> (8 * j)) & 0xFFu, &ok)) << (2 * (hi - 1 - (w + j)));
+        }
+    }
+    if (!ok) return -1;
+    uint64_t ef, er;
+#if MGB_DEVICE_CODE
+    {
+        KhProbe pf, pr;                                     // both lookups in flight
+        pf.issue(ix, kf, true); pr.issue(ix, kr, true);
+        pf.find(ix); pr.find(ix);
+        ef = pf.value(ix); er = pr.value(ix);
+    }
+#else
+    ef = kh_lookup(ix, kf); er = kh_lookup(ix, kr);
+#endif
+    if ((ef != 0) == (er != 0)) return -1;
+    const int s = ef ? 0 : 1;
+    const uint64_t e = s ? er : ef;
+    if (!in_graph(ix, e)) return -1;
+    const uint32_t p = ldg32(ix.pl_pos + e);
+    if (p == kPlNone) return -1;
+    // ---- pl_stop / pl_rc over [p, p + nk): a 0 stop bit at p + 1 .. p + nk - 1 keeps the path going (p is a node); this
+    // comes first, so that the text below is read inside the path and its filler
+    const uint32_t end = p + (uint32_t)(n - K + 1);
+    for (uint32_t q0 = p & ~31u; q0 < end; q0 += 32) {
+        uint32_t m = q0 < p ? ~0u << (p - q0) : ~0u;
+        if (end - q0 < 32) m &= (1u << (end - q0)) - 1u;
+        if ((ldg32(ix.pl_stop + (q0 >> 5)) | ldg32(ix.pl_rc + (q0 >> 5))) & m) return -1;
+    }
+    // ---- the primary strand against pl_text[p .. p + L), 32 characters per compare; its Σ diag on the way
+    const uint32_t dg4 = (uint32_t)(uint8_t)a.ex.diag['A'] | (uint32_t)(uint8_t)a.ex.diag['C'] << 8
+                       | (uint32_t)(uint8_t)a.ex.diag['G'] << 16 | (uint32_t)(uint8_t)a.ex.diag['T'] << 24;
+    int sum = 0;
+    unsigned long long acc = 0;                             // primary characters i0 .. i0 + na - 1
+    int na = 0;
+    uint32_t i0 = 0;
+    bool same = true;
+    auto compare = [&]() {
+        const uint32_t P = p + i0, sh = 2 * (P & 31);
+        unsigned long long t = ldg64(ix.pl_text + (P >> 5)) >> sh;
+        if (sh) t |= ldg64(ix.pl_text + (P >> 5) + 1) << (64 - sh);
+        if (na < 32) t &= (1ull << (2 * na)) - 1;
+        same = same && t == acc;
+        i0 += 32; acc = 0; na = 0;
+    };
+    auto put = [&](uint32_t code) {
+        sum += diag_of(dg4, code);
+        acc |= (unsigned long long)code << (2 * na);
+        if (++na == 32) compare();
+    };
+    if (s == 0) {
+        for (uintptr_t w = lo & ~(uintptr_t)7; w < hi && same; w += 8) {
+            const unsigned long long x = ldg64(reinterpret_cast<const unsigned long long*>(w));
+            const int j0 = w < lo ? (int)(lo - w) : 0, j1 = hi - w < 8 ? (int)(hi - w) : 8;
+            for (int j = j0; j < j1; ++j) put(acgt_code((uint32_t)(x >> (8 * j)) & 0xFFu, &ok));
+        }
+    } else {
+        for (uintptr_t w = (hi - 1) & ~(uintptr_t)7; w + 8 > lo && same; w -= 8) {
+            const unsigned long long x = ldg64(reinterpret_cast<const unsigned long long*>(w));
+            const int j0 = w < lo ? (int)(lo - w) : 0, j1 = hi - w < 8 ? (int)(hi - w) : 8;
+            for (int j = j1 - 1; j >= j0; --j) put(3u - acgt_code((uint32_t)(x >> (8 * j)) & 0xFFu, &ok));
+        }
+    }
+    if (na) compare();
+    if (!ok || !same) return -1;
+    const score_t full = sum + a.ex.end_bonus;
+    if (full < a.ex.min_score) return -1;
+#if defined(MGB_HOST_EMU)
+    ++mgb_emu_path_read_hits;
+#endif
+    *pos = p; *score = full;
+    return s;
+}
+
+// exact_record_write of a read exact_path_strand answered: node ids from the path layout, characters from the raw read
+MGB_HD void exact_path_write(const PrepExactArgs &a, uint32_t r, uint64_t b, int L, int s, uint32_t p, score_t score,
+                             uint64_t off, int lane, int width) {
+    const uint32_t *pn = a.ix.pl_node + p;
+    const char *raw = a.prep.seqs + b;
+    exact_record_write(a.ex, r, L, s, score, off, [pn](int t) { return (uint64_t)ldg32(pn + t); },
+                       [raw, L, s](int t) {
+                           return s ? (char)complement_char(sanitize_char((uint8_t)raw[L - 1 - t])) : (char)sanitize_char((uint8_t)raw[t]);
+                       }, lane, width);
 }
 
 // One refinement level of the suffix-range table (boss.hpp:651-655 index order: the appended
@@ -700,37 +892,6 @@ MGB_D unsigned long long first_kmer(CodeStream &cs, const uint8_t *codes, int L,
     return key;
 }
 
-// One k-mer lookup in the hash index (kh_lookup) in three parts, so that a lane keeps several in flight: issue() loads
-// the k-mer's bucket (nothing when `on` is false), find() settles it (a full bucket without the k-mer continues in the
-// next one, rare at this load factor), value() loads the edge (0: not in the graph).
-struct KhProbe {
-    unsigned long long want;
-    uint64_t slot;
-    ulonglong2 ka, kb;
-    int h;
-    MGB_D void issue(const IndexView &ix, unsigned long long key, bool on) {
-        want = key | (1ull << 63);
-        slot = kh_slot_of(want, ix.kh_slots);
-        ka = make_ulonglong2(0ull, 0ull); kb = ka;
-        if (on) {
-            ka = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot));
-            kb = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot + 2));
-        }
-    }
-    MGB_D void find(const IndexView &ix) {
-        h = ka.x == want ? 0 : ka.y == want ? 1 : kb.x == want ? 2 : kb.y == want ? 3 : -1;
-        bool more = h < 0 && ka.x != 0 && ka.y != 0 && kb.x != 0 && kb.y != 0;     // never when not issued
-        while (more) {
-            slot += 4; if (slot >= ix.kh_slots) slot = 0;
-            const ulonglong2 x = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot));
-            const ulonglong2 y = __ldg(reinterpret_cast<const ulonglong2*>(ix.kh_keys + slot + 2));
-            h = x.x == want ? 0 : x.y == want ? 1 : y.x == want ? 2 : y.y == want ? 3 : -1;
-            more = h < 0 && x.x != 0 && x.y != 0 && y.x != 0 && y.y != 0;
-        }
-    }
-    MGB_D uint64_t value(const IndexView &ix) const { return h >= 0 ? __ldg(ix.kh_vals + slot + h) : 0u; }
-};
-
 // Node ids of a strand leave in whole 32-byte sectors: s0..s3 are the slots of the sector being filled (slot q of
 // node id i is (address / 8) % 4). A sector the strand shares with a neighbouring read gets single stores of the
 // strand's own slots. Single 8-byte stores left sectors partly written in L2, and evicting one of those most likely
@@ -828,7 +989,7 @@ struct PathWalk {
 // return to it. (c2 k_seed_hash: 6.0 ms -> 2.85 ms, DESIGN.md §3.2.)
 //
 // Steps are written with selects rather than branches: lanes in different regimes issue together. Persistent grid:
-// lane t of n_lanes takes the reads t + n_lanes * round.
+// lane t of n_lanes takes the reads t + n_lanes * round, or those entries of a.list (the reads k_prepare_exact left over).
 __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash(const __grid_constant__ SeedArgs a) {
     const IndexView &ix = a.ix;
     const int K = (int)ix.k;
@@ -836,8 +997,10 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
     const unsigned long long mask = (1ull << (2 * K)) - 1;
     const uint32_t sigma = ix.sigma;
     const bool two = a.n_strands == 2;
-    const uint64_t lanes = (uint64_t)gridDim.x * blockDim.x;
-    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < a.n_reads; r += lanes) {
+    const uint32_t lanes = gridDim.x * blockDim.x;
+    const uint32_t n_items = a.list ? *a.n_list : a.n_reads;
+    for (uint32_t it = blockIdx.x * blockDim.x + threadIdx.x; it < n_items; it += lanes) {
+        const uint32_t r = a.list ? __ldg(a.list + it) : it;
         const uint64_t b = a.offsets[r];
         const int L = (int)(a.offsets[r + 1] - b);
         const int nk = L >= K ? L - K + 1 : 0;
@@ -1044,6 +1207,8 @@ __global__ void __launch_bounds__(256) k_prepare(PrepArgs a) {
 // others one append to a.rest. Then each warp writes its answered records one after the other, 32 lanes per record.
 // Persistent grid. No index structure is read.
 static constexpr int kExactThreads = 256;
+// the length of a.list (loaded again each round: holding it across the loop made ptxas spill)
+__device__ __forceinline__ uint32_t exact_list_len(const ExactArgs &a) { return a.n_list_dev ? __ldg(a.n_list_dev) : a.n_list; }
 __global__ void __launch_bounds__(kExactThreads) k_exact_reads(const __grid_constant__ ExactArgs a) {
     constexpr int kWarps = kExactThreads / 32;
     __shared__ int8_t diag[128];
@@ -1053,10 +1218,11 @@ __global__ void __launch_bounds__(kExactThreads) k_exact_reads(const __grid_cons
     __syncthreads();
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const unsigned below = (1u << lane) - 1u;
-    for (uint64_t base = (uint64_t)blockIdx.x * kExactThreads; base < a.n_list; base += (uint64_t)gridDim.x * kExactThreads) {
+    for (uint64_t base = (uint64_t)blockIdx.x * kExactThreads; base < exact_list_len(a); base += (uint64_t)gridDim.x * kExactThreads) {
+        const uint32_t n_list = exact_list_len(a);
         const uint64_t t = base + threadIdx.x;
         uint32_t r = 0; uint64_t b = 0; int L = 0, s = -1; score_t score = 0;
-        if (t < a.n_list) {
+        if (t < n_list) {
             r = a.list[t];
             s = exact_read_strand(a, diag, r, &b, &L, &score);
         }
@@ -1064,7 +1230,7 @@ __global__ void __launch_bounds__(kExactThreads) k_exact_reads(const __grid_cons
         uint32_t inc = bytes;                                          // inclusive prefix sum over the warp
         #pragma unroll
         for (int d = 1; d < 32; d <<= 1) { const uint32_t o = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += o; }
-        const unsigned left = __ballot_sync(0xffffffffu, t < a.n_list && s < 0);
+        const unsigned left = __ballot_sync(0xffffffffu, t < n_list && s < 0);
         if (lane == 31) s_bytes[w] = inc;
         if (lane == 0) s_left[w] = (uint32_t)__popc(left);
         __syncthreads();
@@ -1103,6 +1269,72 @@ cudaError_t launch_exact_reads(int num_sms, cudaStream_t s, const ExactArgs &a) 
     const uint64_t need = ((uint64_t)a.n_list + kExactThreads - 1) / kExactThreads;
     const uint64_t resident = (uint64_t)per_sm * num_sms;
     k_exact_reads<<<(unsigned)(need < resident ? need : resident), kExactThreads, 0, s>>>(a);
+    return cudaGetLastError();
+}
+
+// Exclusive prefix sum of v over the threads of the block, with one atomicAdd of the block's total to *ctr: the thread's
+// share of what the atomic handed out. s_sum / s_base: kWarps words of shared memory each.
+template <int kWarps, class C>
+__device__ __forceinline__ C tile_alloc(uint32_t v, C *ctr, uint32_t *s_sum, C *s_base) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    uint32_t inc = v;
+    #pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t o = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += o; }
+    if (lane == 31) s_sum[w] = inc;
+    __syncthreads();
+    if (w == 0) {
+        const uint32_t x = lane < kWarps ? s_sum[lane] : 0u;
+        uint32_t xi = x;
+        #pragma unroll
+        for (int d = 1; d < kWarps; d <<= 1) { const uint32_t o = __shfl_up_sync(0xffffffffu, xi, d); if (lane >= d) xi += o; }
+        const uint32_t total = __shfl_sync(0xffffffffu, xi, kWarps - 1);
+        C base = 0;
+        if (lane == 0 && total) base = atomicAdd(ctr, (C)total);
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (lane < kWarps) s_base[lane] = base + (xi - x);
+    }
+    __syncthreads();
+    return s_base[w] + (inc - v);
+}
+
+// Whole-read exact answers from the raw reads (exact_path_strand), in place of k_prepare, a tile of kPrepExactThreads
+// reads per block and round, one read per thread. The answered reads of a tile take one heap allocation (a record that
+// does not fit makes its read a left-over one), the left-over reads one append to a.list; then each warp writes its
+// answered records and prepares its left-over reads (prepare_read), one after the other, 32 lanes each. Persistent grid.
+static constexpr int kPrepExactThreads = 256;
+__global__ void __launch_bounds__(kPrepExactThreads) k_prepare_exact(const __grid_constant__ PrepExactArgs a) {
+    constexpr int kWarps = kPrepExactThreads / 32;
+    __shared__ unsigned long long s_off[kWarps];
+    __shared__ uint32_t s_bytes[kWarps], s_left[kWarps], s_slot[kWarps];
+    const int lane = threadIdx.x & 31;
+    const uint32_t n_reads = a.prep.n_reads;
+    for (uint64_t base = (uint64_t)blockIdx.x * kPrepExactThreads; base < n_reads; base += (uint64_t)gridDim.x * kPrepExactThreads) {
+        const uint32_t r = (uint32_t)(base + threadIdx.x);
+        uint64_t b = 0; int L = 0, s = -1; uint32_t p = 0; score_t score = 0;
+        if (r < n_reads) s = exact_path_strand(a, r, &b, &L, &p, &score);
+        const uint32_t bytes = s >= 0 ? exact_read_bytes(a.ex, L) : 0u;
+        const unsigned long long off = tile_alloc<kWarps>(bytes, a.ex.heap_used, s_bytes, s_off);
+        if (s >= 0 && off + bytes > a.ex.heap_cap) s = -1;
+        const bool left = r < n_reads && s < 0;
+        const uint32_t slot = tile_alloc<kWarps>(left ? 1u : 0u, a.n_list, s_left, s_slot);
+        if (left) a.list[slot] = r;
+        for (unsigned todo = __ballot_sync(0xffffffffu, s >= 0); todo; todo &= todo - 1) {
+            const int j = __ffs(todo) - 1;
+            exact_path_write(a, __shfl_sync(0xffffffffu, r, j), __shfl_sync(0xffffffffu, (unsigned long long)b, j),
+                             __shfl_sync(0xffffffffu, L, j), __shfl_sync(0xffffffffu, s, j), __shfl_sync(0xffffffffu, p, j),
+                             __shfl_sync(0xffffffffu, score, j), __shfl_sync(0xffffffffu, off, j), lane, 32);
+        }
+        for (unsigned todo = __ballot_sync(0xffffffffu, left); todo; todo &= todo - 1)
+            prepare_read(a.prep, __shfl_sync(0xffffffffu, r, __ffs(todo) - 1));
+    }
+}
+cudaError_t launch_prepare_exact(int num_sms, cudaStream_t s, const PrepExactArgs &a) {
+    int per_sm = 0;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_prepare_exact, kPrepExactThreads, 0);
+    if (e != cudaSuccess) return e;
+    const uint64_t need = ((uint64_t)a.prep.n_reads + kPrepExactThreads - 1) / kPrepExactThreads;
+    const uint64_t resident = (uint64_t)per_sm * num_sms;
+    k_prepare_exact<<<(unsigned)(need < resident ? need : resident), kPrepExactThreads, 0, s>>>(a);
     return cudaGetLastError();
 }
 // round r (0-based) brings character k - 3 - r of every edge's k-mer to c_nxt[e]; kmer_shift = 2 * (k - 3 - r)
