@@ -58,7 +58,7 @@ typedef struct mgb_results mgb_results_t;
 /* DBGAlignerConfig (aligner_config.hpp:23-61). Penalties are negative as in the struct
  * (cli/align.cpp:33-69 negates the positive CLI values). */
 typedef struct mgb_config {
-    uint64_t num_alternative_paths;
+    uint64_t num_alternative_paths;   /* 1..32 (--align-alternative-alignments); larger: MGB_ERR_UNSUPPORTED */
     uint64_t min_seed_length;
     uint64_t max_seed_length;
     uint64_t max_num_seeds_per_locus;

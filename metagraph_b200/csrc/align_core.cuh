@@ -60,7 +60,8 @@ struct DevConfig {
     uint32_t exact_shortcut;           // the scores allow the exact-path shortcut (lower_config) and it is not switched off
 };
 
-static constexpr int kMaxAlt = 4;            // supported num_alternative_paths
+// largest num_alternative_paths served: the aggregator keeps one entry per lane of the warp that aligns the read
+static constexpr int kMaxAlt = 32;
 static constexpr int kMaxOut = kMaxSigma;     // max outgoing edges handled per column
 
 enum ReadStatus : uint32_t { MGB_READ_OK = 0, MGB_READ_OVERFLOW = 1 };
@@ -75,6 +76,7 @@ struct Caps {
     uint32_t max_conv_cells;
     uint32_t max_seeds;        // per strand
     uint32_t aln_nodes, aln_seq, aln_cigar;   // per alignment slot
+    uint32_t n_alt;            // num_alternative_paths: the arena holds 3 * n_alt + 2 alignment slots
 };
 
 // Cells of a column in the DP table arena (ColMeta::fmt):
@@ -122,6 +124,10 @@ struct AlnHdr {
 
 struct AlnSlot { AlnHdr *h; uint64_t *nodes; char *seq; uint32_t *cigar; };
 
+// An aggregator entry's key, kept on chip: the fields LocalAlignmentLess orders by (score, query length, orientation,
+// clipping) and the header fields Alignment::operator== compares before the arrays.
+struct AggKey { int32_t score, q_len; uint32_t orientation; int32_t clip; uint32_t offset; int32_t seq_len, n_cigar, n_nodes; };
+
 // Per-strand state. Lives in shared memory so that it can be indexed with a run-time strand
 // number without forcing the aligner object out of registers.
 struct StrandCtx {
@@ -166,8 +172,17 @@ enum EmuPath : int {
 };
 extern "C" unsigned long long mgb_emu_path_hits[EMU_N_PATHS];
 #define MGB_EMU_HIT(path) __atomic_fetch_add(&mgb_emu_path_hits[path], 1ull, __ATOMIC_RELAXED)
+// host emulation (tests) only: what the aggregator did with an alignment offered to it (mgb_emu_agg_hits[EmuAgg])
+enum EmuAgg : int {
+    EMU_AGG_REPLACE,          // it took the slot of the smallest entry of a full aggregator
+    EMU_AGG_DUPLICATE,        // it was dropped as equal to an entry
+    EMU_N_AGG
+};
+extern "C" unsigned long long mgb_emu_agg_hits[EMU_N_AGG];
+#define MGB_EMU_AGG(ev) __atomic_fetch_add(&mgb_emu_agg_hits[ev], 1ull, __ATOMIC_RELAXED)
 #else
 #define MGB_EMU_HIT(path) ((void)0)
+#define MGB_EMU_AGG(ev) ((void)0)
 #endif
 
 #if defined(MGB_PHASE_TIMERS) && MGB_DEVICE_CODE
@@ -180,8 +195,9 @@ extern "C" unsigned long long mgb_emu_path_hits[EMU_N_PATHS];
 #define MGB_TOC(var, slot)
 #endif
 
-static constexpr int kNumSlots = 3 * kMaxAlt + 2;   // seed, ext[alt], bwd[alt], agg[alt], tmp
-enum { SLOT_SEED = 0, SLOT_TMP = 1, SLOT_EXT = 2, SLOT_BWD = 2 + kMaxAlt, SLOT_AGG = 2 + 2 * kMaxAlt };
+// alignment slots: seed, tmp, ext[n_alt], bwd[n_alt], agg[n_alt]; the first bwd and agg slots depend on the configuration
+// and are in WarpLayout (slot_bwd, slot_agg)
+enum { SLOT_SEED = 0, SLOT_TMP = 1, SLOT_EXT = 2 };
 
 // ------------------------------------------------------------------------------------
 // Arena carving (shared by host sizing code and the kernel)
@@ -219,6 +235,7 @@ void chain_entry(const IndexView &ix, const DevConfig &cfg, const Caps &caps, co
 struct WarpLayout {
     uint64_t cols, cells, heap, next_nodes, starts, conv_slots[2], conv_cells[2], seeds[2], psum[2];
     uint64_t slot0, slot_stride, slot_nodes, slot_seq, slot_cigar;      // alignment slot s starts at slot0 + s * slot_stride
+    uint32_t slot_bwd, slot_agg;                                        // first slot of the bwd[] and agg[] groups
     uint64_t bt_ops, bt_path, bt_seq;
     uint64_t sfx_min;       // per query position: current min_seed_length (SuffixSeeder)
     uint64_t sfx_first, sfx_last, sfx_len;   // index_range result per query position
@@ -249,7 +266,9 @@ struct WarpLayout {
         slot_seq = take(c.aln_seq) - slot0;
         slot_cigar = take(4 * (size_t)c.aln_cigar) - slot0;
         slot_stride = o - slot0;
-        o = slot0 + slot_stride * kNumSlots;
+        slot_bwd = 2 + c.n_alt;
+        slot_agg = 2 + 2 * c.n_alt;
+        o = slot0 + slot_stride * (2 + 3 * (size_t)c.n_alt);
         bt_ops = take(4 * (size_t)c.aln_cigar);
         bt_path = take(8 * (size_t)c.aln_nodes);
         bt_seq = take(c.aln_seq);
@@ -295,13 +314,14 @@ struct WarpMem {
 
 // Per-warp on-chip working set (shared memory on the device, a heap block in the host emulation), again as
 // offsets from the warp's base: two DP column buffers (parent / child ping-pong), the query strands and their
-// suffix sums, the best-first queue and the outgoing-edge scratch.
+// suffix sums, the best-first queue, the outgoing-edge scratch and the aggregator's keys.
 struct SmemLayout {
     int bmax, lq, hcap;       // column buffer cells; staged query capacity in characters (0: not staged); queue entries
     uint32_t buf0, psum0, psum1, q0, q1, ctx, mask0, mask1, heap, nn, out_nodes, out_scores, out_chars, total;
+    uint32_t agg, agg_ord;    // AggKey per aggregator entry; the entries in output order (run())
     uint32_t prof0, prof1;    // DNA block layout only: per query position the scores against A, C, G, T, one byte each
     uint32_t has_prof;
-    MGB_HOSTDEV size_t carve(int bmax_, int lq_, int hcap_, bool with_prof = false) {
+    MGB_HOSTDEV size_t carve(int bmax_, int lq_, int hcap_, int n_alt, bool with_prof = false) {
         size_t o = 0;
         auto take = [&](size_t bytes) { size_t r = o; o += align_up(bytes); return (uint32_t)r; };
         bmax = bmax_; lq = lq_; hcap = hcap_;
@@ -314,6 +334,7 @@ struct SmemLayout {
         nn = take(sizeof(HeapItem) * hcap);
         out_nodes = take(8 * kMaxOut);
         out_scores = take(4 * kMaxOut); out_chars = take(kMaxOut);
+        agg = take(sizeof(AggKey) * (size_t)n_alt); agg_ord = take(4 * (size_t)n_alt);
         has_prof = with_prof && lq > 0 ? 1u : 0u;
         prof0 = prof1 = 0;
         if (has_prof) { prof0 = take(4 * ((size_t)lq + 8)); prof1 = take(4 * ((size_t)lq + 8)); }
@@ -339,6 +360,8 @@ struct WarpSmem {
     MGB_HD uint64_t* out_nodes() const { return (uint64_t*)(base + lay->out_nodes); }
     MGB_HD int32_t* out_scores() const { return (int32_t*)(base + lay->out_scores); }
     MGB_HD uint8_t* out_chars() const { return (uint8_t*)(base + lay->out_chars); }
+    MGB_HD AggKey* agg() const { return (AggKey*)(base + lay->agg); }
+    MGB_HD int32_t* agg_ord() const { return (int32_t*)(base + lay->agg_ord); }
     MGB_HD uint32_t* prof4(int s) const { return (uint32_t*)(base + (s ? lay->prof1 : lay->prof0)); }
 };
 
@@ -3089,50 +3112,94 @@ struct ReadAligner {
 
     // --------------------------------------------------------------------------------
     // aggregator (aligner_aggregator.hpp:59-149, unlabeled queue)
+    // Entry i lives in slot lay->slot_agg + i and its key in sm.agg()[i]: on the device lane i owns entry i (n_agg <=
+    // kMaxAlt = kWarp), so a question about all entries is one pass and one warp collective; the one-lane emulation
+    // runs the same loops over all entries.
     // --------------------------------------------------------------------------------
-    MGB_HD bool aln_less(const AlnSlot &a, const AlnSlot &b) const {     // LocalAlignmentLess
-        int as = a.h->score, bs = b.h->score;
-        if (bs != as) return bs > as;
-        int aq = a.h->q_len, bq = b.h->q_len;
-        if (aq != bq) return aq > bq;
-        int ao = a.h->orientation, bo = b.h->orientation;
-        if (ao != bo) return ao > bo;
-        return aln_clipping(a) > aln_clipping(b);
+    MGB_HD static bool key_less(const AggKey &a, const AggKey &b) {      // LocalAlignmentLess
+        if (a.score != b.score) return b.score > a.score;
+        if (a.q_len != b.q_len) return a.q_len > b.q_len;
+        if (a.orientation != b.orientation) return a.orientation > b.orientation;
+        return a.clip > b.clip;
     }
-    MGB_HD bool aln_equal(const AlnSlot &a, const AlnSlot &b) {
-        const AlnHdr x = *a.h, y = *b.h;
-        if (x.orientation != y.orientation || x.offset != y.offset || x.score != y.score
-                || x.q_len != y.q_len || x.seq_len != y.seq_len || x.n_cigar != y.n_cigar
-                || x.n_nodes != y.n_nodes)
-            return false;
+    MGB_HD static bool key_same_hdr(const AggKey &a, const AggKey &b) {  // operator=='s fields before the arrays
+        return a.orientation == b.orientation && a.offset == b.offset && a.score == b.score && a.q_len == b.q_len
+            && a.seq_len == b.seq_len && a.n_cigar == b.n_cigar && a.n_nodes == b.n_nodes;
+    }
+    MGB_HD AggKey agg_key(const AlnSlot &a) const {
+        const AlnHdr h = *a.h;
+        AggKey k;
+        k.score = h.score; k.q_len = h.q_len; k.orientation = h.orientation; k.clip = aln_clipping(a);
+        k.offset = h.offset; k.seq_len = h.seq_len; k.n_cigar = h.n_cigar; k.n_nodes = h.n_nodes;
+        return k;
+    }
+    // Alignment::operator== for two alignments whose keys pass key_same_hdr: query views, sequences, CIGARs, node paths
+    MGB_HD bool aln_same_arrays(const AlnSlot &a, const AggKey &x, const AlnSlot &b, const AggKey &y) {
         bool diff = false;
-        int ca = aln_clipping(a), cb = aln_clipping(b);
         for (int i = wlane(); i < x.q_len; i += kWarp)
-            if (cx[x.orientation].q[ca + i] != cx[y.orientation].q[cb + i]) diff = true;
+            if (cx[x.orientation].q[x.clip + i] != cx[y.orientation].q[y.clip + i]) diff = true;
         for (int i = wlane(); i < x.seq_len; i += kWarp) if (a.seq[i] != b.seq[i]) diff = true;
         for (int i = wlane(); i < x.n_cigar; i += kWarp) if (a.cigar[i] != b.cigar[i]) diff = true;
         for (int i = wlane(); i < x.n_nodes; i += kWarp) if (a.nodes[i] != b.nodes[i]) diff = true;
         return !wballot(diff);
     }
+    // Position of entry i in a stable sort of the entries by LocalAlignmentLess: descending (get_alignments' order) or
+    // ascending (position 0 is the entry std::min_element returns, the first of the minimal ones). An entry j comes
+    // before i if it is strictly on i's side of the order or, being equivalent to i, has the lower index.
+    MGB_HD int agg_rank(int i, bool desc) const {
+        const AggKey *keys = sm.agg();
+        const AggKey a = keys[i];
+        int r = 0;
+        for (int j = 0; j < n_agg; ++j) {
+            if (j == i) continue;
+            const AggKey b = keys[j];
+            const AggKey &x = desc ? a : b, &y = desc ? b : a;
+            r += j < i ? !key_less(y, x) : key_less(x, y);
+        }
+        return r;
+    }
     MGB_HD score_t agg_global_cutoff() {
         if (!n_agg) return kNinf;
-        int mx = 0;
-        for (int i = 1; i < n_agg; ++i)
-            if (aln_less(m.slot(SLOT_AGG + mx), m.slot(SLOT_AGG + i))) mx = i;
-        score_t cur_max = m.slot(SLOT_AGG + mx).h->score;
+        // the score of std::max_element's entry is the largest score
+        score_t mx = INT32_MIN;
+        for (int i = wlane(); i < n_agg; i += kWarp) mx = imax(mx, sm.agg()[i].score);
+        const score_t cur_max = wreduce_max(mx);
         return cur_max > 0 ? (score_t)((double)cur_max * cfg.rel_score_cutoff) : cur_max;
     }
     MGB_HD void agg_add(int slot) {
-        if (!n_agg) { copy_slot(SLOT_AGG, slot); n_agg = 1; return; }
-        if (m.slot(slot).h->score < agg_global_cutoff()) return;
-        for (int i = 0; i < n_agg; ++i)
-            if (aln_equal(m.slot(slot), m.slot(SLOT_AGG + i))) return;
-        if (n_agg < (int)cfg.num_alternative_paths) { copy_slot(SLOT_AGG + n_agg, slot); ++n_agg; return; }
-        int mn = 0;
-        for (int i = 1; i < n_agg; ++i)
-            if (aln_less(m.slot(SLOT_AGG + i), m.slot(SLOT_AGG + mn))) mn = i;
-        if (aln_less(m.slot(slot), m.slot(SLOT_AGG + mn))) return;
-        copy_slot(SLOT_AGG + mn, slot);
+        const AlnSlot a = m.slot(slot);
+        const AggKey nk = agg_key(a);
+        AggKey *keys = sm.agg();
+        const int agg0 = (int)m.lay->slot_agg;
+        int dst = n_agg;
+        if (n_agg) {
+            if (nk.score < agg_global_cutoff()) return;
+            // duplicates: a ballot of the entries whose header fields match, then the arrays of those only
+            uint32_t cand = 0;
+            for (int b = 0; b < n_agg; b += kWarp) {             // one pass on the device
+                const int i = b + wlane();
+                cand |= wballot(i < n_agg && key_same_hdr(keys[i], nk)) << b;
+            }
+            for (; cand; cand &= cand - 1) {
+                const int i = ffs32(cand) - 1;
+                if (aln_same_arrays(a, nk, m.slot(agg0 + i), keys[i])) { MGB_EMU_AGG(EMU_AGG_DUPLICATE); return; }
+            }
+            if (n_agg == (int)cfg.num_alternative_paths) {
+                // *std::min_element(q_, cmp_) = alignment, unless alignment is smaller still
+                uint32_t first = 0;
+                for (int b = 0; b < n_agg; b += kWarp) {
+                    const int i = b + wlane();
+                    first |= wballot(i < n_agg && agg_rank(i, false) == 0) << b;
+                }
+                dst = ffs32(first) - 1;
+                if (key_less(nk, keys[dst])) return;
+                MGB_EMU_AGG(EMU_AGG_REPLACE);
+            }
+        }
+        copy_slot(agg0 + dst, slot);
+        keys[dst] = nk;
+        if (dst == n_agg) ++n_agg;
+        wsync();
     }
     MGB_HD score_t get_min_path_score() { return imax(cfg.min_path_score, agg_global_cutoff()); }
 
@@ -3183,6 +3250,7 @@ struct ReadAligner {
             // spawns): the extender is by far the largest piece of code and must exist once.
             // A backward seed dropped by an earlier backward extension stays in its slot, unused: extend() does
             // nothing for it.
+            const int bwd0 = (int)m.lay->slot_bwd;
             int n_rc = 0;
             for (int it = 0; !overflow && it <= n_rc; ++it) {
                 const int r = it - 1;
@@ -3195,12 +3263,12 @@ struct ReadAligner {
                     seed_is_query = false;
                 }
                 const int n_ext = extend(it ? be : fe, it ? SLOT_EXT + r : SLOT_SEED,
-                                         (ext_ok && it) ? get_min_path_score() : mps_fwd, it != 0, it ? SLOT_BWD : SLOT_EXT);
+                                         (ext_ok && it) ? get_min_path_score() : mps_fwd, it != 0, it ? bwd0 : SLOT_EXT);
                 // results of this extension: one loop (and one agg_add site: the aggregator's comparison
                 // code is large) for the forward case (aggregate, then reverse-complement the clipped
                 // ones for the backward pass) and the backward case (reverse-complement back, then aggregate)
                 for (int r0 = 0; ext_ok && !overflow && r0 < n_ext; ++r0) {
-                    const int slot = (it ? SLOT_BWD : SLOT_EXT) + r0;
+                    const int slot = (it ? bwd0 : SLOT_EXT) + r0;
                     // is_reversible (:652-656): on a CANONICAL-mode graph an alignment to the reverse strand
                     // with no offset is reported as its reverse complement
                     const bool reversible = MGB_CANONICAL(cfg) && m.slot(slot).h->orientation && !m.slot(slot).h->offset;
@@ -3340,12 +3408,12 @@ struct ReadAligner {
         wsync();
     }
 
-    // whole pipeline for one read; returns the number of alignments left in SLOT_AGG.. (sorted)
+    // whole pipeline for one read; returns the number of aggregator entries, sm.agg_ord() lists them in output order
     // optional: per-position index_range results of both strands (k_subk), set before run()
     const uint32_t *subk_first[2] = { nullptr, nullptr }, *subk_last[2] = { nullptr, nullptr };
     const uint8_t *subk_len[2] = { nullptr, nullptr };
     MGB_HD int run(int L_, const char *qf, const char *qr, const uint8_t *cf, const uint8_t *cr,
-                   const uint64_t *nf, const uint64_t *nr, int *order) {
+                   const uint64_t *nf, const uint64_t *nr) {
         MGB_TIC(t_setup);
         L = L_;
         overflow = false; n_agg = 0; seed_is_query = false;
@@ -3420,15 +3488,9 @@ struct ReadAligner {
         if (overflow) return 0;
         stats.num_extensions += cx[0].num_ext + cx[1].num_ext;
         stats.num_explored_nodes += cx[0].explored_prev + cx[0].conv_n + cx[1].explored_prev + cx[1].conv_n;
-        // AlignmentAggregator::get_alignments: descending LocalAlignmentLess order
-        for (int i = 0; i < n_agg; ++i) order[i] = i;
-        for (int i = 1; i < n_agg; ++i) {
-            int x = order[i], j = i - 1;
-            while (j >= 0 && aln_less(m.slot(SLOT_AGG + order[j]), m.slot(SLOT_AGG + x))) {
-                order[j + 1] = order[j]; --j;
-            }
-            order[j + 1] = x;
-        }
+        // AlignmentAggregator::get_alignments: descending LocalAlignmentLess order, ties in entry order
+        for (int i = wlane(); i < n_agg; i += kWarp) sm.agg_ord()[agg_rank(i, true)] = i;
+        wsync();
         return n_agg;
     }
 };

@@ -1153,7 +1153,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             if (const char *e = std::getenv("MGB_TEST_BMAX")) bmax_v = std::atoi(e);
             if (const char *e = std::getenv("MGB_TEST_HCAP")) hcap = std::atoi(e);
             SmemLayout slay;
-            const size_t smem_per_warp = slay.carve(bmax_v, lq_v, hcap, !index->view.wide);
+            const size_t smem_per_warp = slay.carve(bmax_v, lq_v, hcap, (int)dcfg.num_alternative_paths, !index->view.wide);
             DevBufs pass_bufs(st, wsg.w, 32);          // slot 32: the arena
 #if defined(MGB_HOST_EMU)
             uint32_t n_warps = 1;
@@ -1190,8 +1190,8 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             }
             if (n_warps64 > ((uint64_t)list.size() + wpb - 1) / wpb * wpb) n_warps64 = ((uint64_t)list.size() + wpb - 1) / wpb * wpb;
             uint32_t n_warps = (uint32_t)n_warps64;
-            if (dbg_time) std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident)\n", n_warps,
-                                       (unsigned long long)index->num_sms * blocks_per_sm * wpb);
+            if (dbg_time) std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident), arena %zu bytes per warp\n",
+                                       n_warps, (unsigned long long)index->num_sms * blocks_per_sm * wpb, stride);
 #endif
             // pass 0 after k_prepare_exact: its heap, counters and list of reads left over are in place already
             const bool listed = pass == 0 && prep_exact;
@@ -1371,7 +1371,8 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
 
 static std::atomic<uint32_t> g_max_pieces{0};      // 0 = automatic
 #if defined(MGB_HOST_EMU)
-extern "C" { unsigned long long mgb_emu_whole_read_hits = 0, mgb_emu_path_read_hits = 0; unsigned long long mgb_emu_path_hits[EMU_N_PATHS] = {}; }
+extern "C" { unsigned long long mgb_emu_whole_read_hits = 0, mgb_emu_path_read_hits = 0; unsigned long long mgb_emu_path_hits[EMU_N_PATHS] = {};
+             unsigned long long mgb_emu_agg_hits[EMU_N_AGG] = {}; }
 #endif
 
 extern "C" {

@@ -184,6 +184,7 @@ inline Caps choose_caps(uint32_t L_max, const DevConfig &d, uint32_t k, uint32_t
     c.aln_nodes = scale * (3 * L + 128 + k);
     c.aln_seq = scale * (3 * L + 128 + 2 * k);
     c.aln_cigar = scale * (2 * L + 64);
+    c.n_alt = d.num_alternative_paths;
     return c;
 }
 

@@ -149,7 +149,6 @@ MGB_HD void align_read(const AlignArgs &a, uint32_t r, const WarpMem &mem, const
     al.use_fast = a.use_fast != 0;
     const uint64_t b = a.offsets[r];
     const int L = (int)(a.offsets[r + 1] - b);
-    int order[kMaxAlt];
     const bool has_k = L >= (int)a.ix.k;
     if (a.sub_len_f) {
         al.subk_first[0] = a.sub_first_f + b; al.subk_last[0] = a.sub_last_f + b; al.subk_len[0] = a.sub_len_f + b;
@@ -158,7 +157,7 @@ MGB_HD void align_read(const AlignArgs &a, uint32_t r, const WarpMem &mem, const
     const uint64_t ko = has_k ? a.koff[r] : 0;
     int n = al.run(L, a.qf + b, a.qr + b, a.cf + b, a.cr + b,
                    has_k ? a.nodes_f + ko : nullptr,
-                   has_k && a.cfg.forward_and_reverse_complement ? a.nodes_r + ko : nullptr, order);
+                   has_k && a.cfg.forward_and_reverse_complement ? a.nodes_r + ko : nullptr);
 #if defined(MGB_PHASE_TIMERS) && MGB_DEVICE_CODE
     if (wlane() == 0 && a.phase_out) {
         for (int p = 0; p < 8; ++p) atomicAdd((unsigned long long*)a.phase_out + p, (unsigned long long)al.phase_cycles[p]);
@@ -168,12 +167,14 @@ MGB_HD void align_read(const AlignArgs &a, uint32_t r, const WarpMem &mem, const
     h.status = al.overflow ? MGB_READ_OVERFLOW : MGB_READ_OK;
     h.n_aln = 0; h.heap_off = 0; h.stats = al.stats;
     if (!al.overflow && n) {
-        // bytes: per alignment OutAln + nodes*8 + cigar*4 + seq (padded to 8)
+        // bytes: per alignment OutAln + nodes*8 + cigar*4 + seq (padded to 8), from the aggregator's keys on chip
+        const AggKey *keys = sm.agg();
+        const int32_t *ord = sm.agg_ord();
         uint64_t bytes = 0;
         for (int i = 0; i < n; ++i) {
-            const AlnHdr ah = *mem.slot(SLOT_AGG + order[i]).h;
-            bytes += sizeof(OutAln) + (a.cfg.result_nodes ? 0ull : 8ull * ah.n_nodes) + ((4ull * ah.n_cigar + 7) & ~7ull)
-                   + (((uint64_t)ah.seq_len + 7) & ~7ull);
+            const AggKey ak = keys[i];
+            bytes += sizeof(OutAln) + (a.cfg.result_nodes ? 0ull : 8ull * ak.n_nodes) + ((4ull * ak.n_cigar + 7) & ~7ull)
+                   + (((uint64_t)ak.seq_len + 7) & ~7ull);
         }
         unsigned long long off = 0;
 #if MGB_DEVICE_CODE
@@ -188,24 +189,24 @@ MGB_HD void align_read(const AlignArgs &a, uint32_t r, const WarpMem &mem, const
             h.n_aln = n; h.heap_off = off;
             char *p = a.heap + off;
             for (int i = 0; i < n; ++i) {
-                const AlnSlot sl = mem.slot(SLOT_AGG + order[i]);
-                const AlnHdr ah = *sl.h;
+                const AlnSlot sl = mem.slot(a.lay.slot_agg + ord[i]);
+                const AggKey ak = keys[ord[i]];
                 OutAln o;
-                o.orientation = ah.orientation; o.score = ah.score; o.offset = ah.offset;
-                o.query_begin = al.aln_clipping(sl); o.query_len = ah.q_len;
-                o.n_nodes = ah.n_nodes; o.seq_len = ah.seq_len; o.n_cigar = ah.n_cigar;
+                o.orientation = ak.orientation; o.score = ak.score; o.offset = ak.offset;
+                o.query_begin = ak.clip; o.query_len = ak.q_len;
+                o.n_nodes = ak.n_nodes; o.seq_len = ak.seq_len; o.n_cigar = ak.n_cigar;
                 if (wlane() == 0) *(OutAln*)p = o;
                 p += sizeof(OutAln);
                 if (!a.cfg.result_nodes) {
                     uint64_t *pn = (uint64_t*)p;
-                    for (int t = wlane(); t < ah.n_nodes; t += kWarp) pn[t] = sl.nodes[t];
-                    p += 8ull * ah.n_nodes;
+                    for (int t = wlane(); t < ak.n_nodes; t += kWarp) pn[t] = sl.nodes[t];
+                    p += 8ull * ak.n_nodes;
                 }
                 uint32_t *pc = (uint32_t*)p;
-                for (int t = wlane(); t < ah.n_cigar; t += kWarp) pc[t] = sl.cigar[t];
-                p += (4ull * ah.n_cigar + 7) & ~7ull;
-                for (int t = wlane(); t < ah.seq_len; t += kWarp) p[t] = sl.seq[t];
-                p += ((uint64_t)ah.seq_len + 7) & ~7ull;
+                for (int t = wlane(); t < ak.n_cigar; t += kWarp) pc[t] = sl.cigar[t];
+                p += (4ull * ak.n_cigar + 7) & ~7ull;
+                for (int t = wlane(); t < ak.seq_len; t += kWarp) p[t] = sl.seq[t];
+                p += ((uint64_t)ak.seq_len + 7) & ~7ull;
             }
         }
     }
