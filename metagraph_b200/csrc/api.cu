@@ -766,7 +766,8 @@ int launch_prepare(const mgb_index_t *index, const Batch &b, Stream &st, int num
     for (uint32_t r = 0; r < b.n_reads; ++r) prepare_read(a, r);
 #else
     if (!b.n_reads) return 0;
-    int blocks = std::min<uint64_t>((b.n_reads + 7) / 8, (uint64_t)num_sms * 8);
+    const unsigned blocks = (unsigned)kern_dna::read_path_grid(std::min<uint64_t>((b.n_reads + 7) / 8, (uint64_t)num_sms * 8));
+    kern_dna::log_launch("k_prepare", blocks, 256, (uint64_t)blocks * 8, b.n_reads);     // a warp per read
     kern_dna::k_prepare<<<blocks, 256, 0, st.s>>>(a);
     CUDA_TRY(cudaGetLastError());
 #endif
@@ -1189,9 +1190,8 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
                 if (n_warps64 > mem_warps) n_warps64 = mem_warps / wpb * wpb;
             }
             if (n_warps64 > ((uint64_t)list.size() + wpb - 1) / wpb * wpb) n_warps64 = ((uint64_t)list.size() + wpb - 1) / wpb * wpb;
+            n_warps64 = kern_dna::read_path_grid(n_warps64 / wpb) * wpb;    // (MGB_TEST_MAX_BLOCKS)
             uint32_t n_warps = (uint32_t)n_warps64;
-            if (dbg_time) std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident), arena %zu bytes per warp\n",
-                                       n_warps, (unsigned long long)index->num_sms * blocks_per_sm * wpb, stride);
 #endif
             // pass 0 after k_prepare_exact: its heap, counters and list of reads left over are in place already
             const bool listed = pass == 0 && prep_exact;
@@ -1254,7 +1254,8 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
                 CUDA_TRY(cudaStreamSynchronize(st.s));
 #endif
                 if (listed && dbg_time)
-                    std::fprintf(stderr, "[mgb] reads %u+%u k_prepare_exact answered %u\n", lo, n_reads, n_reads - n_rest[1]);
+                    std::fprintf(stderr, "[mgb] reads %u+%u k_prepare_exact answered %u, left over %u\n", lo, n_reads,
+                                 n_reads - n_rest[1], n_rest[1]);
                 a.read_list = d_rest; a.n_list = n_rest[0];
                 res->stats.kernel_launches += 1;
             }
@@ -1266,8 +1267,15 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             for (uint32_t t = 0; t < a.n_list; ++t) align_read(a, a.read_list[t], mem_emu, sm_emu);
             used = *d_used;
 #else
+            const uint32_t grid = (uint32_t)(std::min<uint64_t>(n_warps, ((uint64_t)a.n_list + wpb - 1) / wpb * wpb) / wpb);
+            if (dbg_time) {         // every pass; per_round: warps launched, each aligning one read of the list at a time
+                char launched[128] = "";          // (one fprintf: pieces on two host threads print at once)
+                if (a.n_list) std::snprintf(launched, sizeof(launched), "; launch k_align grid=%u block=%d per_round=%llu items=%u",
+                                            grid, kern_dna::kAlignThreads, (unsigned long long)grid * wpb, a.n_list);
+                std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident), arena %zu bytes per warp%s\n", n_warps,
+                             (unsigned long long)index->num_sms * blocks_per_sm * wpb, stride, launched);
+            }
             if (a.n_list) {
-                const uint32_t grid = (uint32_t)(std::min<uint64_t>(n_warps, ((uint64_t)a.n_list + wpb - 1) / wpb * wpb) / wpb);
                 CUDA_TRY(index->view.wide ? kern_any::launch_align(grid, smem_block, st.s, a)
                        : index->view.mode != 0 ? kern_canon::launch_align(grid, smem_block, st.s, a)
                                                : kern_dna::launch_align(grid, smem_block, st.s, a));

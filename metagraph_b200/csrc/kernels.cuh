@@ -12,6 +12,8 @@
 #include "align_core.cuh"
 #if !defined(MGB_HOST_EMU)
 #include <cuda_runtime.h>
+#include <cstdio>
+#include <cstdlib>
 #endif
 
 #ifndef MGB_KERNEL_NS
@@ -1153,16 +1155,50 @@ __global__ void __launch_bounds__(kAlignThreads, MGB_ALIGN_MIN_BLOCKS) k_align(c
     }
 }
 
+// Grid of a read-path kernel (k_prepare, k_prepare_exact, k_premap, k_seed, k_seed_hash, k_subk, k_exact_reads, k_align):
+// `blocks`, or fewer under MGB_TEST_MAX_BLOCKS=n (test knob: at most n blocks, so that the kernels' persistent and
+// grid-stride loops run several rounds on small inputs). Read on every launch; host code only.
+static inline uint64_t read_path_grid(uint64_t blocks) {
+    if (const char *e = std::getenv("MGB_TEST_MAX_BLOCKS")) {
+        const long long n = std::atoll(e);
+        if (n > 0 && (uint64_t)n < blocks) blocks = (uint64_t)n;
+    }
+    return blocks;
+}
+// MGB_DEBUG=1: one line per read-path launch on stderr: the grid, the threads per block, the items (reads, strands,
+// 32-position blocks of a strand) one round of the kernel's loop covers and, when the host knows it, the number of items
+// (items=dev: a length the device holds)
+static inline void log_launch(const char *kernel, uint64_t grid, int threads, uint64_t per_round, long long items) {
+    if (!std::getenv("MGB_DEBUG")) return;
+    char n[24];
+    if (items >= 0) std::snprintf(n, sizeof(n), "%lld", items); else std::snprintf(n, sizeof(n), "dev");
+    std::fprintf(stderr, "[mgb] launch %s grid=%llu block=%d per_round=%llu items=%s\n", kernel,
+                 (unsigned long long)grid, threads, (unsigned long long)per_round, n);
+}
+
 // launchers (the only entry points the host code uses)
 #if !defined(MGB_ALIGN_KERNEL_ONLY)
 cudaError_t launch_radj_bwd(unsigned grid, const RadjArgs &a) { k_radj_bwd<<<grid, 128>>>(a); return cudaGetLastError(); }
 cudaError_t launch_sfx_extend(unsigned grid, const SfxArgs &a) { k_sfx_extend<<<grid, 128>>>(a); return cudaGetLastError(); }
 cudaError_t launch_subk(unsigned grid, cudaStream_t s, const SubkArgs &a, uint32_t chunks_per_strand) {
+    grid = (unsigned)read_path_grid(grid);
+    log_launch("k_subk", grid, 128, (uint64_t)grid * 4,          // one warp per 32 positions of a strand
+               (long long)a.n_reads * a.n_strands * ((chunks_per_strand * (uint32_t)kSubkChunk + 31) / 32));
     k_subk<<<grid, 128, 0, s>>>(a, chunks_per_strand);
     return cudaGetLastError();
 }
-cudaError_t launch_premap(unsigned grid, cudaStream_t s, const SeedArgs &a) { k_premap<<<grid, 256, 0, s>>>(a); return cudaGetLastError(); }
-cudaError_t launch_seed(unsigned grid, cudaStream_t s, const SeedArgs &a) { k_seed<<<grid, 128, 0, s>>>(a); return cudaGetLastError(); }
+cudaError_t launch_premap(unsigned grid, cudaStream_t s, const SeedArgs &a) {
+    grid = (unsigned)read_path_grid(grid);
+    log_launch("k_premap", grid, 256, (uint64_t)grid * 8, (long long)a.n_reads * a.n_strands);     // a warp per strand
+    k_premap<<<grid, 256, 0, s>>>(a);
+    return cudaGetLastError();
+}
+cudaError_t launch_seed(unsigned grid, cudaStream_t s, const SeedArgs &a) {
+    grid = (unsigned)read_path_grid(grid);
+    log_launch("k_seed", grid, 128, (uint64_t)grid * 128, (long long)a.n_reads * a.n_strands);     // a lane per strand
+    k_seed<<<grid, 128, 0, s>>>(a);
+    return cudaGetLastError();
+}
 #if !defined(MGB_WIDE_ONLY)
 // persistent grid: as many blocks as are resident at once, or fewer when the reads do not fill them
 cudaError_t launch_seed_hash(int num_sms, cudaStream_t s, const SeedArgs &a) {
@@ -1171,7 +1207,9 @@ cudaError_t launch_seed_hash(int num_sms, cudaStream_t s, const SeedArgs &a) {
     if (e != cudaSuccess) return e;
     const uint64_t need = ((uint64_t)a.n_reads + kSeedThreads - 1) / kSeedThreads;     // one read per lane
     const uint64_t resident = (uint64_t)per_sm * num_sms;
-    k_seed_hash<<<(unsigned)(need < resident ? need : resident), kSeedThreads, 0, s>>>(a);
+    const unsigned grid = (unsigned)read_path_grid(need < resident ? need : resident);
+    log_launch("k_seed_hash", grid, kSeedThreads, (uint64_t)grid * kSeedThreads, a.list ? -1 : (long long)a.n_reads);
+    k_seed_hash<<<grid, kSeedThreads, 0, s>>>(a);
     return cudaGetLastError();
 }
 #endif
@@ -1269,7 +1307,10 @@ cudaError_t launch_exact_reads(int num_sms, cudaStream_t s, const ExactArgs &a) 
     if (e != cudaSuccess) return e;
     const uint64_t need = ((uint64_t)a.n_list + kExactThreads - 1) / kExactThreads;
     const uint64_t resident = (uint64_t)per_sm * num_sms;
-    k_exact_reads<<<(unsigned)(need < resident ? need : resident), kExactThreads, 0, s>>>(a);
+    const unsigned grid = (unsigned)read_path_grid(need < resident ? need : resident);
+    log_launch("k_exact_reads", grid, kExactThreads, (uint64_t)grid * kExactThreads,
+               a.n_list_dev ? -1 : (long long)a.n_list);
+    k_exact_reads<<<grid, kExactThreads, 0, s>>>(a);
     return cudaGetLastError();
 }
 
@@ -1335,7 +1376,9 @@ cudaError_t launch_prepare_exact(int num_sms, cudaStream_t s, const PrepExactArg
     if (e != cudaSuccess) return e;
     const uint64_t need = ((uint64_t)a.prep.n_reads + kPrepExactThreads - 1) / kPrepExactThreads;
     const uint64_t resident = (uint64_t)per_sm * num_sms;
-    k_prepare_exact<<<(unsigned)(need < resident ? need : resident), kPrepExactThreads, 0, s>>>(a);
+    const unsigned grid = (unsigned)read_path_grid(need < resident ? need : resident);
+    log_launch("k_prepare_exact", grid, kPrepExactThreads, (uint64_t)grid * kPrepExactThreads, a.prep.n_reads);
+    k_prepare_exact<<<grid, kPrepExactThreads, 0, s>>>(a);
     return cudaGetLastError();
 }
 // round r (0-based) brings character k - 3 - r of every edge's k-mer to c_nxt[e]; kmer_shift = 2 * (k - 3 - r)

@@ -178,7 +178,7 @@ EXACT_SHORTCUT_CASES = [
     (107, 19, lambda k: cli_defaults(k, num_alternative_paths=2)),                  # two reported paths: no shortcut
 ]
 
-def whole_read_case(lib, seed, k, cfg, G=2500, L=70):
+def whole_read_case(lib, seed, k, cfg, G=2500, L=70, n_path=40):
     """Reads around the whole-read form of the exact-path shortcut (exact seeder, both strands): reads that are paths
     of the graph on either strand, reads whose other strand has k-mers in the graph as well (the graph holds a region
     and its reverse complement; palindromes), reads of length k and k - 1, reads with an 'N' or one wrong base, a read
@@ -193,7 +193,7 @@ def whole_read_case(lib, seed, k, cfg, G=2500, L=70):
     g = O.OracleGraph(k, seqs)
     idx = DBGSuccinctIndex(BOSSTable.from_sequences(k, seqs, lib=lib), lib=lib)
     reads = []
-    for i in range(40):
+    for i in range(n_path):
         p = int(rng.integers(0, G - L))
         r = base[p:p + L]
         reads.append(r.translate(COMP)[::-1] if i % 2 else r)
@@ -563,7 +563,7 @@ def check_mt_primary(lib, **kw):
     return got
 
 
-def fuzz_case(lib, seed, canonical=False, primary=False, k=None):
+def fuzz_case(lib, seed, canonical=False, primary=False, k=None, nreads=25, threads=1):
     """One randomized (graph, reads, config) triple: k, graph shape (variants, repeats, dummy mask), scoring
     matrix, gap penalties, xdrop, seed lengths (exact / MEM / sub-k), seeds per locus, alternative paths,
     strands, end bonuses, cut-offs, node budget, left trim, complexity filter. Returns the mismatching reads."""
@@ -608,7 +608,7 @@ def fuzz_case(lib, seed, canonical=False, primary=False, k=None):
                            mode=2 if primary else 1 if canonical else 0)
     seqs = read_src
     reads = []
-    for i in range(25):
+    for i in range(nreads):
         s_ = seqs[int(rng.integers(0, len(seqs)))]
         L = int(rng.integers(max(3, k - 3), 160))
         p = int(rng.integers(0, max(1, len(s_) - L)))
@@ -617,7 +617,7 @@ def fuzz_case(lib, seed, canonical=False, primary=False, k=None):
         if rng.random() < 0.1 and len(r) > 5: r = r[:len(r)//2] + "N" + r[len(r)//2+1:]
         reads.append(r)
     try:
-        exp = g.align_tsv(cfg, reads, with_nodes=True)
+        exp = g.align_tsv(cfg, reads, with_nodes=True, threads=threads)
     except RuntimeError as err:                         # DBGAligner ctor: check_config_scores failed
         assert "too low" in str(err)
         import pytest
@@ -848,6 +848,8 @@ SPILL_KNOBS = (
     ("no_path_index", {"MGB_NO_PATH_INDEX": "1"}),
     ("wide", {"MGB_TEST_WIDE": "1"}),                                    # the alphabet-generic index layout
     ("pieces3", {"MGB_TEST_PIECES": "3"}),                               # retried reads in several pieces and heaps
+    ("grid1", {"MGB_TEST_MAX_BLOCKS": "1"}),                             # one block of each read-path kernel: k_align's
+                                                                         # 4 warps align every read, one after another
 )
 DP_COUNTERS = ("num_seeds", "num_extensions", "num_explored_nodes", "dp_cells", "dp_columns")
 

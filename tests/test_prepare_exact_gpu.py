@@ -76,7 +76,7 @@ class Graph:
 
 
 def run(idx, cfg, reads, route, monkeypatch, capfd):
-    """(TSV lines, counters, reads the route answered)"""
+    """(TSV lines, counters, reads the route answered, the MGB_DEBUG lines)"""
     if route:
         monkeypatch.delenv("MGB_TEST_NO_PREPARE_EXACT", raising=False)
     else:
@@ -90,11 +90,13 @@ def run(idx, cfg, reads, route, monkeypatch, capfd):
     monkeypatch.delenv("MGB_TEST_NO_PREPARE_EXACT", raising=False)
     lines = [format_alignment("", a, cfg.min_path_score, with_nodes=not cfg.result_nodes) for a in res]
     stats = al.last_stats
-    return lines, {c: stats[c] for c in COUNTERS}, sum(int(m) for m in re.findall(r"k_prepare_exact answered (\d+)", err))
+    return (lines, {c: stats[c] for c in COUNTERS}, sum(int(m) for m in re.findall(r"k_prepare_exact answered (\d+)", err)),
+            err)
 
 
-def check(g, reads, monkeypatch, capfd, expect=None):
-    """route on == route off == oracle, with and without node ids in the records; returns the reads the route answered"""
+def check(g, reads, monkeypatch, capfd, expect=None, runs=None):
+    """route on == route off == oracle, with and without node ids in the records; returns the reads the route answered.
+    runs: a list that receives what run() returned, route on and off, first without node ids in the records"""
     cfg = cli_defaults(g.k, min_seed_length=g.k, max_seed_length=g.k)
     expect = g.expected(reads) if expect is None else expect
     for result_nodes in (0, 1):
@@ -102,6 +104,8 @@ def check(g, reads, monkeypatch, capfd, expect=None):
         exp = g.og.align_tsv(cfg, reads, with_nodes=not result_nodes)
         on = run(g.idx, c, reads, True, monkeypatch, capfd)
         off = run(g.idx, c, reads, False, monkeypatch, capfd)
+        if runs is not None:
+            runs += [on, off]
         bad = [i for i in range(len(reads)) if exp[i] != on[0][i]]
         assert not bad, (result_nodes, len(bad), reads[bad[0]], exp[bad[0]], on[0][bad[0]])
         assert off[0] == on[0]
@@ -191,7 +195,7 @@ def test_prepare_exact_heap_full_gpu(monkeypatch, capfd):
     # room for some of the records: the rest are left over; the results are the oracle's either way
     monkeypatch.setenv("MGB_TEST_HEAP0", str(100 * 400))
     cfg = cli_defaults(31, min_seed_length=31, max_seed_length=31)
-    lines, stats, n = run(g.idx, cfg, reads, True, monkeypatch, capfd)
+    lines, stats, n, _ = run(g.idx, cfg, reads, True, monkeypatch, capfd)
     assert lines == g.og.align_tsv(cfg, reads, with_nodes=True)
     assert 0 < n < len(reads) and stats["num_reads_retried"] > 0
     g.close()
