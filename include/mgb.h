@@ -190,6 +190,24 @@ int mgb_map_to_nodes_strands(const mgb_index_t *index, const char *seqs, const u
 int mgb_align_batch(const mgb_index_t *index, const mgb_config_t *config, const char *seqs,
                     const uint64_t *offsets, uint32_t n_reads, mgb_results_t **out);
 
+/* The same seed-and-extend as mgb_align_batch, delivered as the text `metagraph align` prints (cli/align.cpp:254-307),
+ * rendered on the device: the records never leave it, only the text is downloaded.
+ *   MGB_TEXT_TSV   one line per read: header, upper-cased query (bytes >= 0x80 as 0x7F), then per alignment strand,
+ *                  path sequence, score, matches, CIGAR and offset; an unaligned read gets "*\t*\t{min_path_score}\t*\t*\t*"
+ *   MGB_TEXT_JSON  one Alignment::to_json record per alignment (one empty record for an unaligned read), keys sorted,
+ *                  no whitespace, node ids included
+ * Every line ends with '\n'; reads in input order. headers: concatenated header bytes, header_offsets[n_reads + 1]
+ * (copied as they are; in JSON only '"', '\\' and bytes below 0x20 are escaped). The bytes are those of
+ * format_alignment / format_alignment_json in metagraph_b200/aligner.py. The result set answers mgb_results_text,
+ * mgb_results_num_reads, mgb_results_read_range (counts), mgb_results_num_alignments and mgb_results_stats;
+ * mgb_results_alignments returns NULL and mgb_results_export fails. An unknown format: MGB_ERR_INVALID_ARGUMENT. */
+enum { MGB_TEXT_TSV = 1, MGB_TEXT_JSON = 2 };
+int mgb_align_batch_text(const mgb_index_t *index, const mgb_config_t *config, const char *seqs,
+                         const uint64_t *offsets, const char *headers, const uint64_t *header_offsets,
+                         uint32_t n_reads, int format, mgb_results_t **out);
+/* The text block of a result set of mgb_align_batch_text (owned by it); MGB_ERR_INVALID_ARGUMENT for a record set. */
+int mgb_results_text(const mgb_results_t *results, const char **text, uint64_t *bytes);
+
 /* A batch of >= 128k reads is split into up to 8 contiguous pieces that run on two streams, so the
  * download and unpacking of one piece overlap the kernels of the next (reads are independent,
  * dbg_aligner.cpp:251-355). max_pieces caps the split; 1 = one piece (device timers in mgb_stats_t

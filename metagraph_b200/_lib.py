@@ -82,6 +82,10 @@ def load_library(path=None):
     L.mgb_map_to_nodes_strands.argtypes = [vp, vp, vp, u32, vp, vp]
     L.mgb_align_batch.restype = i
     L.mgb_align_batch.argtypes = [vp, ctypes.POINTER(mgb_config_t), vp, vp, u32, ctypes.POINTER(vp)]
+    L.mgb_align_batch_text.restype = i
+    L.mgb_align_batch_text.argtypes = [vp, ctypes.POINTER(mgb_config_t), vp, vp, vp, vp, u32, i, ctypes.POINTER(vp)]
+    L.mgb_results_text.restype = i
+    L.mgb_results_text.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(u64)]
     L.mgb_results_num_reads.restype = u32
     L.mgb_results_num_reads.argtypes = [vp]
     L.mgb_results_read_range.argtypes = [vp, u32, ctypes.POINTER(u64), ctypes.POINTER(u32)]
@@ -129,4 +133,6 @@ REQUIRED_SYMBOLS = [
     "mgb_results_alignments", "mgb_results_stats", "mgb_results_free", "mgb_results_export_bytes",
     "mgb_results_export", "mgb_results_import", "mgb_boss_build", "mgb_boss_free",
     "mgb_boss_mask_dummy", "mgb_set_pipeline_pieces", "mgb_set_host_threads", "mgb_dbg_load", "mgb_dbg_last_error", "mgb_boss_last_error", "mgb_config_check", "mgb_dbg_load_suffix_ranges", "mgb_dbg_free_suffix_ranges", "mgb_index_set_mode",
+    "mgb_align_batch_text", "mgb_results_text",
 ]
+MGB_TEXT_TSV, MGB_TEXT_JSON = 1, 2

@@ -450,5 +450,35 @@ class B200Aligner:
         finally:
             self.free_raw(res)
 
+    def align_batch_text_raw(self, buf, offsets, hbuf, hoffsets, json=False):
+        """Runs mgb_align_batch_text on packed reads and headers; returns the opaque results handle."""
+        c = self.config.to_c() if not isinstance(self.config, mgb_config_t) else self.config
+        res = ctypes.c_void_p()
+        fmt = _lib.MGB_TEXT_JSON if json else _lib.MGB_TEXT_TSV
+        _lib.check(self._L, self._L.mgb_align_batch_text(self.graph.handle, ctypes.byref(c), buf.ctypes.data,
+                                                         offsets.ctypes.data, hbuf.ctypes.data, hoffsets.ctypes.data,
+                                                         len(offsets) - 1, fmt, ctypes.byref(res)))
+        return res
+
+    def text_of(self, res):
+        """the text block of a result set of mgb_align_batch_text, as bytes"""
+        p, n = ctypes.c_void_p(), ctypes.c_uint64()
+        _lib.check(self._L, self._L.mgb_results_text(res, ctypes.byref(p), ctypes.byref(n)))
+        # (ctypes.string_at takes a C int size: blocks of 2 GiB and more are copied through an array type)
+        return bytes((ctypes.c_char * n.value).from_address(p.value)) if n.value else b""
+
+    def align_batch_text(self, seq_batch, json=False):
+        """seq_batch: list of (header, sequence), str or bytes. Returns what `metagraph align` prints for them, rendered
+        on the device: the concatenation of format_alignment(header, paths, min_path_score) + "\\n" per read (json=False)
+        or of format_alignment_json(header, paths, k) + "\\n" (json=True), in input order, as bytes."""
+        buf, offsets = _pack([s for _, s in seq_batch])
+        hbuf, hoffsets = _pack([h for h, _ in seq_batch])
+        res = self.align_batch_text_raw(buf, offsets, hbuf, hoffsets, json)
+        try:
+            self.last_stats = self.stats_of(res)
+            return self.text_of(res)
+        finally:
+            self.free_raw(res)
+
     def align(self, query):
         return self.align_batch([("", query)])[0]

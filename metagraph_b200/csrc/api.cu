@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -42,6 +43,7 @@
 #endif
 #define MGB_KERNEL_NS kern_dna
 #include "kernels.cuh"
+#include "format_core.cuh"
 #include "host_common.hpp"
 #include "index_build.hpp"
 
@@ -284,7 +286,15 @@ struct mgb_results {
     std::vector<uint64_t> src_off;
     std::vector<uint32_t> src_heap;
     uint32_t result_nodes = 0;
-    ~mgb_results() { for (HostBuf b : heaps) hostbuf_release(b); hostbuf_release(alns_buf); }
+    // a text result set (mgb_align_batch_text): MGB_TEXT_TSV / MGB_TEXT_JSON, and the block (no records, no heaps)
+    int text_format = 0;
+    HostBuf text;
+    uint64_t text_bytes = 0;
+    ~mgb_results() {
+        for (HostBuf b : heaps) hostbuf_release(b);
+        if (alns_buf.p) hostbuf_release(alns_buf);
+        if (text.p) hostbuf_release(text);
+    }
     mgb_stats_t stats;
 };
 
@@ -864,6 +874,159 @@ int launch_prepare_exact(const mgb_index_t *index, const PrepExactArgs &a, Strea
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------
+// text route (mgb_align_batch_text): the TSV lines or JSON records of a piece's reads, rendered from the records the
+// align passes left in their heaps (format_core.cuh). Independent of the index layout and the graph mode, so compiled
+// in this translation unit only.
+// ---------------------------------------------------------------------------------------
+constexpr int kMaxPasses = 6;          // align_range gives up on a read after six passes
+
+struct TextArgs {
+    const char *seqs; const uint64_t *offsets;       // the piece's raw reads
+    const char *names; const uint64_t *name_off;     // and their headers
+    const ReadHdr *hdr;                              // per read: n_aln and heap_off of the pass that answered it
+    const uint8_t *pass;                             // ... and that pass
+    const char *heap[kMaxPasses];                    // the output heap of every pass
+    uint32_t n_reads, k, json, result_nodes;
+    int32_t min_path_score;
+    uint64_t *off;         // k_text_size: bytes of each read's text; after the scan its offset, off[n_reads] = total
+    char *out; uint64_t lo, hi;                      // k_text_write: bytes [lo, hi) of the text, at out[0, hi - lo)
+};
+
+// the text of read r (its line, or one JSON record per alignment) into sink s
+template <class S> MGB_HD void text_read(const TextArgs &a, uint32_t r, S &s) {
+    const uint64_t b = a.offsets[r], nb = a.name_off[r];
+    const TextRead rd { a.seqs + b, (uint32_t)(a.offsets[r + 1] - b), a.names + nb, (uint32_t)(a.name_off[r + 1] - nb) };
+    const uint32_t n_aln = a.hdr[r].n_aln;
+    const char *p = n_aln ? a.heap[a.pass[r]] + a.hdr[r].heap_off : nullptr;
+    if (!a.json) tsv_head(s, rd);
+    for (uint32_t i = 0; i < n_aln; ++i) {            // OutAln | node ids (unless result_nodes) | CIGAR | sequence
+        const OutAln o = *reinterpret_cast<const OutAln*>(p);
+        TextAln t { o.orientation, o.score, o.offset, o.query_begin, o.query_len, o.n_nodes, o.seq_len, o.n_cigar,
+                    nullptr, nullptr, nullptr };
+        p += sizeof(OutAln);
+        if (!a.result_nodes) { t.nodes = reinterpret_cast<const uint64_t*>(p); p += 8ull * o.n_nodes; }
+        t.cigar = reinterpret_cast<const uint32_t*>(p); p += (4ull * o.n_cigar + 7) & ~7ull;
+        t.seq = p; p += ((uint64_t)o.seq_len + 7) & ~7ull;
+        if (a.json) json_aln(s, rd, t, i > 0, a.k); else tsv_aln(s, t);
+    }
+    if (!a.json) {
+        if (!n_aln) tsv_unaligned(s, a.min_path_score);
+        s.put('\n');
+    } else if (!n_aln) {
+        json_unaligned(s, rd);
+    }
+}
+
+// reads [*r0, *r1) are those whose text meets bytes [lo, hi) (off: exclusive offsets, every read's text >= 1 byte)
+MGB_HOSTDEV void text_window(const uint64_t *off, uint32_t n, uint64_t lo, uint64_t hi, uint32_t *r0, uint32_t *r1) {
+    uint32_t a = 0, b = n;                 // first read whose text ends after lo
+    while (a < b) { const uint32_t m = (a + b) / 2; if (off[m + 1] > lo) b = m; else a = m + 1; }
+    *r0 = a;
+    b = n;                                 // first read whose text starts at or after hi
+    while (a < b) { const uint32_t m = (a + b) / 2; if (off[m] >= hi) b = m; else a = m + 1; }
+    *r1 = a;
+}
+
+#if !defined(MGB_HOST_EMU)
+// one warp per read
+__global__ void __launch_bounds__(256) k_text_size(const __grid_constant__ TextArgs a) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) / kWarp, nw = (gridDim.x * blockDim.x) / kWarp;
+    for (uint32_t r = warp; r < a.n_reads; r += nw) {
+        CountSink c;
+        text_read(a, r, c);
+        if (wlane() == 0) a.off[r] = c.pos;
+    }
+}
+
+// exclusive scan of off[0, n) in place, total at off[n]: one block, a contiguous segment per thread
+__global__ void __launch_bounds__(1024) k_text_scan(uint64_t *off, uint32_t n) {
+    __shared__ uint64_t part[1024];
+    const uint32_t t = threadIdx.x, seg = (n + 1023) / 1024;
+    const uint64_t b = (uint64_t)t * seg < n ? (uint64_t)t * seg : n, e = b + seg < n ? b + seg : n;
+    uint64_t sum = 0;
+    for (uint64_t i = b; i < e; ++i) sum += off[i];
+    part[t] = sum;
+    __syncthreads();
+    for (uint32_t d = 1; d < 1024; d <<= 1) {
+        const uint64_t v = t >= d ? part[t - d] : 0;
+        __syncthreads();
+        part[t] += v;
+        __syncthreads();
+    }
+    uint64_t run = part[t] - sum;
+    for (uint64_t i = b; i < e; ++i) { const uint64_t v = off[i]; off[i] = run; run += v; }
+    if (t == 1023) off[n] = part[1023];
+}
+
+// one warp per read of the window [a.lo, a.hi)
+__global__ void __launch_bounds__(256) k_text_write(const __grid_constant__ TextArgs a) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) / kWarp, nw = (gridDim.x * blockDim.x) / kWarp;
+    uint32_t r0, r1;
+    text_window(a.off, a.n_reads, a.lo, a.hi, &r0, &r1);
+    for (uint32_t r = r0 + warp; r < r1; r += nw) {
+        WriteSink w { a.out, a.lo, a.hi, a.off[r] };
+        text_read(a, r, w);
+    }
+}
+#endif
+
+// Renders the text of a piece's reads into `host` (pinned; acquired here, *bytes long): the size pass, the scan, 8 bytes
+// read back, then windows of at most `cap` bytes rendered and downloaded one after the other.
+int render_text(const mgb_index_t *index, TextArgs &ta, DevBufs &tb, Stream &st, HostBuf *host, uint64_t *bytes,
+                mgb_stats_t *stats) {
+    *bytes = 0;
+    int rc;
+    if ((rc = tb.alloc(&ta.off, (size_t)ta.n_reads + 1))) return rc;
+    uint64_t total = 0;
+#if defined(MGB_HOST_EMU)
+    (void)index;
+    for (uint32_t r = 0; r < ta.n_reads; ++r) { CountSink c; text_read(ta, r, c); ta.off[r] = c.pos; }
+    for (uint32_t r = 0; r < ta.n_reads; ++r) { const uint64_t v = ta.off[r]; ta.off[r] = total; total += v; }
+    ta.off[ta.n_reads] = total;
+#else
+    {
+        const unsigned grid = (unsigned)kern_dna::read_path_grid(std::min<uint64_t>((ta.n_reads + 7) / 8, (uint64_t)index->num_sms * 16));
+        kern_dna::log_launch("k_text_size", grid, 256, (uint64_t)grid * 8, ta.n_reads);     // a warp per read
+        k_text_size<<<grid, 256, 0, st.s>>>(ta);
+        k_text_scan<<<1, 1024, 0, st.s>>>(ta.off, ta.n_reads);
+        CUDA_TRY(cudaGetLastError());
+        if ((rc = d2h(&total, ta.off + ta.n_reads, 8, st))) return rc;
+        CUDA_TRY(cudaStreamSynchronize(st.s));
+    }
+#endif
+    stats->kernel_launches += 2;
+    stats->d2h_bytes += 8;
+    *host = hostbuf_acquire(total);
+    if (!host->p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
+    *bytes = total;
+    // device bytes of one window (MGB_TEST_TEXT_CAP: test knob, so that small inputs take many windows)
+    uint64_t cap = 256ull << 20;
+    if (const char *e = std::getenv("MGB_TEST_TEXT_CAP")) cap = std::max<long long>(1, std::atoll(e));
+    cap = std::min<uint64_t>(cap, std::max<uint64_t>(total, 1));
+    if ((rc = tb.alloc(&ta.out, cap))) return rc;
+    for (uint64_t lo = 0; lo < total; lo += cap) {
+        ta.lo = lo; ta.hi = std::min(total, lo + cap);
+#if defined(MGB_HOST_EMU)
+        uint32_t r0, r1;
+        text_window(ta.off, ta.n_reads, ta.lo, ta.hi, &r0, &r1);
+        for (uint32_t r = r0; r < r1; ++r) { WriteSink w { ta.out, ta.lo, ta.hi, ta.off[r] }; text_read(ta, r, w); }
+#else
+        const unsigned grid = (unsigned)kern_dna::read_path_grid(std::min<uint64_t>((ta.n_reads + 7) / 8, (uint64_t)index->num_sms * 16));
+        kern_dna::log_launch("k_text_write", grid, 256, (uint64_t)grid * 8, -1);       // a warp per read of the window
+        k_text_write<<<grid, 256, 0, st.s>>>(ta);
+        CUDA_TRY(cudaGetLastError());
+#endif
+        if ((rc = d2h(host->p + lo, ta.out, ta.hi - ta.lo, st))) return rc;
+        stats->kernel_launches += 1;
+    }
+#if !defined(MGB_HOST_EMU)
+    CUDA_TRY(cudaStreamSynchronize(st.s));
+#endif
+    stats->d2h_bytes += total;
+    return 0;
+}
+
 } // namespace
 
 extern "C" {
@@ -963,10 +1126,16 @@ struct Piece {
     std::vector<HostBuf> heaps;
     std::vector<uint64_t> heap_bytes;
     uint64_t *src_off = nullptr; uint32_t *src_heap = nullptr;   // views into the enclosing mgb_results
+    // text route (mgb_align_batch_text): format (0: records), the batch's headers, and the piece's text
+    int text_format = 0;
+    int32_t min_path_score = 0;
+    const char *names = nullptr; const uint64_t *name_offsets = nullptr;
+    HostBuf text;
+    uint64_t text_bytes = 0;
     mgb_stats_t stats;
     int rc = 0;
     std::string err;
-    ~Piece() { for (HostBuf b : heaps) hostbuf_release(b); }
+    ~Piece() { for (HostBuf b : heaps) hostbuf_release(b); if (text.p) hostbuf_release(text); }
 };
 
 static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const char *all_seqs,
@@ -993,6 +1162,15 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
         for (uint32_t r = 0; r <= n_reads; ++r) offs_local[r] = all_offsets[lo + r] - all_offsets[lo];
         offsets = offs_local.data();
     }
+    const bool text = res->text_format != 0;
+    std::vector<uint64_t> name_offs_local;
+    const uint64_t *name_offs = text ? res->name_offsets + lo : nullptr;
+    const char *names = text && res->names ? res->names + res->name_offsets[lo] : nullptr;
+    if (text && res->name_offsets[lo]) {
+        name_offs_local.resize((size_t)n_reads + 1);
+        for (uint32_t r = 0; r <= n_reads; ++r) name_offs_local[r] = res->name_offsets[lo + r] - res->name_offsets[lo];
+        name_offs = name_offs_local.data();
+    }
 
     Stream st;
     struct WsGuard { const mgb_index_t *ix; Workspace *w; ~WsGuard() { ix->ws_release(w); } } wsg{ index, index->ws_acquire() };
@@ -1017,6 +1195,26 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
 #endif
         tick("setup");
         rc = upload_batch(index, seqs, offsets, n_reads, both, st, bufs, &b, &koff, &res->stats);
+        // text route: the headers go up with the reads (workspace slots from 96 on: above every pass's heap, below)
+        DevBufs text_bufs(st, wsg.w, 96);
+        TextArgs ta;
+        std::memset(&ta, 0, sizeof(ta));
+        if (!rc && text) {
+            const uint64_t name_bytes = name_offs[n_reads];
+            char *d_names = nullptr; uint64_t *d_name_off = nullptr;
+            if (!rc) rc = text_bufs.alloc(&d_names, name_bytes + 64);
+            if (!rc) rc = text_bufs.alloc(&d_name_off, (size_t)n_reads + 1);
+            if (!rc && name_bytes) rc = h2d(d_names, names, name_bytes, st);
+            if (!rc) rc = h2d(d_name_off, name_offs, ((size_t)n_reads + 1) * 8, st);
+            res->stats.h2d_bytes += name_bytes + ((size_t)n_reads + 1) * 8;
+            ta.seqs = b.seqs; ta.offsets = b.offsets; ta.names = d_names; ta.name_off = d_name_off;
+            ta.n_reads = n_reads; ta.k = index->view.k; ta.json = res->text_format == MGB_TEXT_JSON;
+            ta.result_nodes = dcfg.result_nodes; ta.min_path_score = res->min_path_score;
+        }
+        // per pass: its heap, read list and counters (DevBufs from workspace slot 33 on). The record route downloads the
+        // heap after the pass and reuses the slots; the text route keeps every pass's heap on the device until the text is
+        // rendered (slots 40 + 8 pass).
+        std::deque<DevBufs> pass_keep;
         tick("upload_batch (host part)");
         // whole-read exact answers ahead of k_align (kernels.cuh ExactArgs): the configuration part of the gate. The
         // seeding kernel of graphs with the k-mer hash index summarises what it stored per read; without it the node
@@ -1156,6 +1354,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             SmemLayout slay;
             const size_t smem_per_warp = slay.carve(bmax_v, lq_v, hcap, (int)dcfg.num_alternative_paths, !index->view.wide);
             DevBufs pass_bufs(st, wsg.w, 32);          // slot 32: the arena
+            DevBufs &heap_bufs = pass_keep.emplace_back(st, wsg.w, text ? 40 + 8 * (size_t)pass : 33);
 #if defined(MGB_HOST_EMU)
             uint32_t n_warps = 1;
 #else
@@ -1202,12 +1401,13 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             if (listed) {
                 d_heap = pa.ex.heap; d_list = pa.list; d_used = pa.ex.heap_used; d_next = next0; d_rest = rest0;
             } else {
-                if ((rc = pass_bufs.alloc(&d_heap, heap_cap))) break;
-                if ((rc = pass_bufs.alloc(&d_list, list.size()))) break;
-                if ((rc = pass_bufs.alloc(&d_used, 1))) break;
-                if ((rc = pass_bufs.alloc(&d_next, 2))) break;    // k_align's next read; the reads k_exact_reads leaves
-                if (exact_reads && (rc = pass_bufs.alloc(&d_rest, list.size()))) break;
+                if ((rc = heap_bufs.alloc(&d_heap, heap_cap))) break;
+                if ((rc = heap_bufs.alloc(&d_list, list.size()))) break;
+                if ((rc = heap_bufs.alloc(&d_used, 1))) break;
+                if ((rc = heap_bufs.alloc(&d_next, 2))) break;    // k_align's next read; the reads k_exact_reads leaves
+                if (exact_reads && (rc = heap_bufs.alloc(&d_rest, list.size()))) break;
             }
+            ta.heap[pass] = d_heap;
             tick("pass: arena/heap alloc");
             if (!listed) {
                 if ((rc = h2d(d_list, list.data(), list.size() * 4, st))) break;
@@ -1230,7 +1430,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             a.phase_out = nullptr;
 #if defined(MGB_PHASE_TIMERS) && !defined(MGB_HOST_EMU)
             unsigned long long *d_phase = nullptr;
-            if ((rc = pass_bufs.alloc(&d_phase, 8))) break;
+            if ((rc = heap_bufs.alloc(&d_phase, 8))) break;
             if ((rc = dev_zero(d_phase, 64, st))) break;
             a.phase_out = d_phase;
 #endif
@@ -1299,12 +1499,16 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             }
 #endif
             if (used > heap_cap) used = heap_cap;
-            HostBuf heap_host = hostbuf_acquire((size_t)used + 16);
-            tick("pass: host buffer");
-            if (!heap_host.p) { rc = fail(MGB_ERR_CUDA, "host buffer allocation failed"); break; }
-            res->heaps.push_back(heap_host);
-            res->heap_bytes.push_back(used);
-            if (used && (rc = d2h(heap_host.p, d_heap, used, st))) break;
+            if (text) {
+                used = 0;                              // the records stay on the device
+            } else {
+                HostBuf heap_host = hostbuf_acquire((size_t)used + 16);
+                tick("pass: host buffer");
+                if (!heap_host.p) { rc = fail(MGB_ERR_CUDA, "host buffer allocation failed"); break; }
+                res->heaps.push_back(heap_host);
+                res->heap_bytes.push_back(used);
+                if (used && (rc = d2h(heap_host.p, d_heap, used, st))) break;
+            }
             if ((rc = d2h(hdr_host, d_hdr, (size_t)n_reads * sizeof(ReadHdr), st))) break;
 #if !defined(MGB_HOST_EMU)
             CUDA_TRY(cudaStreamSynchronize(st.s));
@@ -1316,7 +1520,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             tick("pass: d2h");
             // classify this pass; alignments are materialised in read order after the last pass
             std::vector<uint32_t> retry;
-            const uint32_t heap_id = (uint32_t)res->heaps.size() - 1;
+            const uint32_t heap_id = text ? (uint32_t)pass : (uint32_t)res->heaps.size() - 1;
             for (uint32_t r : list) {
                 const ReadHdr &h = hdr_host[r];
                 if (h.status == MGB_READ_OVERFLOW) { MGB_EMU_HIT(EMU_READ_OVERFLOW); retry.push_back(r); continue; }
@@ -1333,6 +1537,17 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             list.swap(retry);
             tick("pass: classify");
         }
+        // text route: every read's pass goes up (its heap offset is in d_hdr already), then the text comes down
+        if (!rc && text && n_reads) {
+            uint8_t *d_pass = nullptr;
+            std::vector<uint8_t> pass_of(read_heap.begin(), read_heap.end());
+            if (!rc) rc = text_bufs.alloc(&d_pass, n_reads);
+            if (!rc) rc = h2d(d_pass, pass_of.data(), n_reads, st);
+            res->stats.h2d_bytes += n_reads;
+            ta.hdr = d_hdr; ta.pass = d_pass;
+            if (!rc) rc = render_text(index, ta, text_bufs, st, &res->text, &res->text_bytes, &res->stats);
+            tick("text");
+        }
 #if !defined(MGB_HOST_EMU)
         if (!rc) {
             float ms = 0;
@@ -1347,6 +1562,12 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
 #endif
     if (rc) return rc;
     tick("free device buffers");
+    if (text) {                                   // counts only: the text route has no records on the host
+        uint64_t pos = 0;
+        for (uint32_t r = 0; r < n_reads; ++r) { res->first[r] = pos; pos += res->count[r]; }
+        res->n_alns = pos;
+        return MGB_OK;
+    }
     // materialise mgb_alignment_t records in read order
     {
         std::vector<uint64_t> byte_off(res->first, res->first + n_reads);
@@ -1403,10 +1624,12 @@ int mgb_config_check(const mgb_index_t *index, const mgb_config_t *config) {
     return rc ? fail(rc, err) : MGB_OK;
 }
 
-int mgb_align_batch(const mgb_index_t *index, const mgb_config_t *config, const char *seqs,
-                    const uint64_t *offsets, uint32_t n_reads, mgb_results_t **out) {
-    if (!index || !config || !offsets || !out || (!seqs && n_reads && offsets[n_reads]))
-        return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+} // extern "C"
+
+// mgb_align_batch (text_format 0) and mgb_align_batch_text (MGB_TEXT_TSV / MGB_TEXT_JSON, with the headers)
+static int align_batch(const mgb_index_t *index, const mgb_config_t *config, const char *seqs, const uint64_t *offsets,
+                       const char *names, const uint64_t *name_offsets, uint32_t n_reads, int text_format,
+                       mgb_results_t **out) {
     DevConfig dcfg;
     std::string err;
     int rc = lower_config(*config, index->view.k, index->alphabet, &dcfg, &err);
@@ -1415,6 +1638,8 @@ int mgb_align_batch(const mgb_index_t *index, const mgb_config_t *config, const 
         dcfg.canonical = 1;                      // (get_mode() == CANONICAL): both strands, no RCDBG view
         dcfg.forward_and_reverse_complement = 1; // (dbg_aligner.cpp:224-226)
     }
+    // the text route: TSV lines print no node ids, so its records carry none; JSON records need them on the device
+    if (text_format) dcfg.result_nodes = text_format == MGB_TEXT_TSV ? MGB_NODES_NONE : MGB_NODES_U64;
 
 
     // pieces of >= 64k reads, at most 8; two host threads keep two pieces in flight
@@ -1439,22 +1664,30 @@ int mgb_align_batch(const mgb_index_t *index, const mgb_config_t *config, const 
     res->n_reads = n_reads;
     res->first.assign(n_reads, 0);
     res->count.assign(n_reads, 0);
-    res->src_off.assign(n_reads, 0);
-    res->src_heap.assign(n_reads, 0);
     res->result_nodes = dcfg.result_nodes;
+    res->text_format = text_format;
     const uint64_t num_alt = dcfg.num_alternative_paths;
-    res->alns_buf = hostbuf_acquire(((size_t)n_reads * num_alt + 1) * sizeof(mgb_alignment_t));
-    if (!res->alns_buf.p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
-    res->alns = (mgb_alignment_t*)res->alns_buf.p;
+    if (!text_format) {
+        res->src_off.assign(n_reads, 0);
+        res->src_heap.assign(n_reads, 0);
+        res->alns_buf = hostbuf_acquire(((size_t)n_reads * num_alt + 1) * sizeof(mgb_alignment_t));
+        if (!res->alns_buf.p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
+        res->alns = (mgb_alignment_t*)res->alns_buf.p;
+    }
 
     std::vector<Piece> pieces(n_pieces);
     auto piece_lo = [&](uint32_t i) { return (uint32_t)((uint64_t)n_reads * i / n_pieces); };
     for (uint32_t i = 0; i < n_pieces; ++i) {
         pieces[i].first = res->first.data() + piece_lo(i);
         pieces[i].count = res->count.data() + piece_lo(i);
-        pieces[i].alns = res->alns + (uint64_t)piece_lo(i) * num_alt;
-        pieces[i].src_off = res->src_off.data() + piece_lo(i);
-        pieces[i].src_heap = res->src_heap.data() + piece_lo(i);
+        if (!text_format) {
+            pieces[i].alns = res->alns + (uint64_t)piece_lo(i) * num_alt;
+            pieces[i].src_off = res->src_off.data() + piece_lo(i);
+            pieces[i].src_heap = res->src_heap.data() + piece_lo(i);
+        }
+        pieces[i].text_format = text_format;
+        pieces[i].min_path_score = config->min_path_score;
+        pieces[i].names = names; pieces[i].name_offsets = name_offsets;
     }
     if (n_pieces == 1) {
         rc = align_range(index, dcfg, seqs, offsets, 0, n_reads, &pieces[0]);
@@ -1487,7 +1720,7 @@ int mgb_align_batch(const mgb_index_t *index, const mgb_config_t *config, const 
     for (uint32_t i = 0; i < n_pieces; ++i) {
         Piece &pc = pieces[i];
         const uint64_t region = (uint64_t)pc.lo * num_alt;
-        if (total != region) {
+        if (!text_format && total != region) {
             std::memmove(res->alns + total, res->alns + region, pc.n_alns * sizeof(mgb_alignment_t));
         }
         if (total) {
@@ -1511,8 +1744,63 @@ int mgb_align_batch(const mgb_index_t *index, const mgb_config_t *config, const 
         t.h2d_bytes += u.h2d_bytes; t.d2h_bytes += u.d2h_bytes; t.kernel_launches += u.kernel_launches;
     }
     res->n_alns = total;
+    if (text_format) {
+        // the pieces' blocks in piece order: one piece hands its buffer over, several are copied into one block
+        uint64_t bytes = 0;
+        for (Piece &pc : pieces) bytes += pc.text_bytes;
+        if (n_pieces == 1 && pieces[0].text.p) {
+            res->text = pieces[0].text; pieces[0].text = HostBuf();
+        } else {
+            res->text = hostbuf_acquire(bytes);
+            if (!res->text.p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
+            uint64_t at = 0;
+            for (Piece &pc : pieces) {
+                const uint64_t n = pc.text_bytes;
+                const int64_t chunks = (int64_t)((n + (1 << 22) - 1) >> 22);
+                char *dst = res->text.p + at; const char *src = pc.text.p;
+                #pragma omp parallel for schedule(static) num_threads(host_team()) if (chunks > 4)
+                for (int64_t c = 0; c < chunks; ++c) {
+                    const uint64_t o = (uint64_t)c << 22;
+                    std::memcpy(dst + o, src + o, std::min<uint64_t>(1ull << 22, n - o));
+                }
+                at += n;
+            }
+        }
+        res->text_bytes = bytes;
+    }
     if (dbg_time) std::fprintf(stderr, "[mgb] merged at %.2f ms\n", since());
     *out = res.release();
+    return MGB_OK;
+}
+
+extern "C" {
+
+int mgb_align_batch(const mgb_index_t *index, const mgb_config_t *config, const char *seqs,
+                    const uint64_t *offsets, uint32_t n_reads, mgb_results_t **out) {
+    if (!index || !config || !offsets || !out || (!seqs && n_reads && offsets[n_reads]))
+        return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    return align_batch(index, config, seqs, offsets, nullptr, nullptr, n_reads, 0, out);
+}
+
+int mgb_align_batch_text(const mgb_index_t *index, const mgb_config_t *config, const char *seqs,
+                         const uint64_t *offsets, const char *headers, const uint64_t *header_offsets,
+                         uint32_t n_reads, int format, mgb_results_t **out) {
+    if (!index || !config || !offsets || !out || (!seqs && n_reads && offsets[n_reads]))
+        return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (format != MGB_TEXT_TSV && format != MGB_TEXT_JSON)
+        return fail(MGB_ERR_INVALID_ARGUMENT, "format must be MGB_TEXT_TSV or MGB_TEXT_JSON");
+    if (!header_offsets || (!headers && n_reads && header_offsets[n_reads]))
+        return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    for (uint32_t r = 0; r < n_reads; ++r)
+        if (header_offsets[r + 1] < header_offsets[r]) return fail(MGB_ERR_INVALID_ARGUMENT, "header offsets must be non-decreasing");
+    return align_batch(index, config, seqs, offsets, headers, header_offsets, n_reads, format, out);
+}
+
+int mgb_results_text(const mgb_results_t *results, const char **text, uint64_t *bytes) {
+    if (!results || !text || !bytes) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (!results->text_format) return fail(MGB_ERR_INVALID_ARGUMENT, "not a text result set (mgb_align_batch_text)");
+    *text = results->text.p ? results->text.p : "";
+    *bytes = results->text_bytes;
     return MGB_OK;
 }
 
@@ -1523,6 +1811,7 @@ struct ExportHdr { uint64_t magic, n_reads, n_alns, n_heaps, result_nodes, total
 const uint64_t kExportMagic = 0x3142474d53455231ull;      // "1RESMGB1"
 }
 uint64_t mgb_results_export_bytes(const mgb_results_t *r) {
+    if (r->text_format) return 0;                // a text result set has no records to export
     uint64_t b = sizeof(ExportHdr) + (uint64_t)r->n_reads * (8 + 4 + 4) + 8 * r->heap_bytes.size();
     b = (b + 15) & ~15ull;
     for (uint64_t h : r->heap_bytes) b += (h + 15) & ~15ull;
@@ -1530,6 +1819,7 @@ uint64_t mgb_results_export_bytes(const mgb_results_t *r) {
 }
 int mgb_results_export(const mgb_results_t *r, void *dst, uint64_t capacity) {
     if (!r || !dst) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (r->text_format) return fail(MGB_ERR_INVALID_ARGUMENT, "a text result set (mgb_align_batch_text) has no records to export");
     const uint64_t total = mgb_results_export_bytes(r);
     if (capacity < total) return fail(MGB_ERR_INVALID_ARGUMENT, "export buffer too small");
     char *p = (char*)dst;

@@ -201,6 +201,32 @@ class B200Aligner
         }
     }
 
+    // What `metagraph align` prints for the batch (cli/align.cpp:254-307), rendered on the device by mgb_align_batch_text:
+    // one TSV line per query, or with json = true one JSON record per alignment, each ending in '\n', in batch order,
+    // appended to *out. No AlignmentResults are built; the node ids never leave the device.
+    void align_batch_text(const std::vector<Query> &batch, bool json, std::string *out) const {
+        std::string seqs, names;
+        std::vector<uint64_t> offsets(batch.size() + 1, 0), name_offsets(batch.size() + 1, 0);
+        for (size_t i = 0; i < batch.size(); ++i) {
+            names += batch[i].first;
+            name_offsets[i + 1] = names.size();
+            seqs += batch[i].second;
+            offsets[i + 1] = seqs.size();
+        }
+        mgb_results_t *res = nullptr;
+        int rc = mgb_align_batch_text(index_.handle(), &c_, seqs.data(), offsets.data(), names.data(),
+                                      name_offsets.data(), (uint32_t)batch.size(), json ? MGB_TEXT_JSON : MGB_TEXT_TSV,
+                                      &res);
+        if (rc != MGB_OK) throw std::runtime_error(mgb_last_error());
+        const char *text = nullptr;
+        uint64_t bytes = 0;
+        rc = mgb_results_text(res, &text, &bytes);
+        if (rc == MGB_OK) out->append(text, bytes);
+        std::string err = rc == MGB_OK ? "" : mgb_last_error();
+        mgb_results_free(res);
+        if (rc != MGB_OK) throw std::runtime_error(err);
+    }
+
     Results align(const std::string &query) const {   // IDBGAligner::align (dbg_aligner.cpp:22-31)
         Results result;
         align_batch({ Query{ std::string{}, query } },
