@@ -858,13 +858,20 @@ int launch_prepare_exact(const mgb_index_t *index, const PrepExactArgs &a, Strea
     (void)index; (void)st;
     for (uint32_t r = 0; r < a.prep.n_reads; ++r) {
         uint64_t b; int L; uint32_t p; score_t score;
-        int s = exact_path_strand(a, r, &b, &L, &p, &score);
+        PrepTimer tm;
+        b = a.prep.offsets[r]; L = (int)(a.prep.offsets[r + 1] - b);
+        const uint8_t *raw = reinterpret_cast<const uint8_t*>(a.prep.seqs) + b;
+        int s = exact_path_strand(a, raw, L, &p, &score, tm);
         const uint64_t off = *a.ex.heap_used;
         if (s >= 0) {
             *a.ex.heap_used += exact_read_bytes(a.ex, L);
             if (off + exact_read_bytes(a.ex, L) > a.ex.heap_cap) s = -1;
         }
-        if (s >= 0) { exact_path_write(a, r, b, L, s, p, score, off, 0, 1); continue; }
+        if (s >= 0) {
+            exact_path_hdr(a.ex, r, L, off);
+            exact_path_write(a, raw, L, s, p, score, off, 0, 1);
+            continue;
+        }
         a.list[(*a.n_list)++] = r;
         prepare_read(a.prep, r);
     }
@@ -1275,6 +1282,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             pa.prep = PrepArgs { b.seqs, b.offsets, b.n_reads, b.qf, b.qr, b.cf, b.cr, {0} };
             std::memcpy(pa.prep.code_of, index->at.code_of, sizeof(pa.prep.code_of));
             exact_args(choose_caps(b.L_max, dcfg, k, 1), &pa.ex);
+            pa.stage_bytes = prep_stage_bytes(b.L_max);
             pa.ex.heap_cap = heap_cap_of(n_reads, 1);
             if (!rc) rc = bufs.alloc(&pa.ex.heap, pa.ex.heap_cap);
             if (!rc) rc = bufs.alloc(&pa.ex.heap_used, 1);
@@ -1284,6 +1292,10 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             if (!rc) rc = dev_zero(pa.ex.heap_used, 8, st);
             if (!rc) rc = dev_zero(next0, 16, st);
             pa.n_list = next0 + 2;
+#if defined(MGB_PREP_TIMERS) && !defined(MGB_HOST_EMU)
+            if (!rc) rc = bufs.alloc(&pa.phase_out, PREP_N_PHASES);
+            if (!rc) rc = dev_zero(pa.phase_out, 8 * PREP_N_PHASES, st);
+#endif
         }
 #if !defined(MGB_HOST_EMU)
         cudaEventRecord(ev[1], st.s);
@@ -1456,6 +1468,17 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
                 if (listed && dbg_time)
                     std::fprintf(stderr, "[mgb] reads %u+%u k_prepare_exact answered %u, left over %u\n", lo, n_reads,
                                  n_reads - n_rest[1], n_rest[1]);
+#if defined(MGB_PREP_TIMERS) && !defined(MGB_HOST_EMU)
+                if (listed && dbg_time) {
+                    unsigned long long ph[PREP_N_PHASES];
+                    CUDA_TRY(cudaMemcpy(ph, pa.phase_out, sizeof(ph), cudaMemcpyDeviceToHost));
+                    const double nr = n_reads ? (double)n_reads : 1.0;
+                    std::fprintf(stderr, "[mgb] k_prepare_exact cycles/read: stage %.0f keys %.0f lookup %.0f stop_rc %.0f "
+                                 "text %.0f alloc %.0f write %.0f left %.0f\n", ph[PREP_STAGE] / nr, ph[PREP_KEYS] / nr,
+                                 ph[PREP_LOOKUP] / nr, ph[PREP_STOPRC] / nr, ph[PREP_TEXT] / nr, ph[PREP_ALLOC] / nr,
+                                 ph[PREP_WRITE] / nr, ph[PREP_LEFT] / nr);
+                }
+#endif
                 a.read_list = d_rest; a.n_list = n_rest[0];
                 res->stats.kernel_launches += 1;
             }

@@ -10,6 +10,7 @@
 // The host-emulation build (tests/emu) includes it once with the layout chosen at run time.
 #pragma once
 #include "align_core.cuh"
+#include "acgt_words.cuh"
 #if !defined(MGB_HOST_EMU)
 #include <cuda_runtime.h>
 #include <cstdio>
@@ -389,6 +390,34 @@ struct PrepExactArgs {
     PrepArgs prep;                // the raw reads, and the strand buffers of the reads left over
     ExactArgs ex;                 // k, end_bonus, min_score, max_len, result_nodes, diag; hdr and the heap
     uint32_t *list; unsigned int *n_list;            // the reads left over (prepared, to be seeded)
+    unsigned long long *phase_out;   // MGB_PREP_TIMERS builds: cycles per PrepPhase, summed over the threads
+    uint32_t stage_bytes;            // k_prepare_exact's shared memory for a tile's characters (prep_stage_bytes)
+};
+
+// k_prepare_exact stages a tile's characters in shared memory from the 16-byte word holding its first byte to
+// kPrepStageSlack bytes past its last (the word reads of exact_path_strand go up to 35 past a read), rounded up to 16
+// bytes: 256 * L_max + 80 bytes hold any tile of 256 reads, at most kPrepStageMax (below the 48 KB a block may use without opting in;
+// a longer tile is read from global memory). The read buffer is padded by 64 bytes, so the copy stays inside it.
+static constexpr uint32_t kPrepStageSlack = 48, kPrepStageMax = 45 * 1024;
+MGB_HOSTDEV uint32_t prep_stage_bytes(uint32_t L_max) {
+    const uint64_t need = 256ull * L_max + 32 + kPrepStageSlack;          // rounding both ends to 16 adds <= 30
+    return need < kPrepStageMax ? (uint32_t)need : kPrepStageMax;
+}
+
+// MGB_PREP_TIMERS builds (scripts/build_variant.sh): clock64 cycles of each thread of k_prepare_exact per phase, printed
+// per read under MGB_DEBUG. A thread's time from one lap to the next goes to the phase named at the lap; a read that
+// leaves the gate early adds its time to the next phase the thread reaches. Compiled out of the product build.
+enum PrepPhase : int { PREP_STAGE, PREP_KEYS, PREP_LOOKUP, PREP_STOPRC, PREP_TEXT, PREP_ALLOC, PREP_WRITE, PREP_LEFT,
+                       PREP_N_PHASES };
+struct PrepTimer {
+#if defined(MGB_PREP_TIMERS) && MGB_DEVICE_CODE
+    long long c[PREP_N_PHASES] = {}, t0 = 0;
+    MGB_D void start() { t0 = clock64(); }
+    MGB_D void lap(int ph) { const long long t = clock64(); c[ph] += t - t0; t0 = t; }
+#else
+    MGB_HD void start() {}
+    MGB_HD void lap(int) {}
+#endif
 };
 
 MGB_HD unsigned long long ldg64(const unsigned long long *p) {
@@ -398,44 +427,24 @@ MGB_HD unsigned long long ldg64(const unsigned long long *p) {
     return *p;
 #endif
 }
-// 2-bit code of an A/C/G/T byte, upper or lower case (A 0, C 1, G 2, T 3); *ok is cleared for any other byte
-MGB_HD uint32_t acgt_code(uint32_t ch, bool *ok) {
-    const uint32_t u = ch & 0xDFu;
-    *ok = *ok && ch < 128 && (u == 'A' || u == 'C' || u == 'G' || u == 'T');
-    return ((u >> 1) ^ (u >> 2)) & 3u;
-}
-// Σ diag over the characters whose 2-bit codes are given, from the four diag values packed one byte each
-MGB_HD int diag_of(uint32_t dg4, uint32_t code) { return (int)(int8_t)(uint8_t)(dg4 >> (8 * code)); }
-
-// The primary strand (0 / 1) of read r if the read is answered here (conditions above), else -1; *b / *L: the read's
-// start and length, *pos: its place p on the path, *score: the alignment's score. One lane, no collectives. The raw
-// characters are read as aligned 8-byte words (the buffer is padded past its end).
-MGB_HD int exact_path_strand(const PrepExactArgs &a, uint32_t r, uint64_t *b, int *L, uint32_t *pos, score_t *score) {
+// The primary strand (0 / 1) of a read if it is answered here (conditions above), else -1; raw / n: its characters
+// and length, *pos: its place p on the path, *score: the alignment's score. One lane, no collectives. The characters
+// are read as aligned 4-byte words (acgt_pack32: up to 35 bytes past the read must be readable) and handled as 2-bit
+// codes 32 at a time; both strands run the same word operations. The path layout is read in chunks of kPathChunk
+// characters, all words of a chunk loaded before any is used.
+static constexpr int kPathChunk = 160;
+static constexpr int kChunkWords = kPathChunk / 32;
+MGB_HD int exact_path_strand(const PrepExactArgs &a, const uint8_t *raw, int n, uint32_t *pos, score_t *score,
+                             PrepTimer &tm) {
     const IndexView &ix = a.ix;
-    *b = a.prep.offsets[r];
-    *L = (int)(a.prep.offsets[r + 1] - *b);
-    const int n = *L, K = (int)a.ex.k;
+    const int K = (int)a.ex.k;
     if (n < K || n > (int)a.ex.max_len) return -1;
-    const uintptr_t lo = (uintptr_t)(a.prep.seqs + *b), hi = lo + (uintptr_t)n;
-    // ---- the position-0 k-mers of both strands: characters [0, k) forward, [L - k, L) backwards and complemented
-    bool ok = true;
-    unsigned long long kf = 0, kr = 0;
-    {
-        const uintptr_t e = lo + (uintptr_t)K;
-        for (uintptr_t w = lo & ~(uintptr_t)7; w < e; w += 8) {
-            const unsigned long long x = ldg64(reinterpret_cast<const unsigned long long*>(w));
-            const int j0 = w < lo ? (int)(lo - w) : 0, j1 = e - w < 8 ? (int)(e - w) : 8;
-            for (int j = j0; j < j1; ++j) kf |= (unsigned long long)acgt_code((uint32_t)(x >> (8 * j)) & 0xFFu, &ok) << (2 * (w + j - lo));
-        }
-        const uintptr_t s0 = hi - (uintptr_t)K;
-        for (uintptr_t w = s0 & ~(uintptr_t)7; w < hi; w += 8) {
-            const unsigned long long x = ldg64(reinterpret_cast<const unsigned long long*>(w));
-            const int j0 = w < s0 ? (int)(s0 - w) : 0, j1 = hi - w < 8 ? (int)(hi - w) : 8;
-            for (int j = j0; j < j1; ++j)        // raw position i is reverse-strand position L - 1 - i
-                kr |= (unsigned long long)(3u - acgt_code((uint32_t)(x >> (8 * j)) & 0xFFu, &ok)) << (2 * (hi - 1 - (w + j)));
-        }
-    }
-    if (!ok) return -1;
+    // ---- the position-0 k-mers of both strands: codes [0, k) forward, [L - k, L) reverse-complemented. Their
+    // characters are checked with the whole read below; an invalid one only makes a lookup that cannot matter.
+    uint32_t inv;
+    const unsigned long long kf = acgt_pack32(raw, &inv) & codes_mask(K);
+    const unsigned long long kr = rc_codes32(acgt_pack32(raw + (n - K), &inv)) >> (2 * (32 - K));
+    tm.lap(PREP_KEYS);
     uint64_t ef, er;
 #if MGB_DEVICE_CODE
     {
@@ -452,52 +461,69 @@ MGB_HD int exact_path_strand(const PrepExactArgs &a, uint32_t r, uint64_t *b, in
     const uint64_t e = s ? er : ef;
     if (!in_graph(ix, e)) return -1;
     const uint32_t p = ldg32(ix.pl_pos + e);
+    tm.lap(PREP_LOOKUP);
     if (p == kPlNone) return -1;
-    // ---- pl_stop / pl_rc over [p, p + nk): a 0 stop bit at p + 1 .. p + nk - 1 keeps the path going (p is a node); this
-    // comes first, so that the text below is read inside the path and its filler
-    const uint32_t end = p + (uint32_t)(n - K + 1);
-    for (uint32_t q0 = p & ~31u; q0 < end; q0 += 32) {
-        uint32_t m = q0 < p ? ~0u << (p - q0) : ~0u;
-        if (end - q0 < 32) m &= (1u << (end - q0)) - 1u;
-        if ((ldg32(ix.pl_stop + (q0 >> 5)) | ldg32(ix.pl_rc + (q0 >> 5))) & m) return -1;
-    }
-    // ---- the primary strand against pl_text[p .. p + L), 32 characters per compare; its Σ diag on the way
-    const uint32_t dg4 = (uint32_t)(uint8_t)a.ex.diag['A'] | (uint32_t)(uint8_t)a.ex.diag['C'] << 8
-                       | (uint32_t)(uint8_t)a.ex.diag['G'] << 16 | (uint32_t)(uint8_t)a.ex.diag['T'] << 24;
-    int sum = 0;
-    unsigned long long acc = 0;                             // primary characters i0 .. i0 + na - 1
-    int na = 0;
-    uint32_t i0 = 0;
-    bool same = true;
-    auto compare = [&]() {
-        const uint32_t P = p + i0, sh = 2 * (P & 31);
-        unsigned long long t = ldg64(ix.pl_text + (P >> 5)) >> sh;
-        if (sh) t |= ldg64(ix.pl_text + (P >> 5) + 1) << (64 - sh);
-        if (na < 32) t &= (1ull << (2 * na)) - 1;
-        same = same && t == acc;
-        i0 += 32; acc = 0; na = 0;
-    };
-    auto put = [&](uint32_t code) {
-        sum += diag_of(dg4, code);
-        acc |= (unsigned long long)code << (2 * na);
-        if (++na == 32) compare();
-    };
-    if (s == 0) {
-        for (uintptr_t w = lo & ~(uintptr_t)7; w < hi && same; w += 8) {
-            const unsigned long long x = ldg64(reinterpret_cast<const unsigned long long*>(w));
-            const int j0 = w < lo ? (int)(lo - w) : 0, j1 = hi - w < 8 ? (int)(hi - w) : 8;
-            for (int j = j0; j < j1; ++j) put(acgt_code((uint32_t)(x >> (8 * j)) & 0xFFu, &ok));
+    const int nk = n - K + 1;
+    int cnt[4] = { 0, 0, 0, 0 };                            // A, C, G, T on the primary strand
+    for (int i0 = 0; i0 < n; i0 += kPathChunk) {
+        // ---- the layout words of path positions [P, P + kPathChunk): pl_stop / pl_rc over [p, p + nk) (a 0 stop bit
+        // at p + 1 .. p + nk - 1 keeps the path going, p is a node), pl_text over [p, p + L); all issued first
+        const uint32_t P = p + (uint32_t)i0, w0 = P >> 5;
+        const uint32_t se = p + (uint32_t)(i0 + kPathChunk < nk ? i0 + kPathChunk : nk);
+        const uint32_t te = p + (uint32_t)(i0 + kPathChunk < n ? i0 + kPathChunk : n);
+        uint32_t st[kChunkWords + 1], rc[kChunkWords + 1];
+        unsigned long long tx[kChunkWords + 1];
+#if MGB_DEVICE_CODE
+        #pragma unroll
+#endif
+        for (int t = 0; t <= kChunkWords; ++t) {
+            const uint32_t q = (w0 + (uint32_t)t) << 5;
+            st[t] = q < se ? ldg32(ix.pl_stop + w0 + t) : 0u;
+            rc[t] = q < se ? ldg32(ix.pl_rc + w0 + t) : 0u;
+            tx[t] = q < te ? ldg64(ix.pl_text + w0 + t) : 0ull;
         }
-    } else {
-        for (uintptr_t w = (hi - 1) & ~(uintptr_t)7; w + 8 > lo && same; w -= 8) {
-            const unsigned long long x = ldg64(reinterpret_cast<const unsigned long long*>(w));
-            const int j0 = w < lo ? (int)(lo - w) : 0, j1 = hi - w < 8 ? (int)(hi - w) : 8;
-            for (int j = j1 - 1; j >= j0; --j) put(3u - acgt_code((uint32_t)(x >> (8 * j)) & 0xFFu, &ok));
+        uint32_t stop = 0;
+#if MGB_DEVICE_CODE
+        #pragma unroll
+#endif
+        for (int t = 0; t <= kChunkWords; ++t) {
+            const uint32_t q = (w0 + (uint32_t)t) << 5;
+            if (q < se) {
+                uint32_t m = q < P ? ~0u << (P - q) : ~0u;
+                if (se - q < 32) m &= (1u << (se - q)) - 1u;
+                stop |= (st[t] | rc[t]) & m;
+            }
         }
+        tm.lap(PREP_STOPRC);
+        // ---- the primary strand's codes i0 + 32 j .. against pl_text, every character checked for A/C/G/T, the
+        // per-letter counts on the way. Strand 1's code i is 3 - code n - 1 - i forward: the 32 bytes ending there,
+        // reverse-complemented (near the read's start, the bytes from 0 and the codes shifted into place).
+        const uint32_t sh = 2 * (P & 31);
+        unsigned long long diff = 0;
+        uint32_t bad = 0;
+#if MGB_DEVICE_CODE
+        #pragma unroll
+#endif
+        for (int j = 0; j < kChunkWords; ++j) {
+            const int i = i0 + 32 * j;
+            if (i < n) {
+                const int m = n - i < 32 ? n - i : 32;
+                const int q = s ? n - i - 32 : i;
+                const unsigned long long x = acgt_pack32(raw + (q > 0 ? q : 0), &inv);
+                const unsigned long long xr = rc_codes32(x) >> (q < 0 ? -2 * q : 0);
+                const unsigned long long c = s ? xr : x, cm = codes_mask(m);
+                bad |= inv & (m < 32 ? (1u << m) - 1u : ~0u);
+                unsigned long long t = tx[j] >> sh;
+                if (sh) t |= tx[j + 1] << (64 - sh);
+                diff |= (c ^ t) & cm;
+                acgt_count(c, cm, cnt);
+            }
+        }
+        tm.lap(PREP_TEXT);
+        if (stop || bad || diff) return -1;
     }
-    if (na) compare();
-    if (!ok || !same) return -1;
-    const score_t full = sum + a.ex.end_bonus;
+    const score_t full = cnt[0] * a.ex.diag['A'] + cnt[1] * a.ex.diag['C'] + cnt[2] * a.ex.diag['G']
+                       + cnt[3] * a.ex.diag['T'] + a.ex.end_bonus;
     if (full < a.ex.min_score) return -1;
 #if defined(MGB_HOST_EMU)
     ++mgb_emu_path_read_hits;
@@ -506,15 +532,44 @@ MGB_HD int exact_path_strand(const PrepExactArgs &a, uint32_t r, uint64_t *b, in
     return s;
 }
 
-// exact_record_write of a read exact_path_strand answered: node ids from the path layout, characters from the raw read
-MGB_HD void exact_path_write(const PrepExactArgs &a, uint32_t r, uint64_t b, int L, int s, uint32_t p, score_t score,
+// Word wi of the record of a read exact_path_strand answered (raw / L / s / p / score: its characters, length, strand,
+// place on the path and score): exact_record_write's bytes with node ids pl_node[p + t] and the strand's characters from
+// the raw read (sanitize_char, complement_char: the read is all A/C/G/T), padding as zeros.
+static_assert(sizeof(OutAln) == 32, "OutAln is four words");
+MGB_HD unsigned long long exact_path_word(const PrepExactArgs &a, const uint8_t *raw, int L, int s, uint32_t p,
+                                          score_t score, uint32_t wi) {
+    const uint32_t nk = (uint32_t)(L - (int)a.ex.k + 1), nn = a.ex.result_nodes ? 0u : nk;
+    if (wi < 4) {            // OutAln: orientation, score | offset, query_begin | query_len, n_nodes | seq_len, n_cigar
+        const uint32_t lo = wi == 0 ? (uint32_t)s : wi == 1 ? 0u : (uint32_t)L;
+        const uint32_t hi = wi == 0 ? (uint32_t)score : wi == 1 ? 0u : wi == 2 ? nk : 1u;
+        return lo | (unsigned long long)hi << 32;
+    }
+    wi -= 4;
+    if (wi < nn) return ldg32(a.ix.pl_node + p + wi);
+    wi -= nn;
+    if (wi == 0) return cig_pack(OP_M, (uint32_t)L);
+    const int j = 8 * (int)(wi - 1);                    // characters j .. j + 7 of the strand
+    const int q = s ? L - 8 - j : j;                    // ... from the raw bytes q .. q + 7
+    unsigned long long x = bytes8_at(raw + (q > 0 ? q : 0));
+    if (q < 0) x <<= -8 * q;
+    x = acgt_chars8(x, s != 0);
+    if (L - j < 8) x &= (1ull << (8 * (L - j))) - 1;
+    return x;
+}
+// the record of such a read at heap offset `off` (which fits), lanes `lane` of `width` one word each
+MGB_HD void exact_path_write(const PrepExactArgs &a, const uint8_t *raw, int L, int s, uint32_t p, score_t score,
                              uint64_t off, int lane, int width) {
-    const uint32_t *pn = a.ix.pl_node + p;
-    const char *raw = a.prep.seqs + b;
-    exact_record_write(a.ex, r, L, s, score, off, [pn](int t) { return (uint64_t)ldg32(pn + t); },
-                       [raw, L, s](int t) {
-                           return s ? (char)complement_char(sanitize_char((uint8_t)raw[L - 1 - t])) : (char)sanitize_char((uint8_t)raw[t]);
-                       }, lane, width);
+    unsigned long long *o = reinterpret_cast<unsigned long long*>(a.ex.heap + off);
+    const uint32_t nw = exact_read_bytes(a.ex, L) / 8;
+    for (uint32_t wi = (uint32_t)lane; wi < nw; wi += (uint32_t)width) o[wi] = exact_path_word(a, raw, L, s, p, score, wi);
+}
+// ... and its header, exact_record_write's
+MGB_HD void exact_path_hdr(const ExactArgs &a, uint32_t r, int L, uint64_t off) {
+    ReadHdr h;
+    h.status = MGB_READ_OK; h.n_aln = 1; h.heap_off = off;
+    h.stats.num_seeds = (uint32_t)(L - (int)a.k + 1); h.stats.num_extensions = 1;
+    h.stats.num_explored_nodes = 0; h.stats.dp_columns = 0; h.stats.dp_cells = 0;
+    a.hdr[r] = h;
 }
 
 // One refinement level of the suffix-range table (boss.hpp:651-655 index order: the appended
@@ -1340,45 +1395,93 @@ __device__ __forceinline__ C tile_alloc(uint32_t v, C *ctr, uint32_t *s_sum, C *
 }
 
 // Whole-read exact answers from the raw reads (exact_path_strand), in place of k_prepare, a tile of kPrepExactThreads
-// reads per block and round, one read per thread. The answered reads of a tile take one heap allocation (a record that
-// does not fit makes its read a left-over one), the left-over reads one append to a.list; then each warp writes its
-// answered records and prepares its left-over reads (prepare_read), one after the other, 32 lanes each. Persistent grid.
+// reads per block and round, one read per thread. The block first copies the tile's characters to shared memory with
+// coalesced 16-byte loads (a tile longer than a.stage_bytes is read from global memory through the same code). The
+// answered reads of a tile take one heap allocation (a record that does not fit makes its read a left-over one), the
+// left-over reads one append to a.list; each thread writes its read's header, then each warp writes its answered records
+// (one store per lane and 8-byte word, no loads but node ids) and prepares its left-over reads (prepare_read), one after
+// the other, 32 lanes each. Persistent grid.
 static constexpr int kPrepExactThreads = 256;
-__global__ void __launch_bounds__(kPrepExactThreads) k_prepare_exact(const __grid_constant__ PrepExactArgs a) {
+static_assert(kPrepExactThreads == 256, "prep_stage_bytes sizes tiles of 256 reads");
+// MGB_PREP_TIMERS builds: a warp's sums of the phase cycles added to a.phase_out
+__device__ __forceinline__ void prep_timer_flush(const PrepExactArgs &a, const PrepTimer &tm) {
+#if defined(MGB_PREP_TIMERS)
+    for (int ph = 0; ph < PREP_N_PHASES; ++ph) {
+        unsigned long long v = (unsigned long long)tm.c[ph];
+        for (int d = 16; d; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+        if ((threadIdx.x & 31) == 0 && a.phase_out) atomicAdd(a.phase_out + ph, v);
+    }
+#else
+    (void)a; (void)tm;
+#endif
+}
+// 5 blocks per SM (<= 51 registers): more reads in flight; with fewer, the kernel is latency-bound (DESIGN.md §3.3)
+__global__ void __launch_bounds__(kPrepExactThreads, 5) k_prepare_exact(const __grid_constant__ PrepExactArgs a) {
     constexpr int kWarps = kPrepExactThreads / 32;
+    extern __shared__ uint4 s_tile[];                   // a.stage_bytes: the tile's raw characters
     __shared__ unsigned long long s_off[kWarps];
     __shared__ uint32_t s_bytes[kWarps], s_left[kWarps], s_slot[kWarps];
     const int lane = threadIdx.x & 31;
     const uint32_t n_reads = a.prep.n_reads;
+    PrepTimer tm;
     for (uint64_t base = (uint64_t)blockIdx.x * kPrepExactThreads; base < n_reads; base += (uint64_t)gridDim.x * kPrepExactThreads) {
+        tm.start();
+        // ---- the tile's bytes [offsets[base], offsets[end]) and the slack the word reads go past them, in 16-byte
+        // words from the one holding the first byte; a tile that does not fit is read from global memory instead
+        const uint64_t end = base + kPrepExactThreads < n_reads ? base + kPrepExactThreads : n_reads;
+        const uint64_t lo16 = a.prep.offsets[base] & ~15ull;
+        const uint64_t n16 = (((a.prep.offsets[end] + kPrepStageSlack + 15) & ~15ull) - lo16) >> 4;
+        const uint4 *src = reinterpret_cast<const uint4*>(a.prep.seqs + lo16);
+        const bool staged = n16 * 16 <= a.stage_bytes;
+        if (staged) {
+            #pragma unroll 4
+            for (uint32_t i = threadIdx.x; i < n16; i += kPrepExactThreads) s_tile[i] = __ldg(src + i);
+        }
+        __syncthreads();
+        const uint8_t *tile = reinterpret_cast<const uint8_t*>(staged ? s_tile : src);
+        tm.lap(PREP_STAGE);
         const uint32_t r = (uint32_t)(base + threadIdx.x);
-        uint64_t b = 0; int L = 0, s = -1; uint32_t p = 0; score_t score = 0;
-        if (r < n_reads) s = exact_path_strand(a, r, &b, &L, &p, &score);
+        const uint8_t *raw = nullptr;
+        int L = 0, s = -1; uint32_t p = 0; score_t score = 0;
+        if (r < n_reads) {
+            const uint64_t b = a.prep.offsets[r];
+            L = (int)(a.prep.offsets[r + 1] - b);
+            raw = tile + (b - lo16);
+            s = exact_path_strand(a, raw, L, &p, &score, tm);
+        }
+        tm.lap(PREP_TEXT);
         const uint32_t bytes = s >= 0 ? exact_read_bytes(a.ex, L) : 0u;
         const unsigned long long off = tile_alloc<kWarps>(bytes, a.ex.heap_used, s_bytes, s_off);
         if (s >= 0 && off + bytes > a.ex.heap_cap) s = -1;
         const bool left = r < n_reads && s < 0;
         const uint32_t slot = tile_alloc<kWarps>(left ? 1u : 0u, a.n_list, s_left, s_slot);
         if (left) a.list[slot] = r;
+        tm.lap(PREP_ALLOC);
+        // ---- the answered reads' headers, one per thread, then their records, a warp per record and a lane per word
+        if (s >= 0) exact_path_hdr(a.ex, r, L, off);
         for (unsigned todo = __ballot_sync(0xffffffffu, s >= 0); todo; todo &= todo - 1) {
             const int j = __ffs(todo) - 1;
-            exact_path_write(a, __shfl_sync(0xffffffffu, r, j), __shfl_sync(0xffffffffu, (unsigned long long)b, j),
+            exact_path_write(a, reinterpret_cast<const uint8_t*>(__shfl_sync(0xffffffffu, (unsigned long long)raw, j)),
                              __shfl_sync(0xffffffffu, L, j), __shfl_sync(0xffffffffu, s, j), __shfl_sync(0xffffffffu, p, j),
                              __shfl_sync(0xffffffffu, score, j), __shfl_sync(0xffffffffu, off, j), lane, 32);
         }
+        tm.lap(PREP_WRITE);
         for (unsigned todo = __ballot_sync(0xffffffffu, left); todo; todo &= todo - 1)
             prepare_read(a.prep, __shfl_sync(0xffffffffu, r, __ffs(todo) - 1));
+        __syncthreads();                                 // the tile's characters are read up to here
+        tm.lap(PREP_LEFT);
     }
+    prep_timer_flush(a, tm);
 }
 cudaError_t launch_prepare_exact(int num_sms, cudaStream_t s, const PrepExactArgs &a) {
     int per_sm = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_prepare_exact, kPrepExactThreads, 0);
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_prepare_exact, kPrepExactThreads, a.stage_bytes);
     if (e != cudaSuccess) return e;
     const uint64_t need = ((uint64_t)a.prep.n_reads + kPrepExactThreads - 1) / kPrepExactThreads;
     const uint64_t resident = (uint64_t)per_sm * num_sms;
     const unsigned grid = (unsigned)read_path_grid(need < resident ? need : resident);
     log_launch("k_prepare_exact", grid, kPrepExactThreads, (uint64_t)grid * kPrepExactThreads, a.prep.n_reads);
-    k_prepare_exact<<<grid, kPrepExactThreads, 0, s>>>(a);
+    k_prepare_exact<<<grid, kPrepExactThreads, a.stage_bytes, s>>>(a);
     return cudaGetLastError();
 }
 // round r (0-based) brings character k - 3 - r of every edge's k-mer to c_nxt[e]; kmer_shift = 2 * (k - 3 - r)
