@@ -299,6 +299,40 @@ struct mgb_results {
 };
 
 #if !defined(MGB_HOST_EMU)
+// IndexView::pl_word (0.5 bytes per position) and kh_pos (4 bytes per hash slot), the whole-read gate's leaner copies of
+// the path layout, once the layout is in place. Each is built only if half the device memory (at least 16 GB) stays
+// free after it: the aligner sizes its working memory from what is free, and on a 1 B-node graph (C3) the 6.2 GB of both
+// tables left an 80 GB H100 short at align time. Without them the gate reads the layout arrays. MGB_TEST_NO_LAYOUT_WORDS (test knob) leaves out kh_pos (value "kh_pos"),
+// pl_word ("pl_word") or both (any other value).
+static int build_layout_words(mgb_index *idx) {
+    IndexView &v = idx->view;
+    if (!v.pl_n || !v.kh_slots) return MGB_OK;
+    const char *no = std::getenv("MGB_TEST_NO_LAYOUT_WORDS");
+    const bool want_word = !no || !std::strcmp(no, "kh_pos"), want_pos = !no || !std::strcmp(no, "pl_word");
+    const uint64_t word_bytes = v.pl_n / 32 * 16, pos_bytes = v.kh_slots * 4;
+    ulonglong2 *pl_word = nullptr; uint32_t *kh_pos = nullptr;
+    size_t free_b = 0, total_b = 0;
+    cudaMemGetInfo(&free_b, &total_b);
+    double left = (double)free_b;
+    const double keep = std::max(16e9, 0.5 * (double)total_b);
+    if (want_word && left - word_bytes >= keep && cudaMalloc((void**)&pl_word, word_bytes) == cudaSuccess)
+        left -= word_bytes;
+    else pl_word = nullptr;
+    if (!want_pos || left - pos_bytes < keep || cudaMalloc((void**)&kh_pos, pos_bytes) != cudaSuccess) kh_pos = nullptr;
+    cudaGetLastError();
+    if (!pl_word && !kh_pos) return MGB_OK;
+    kern_dna::k_layout_words<<<(unsigned)idx->num_sms * 16, 256>>>(v, kh_pos, pl_word);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) {
+        cudaFree(pl_word); cudaFree(kh_pos);
+        return fail(MGB_ERR_CUDA, std::string("layout words: ") + cudaGetErrorString(e));
+    }
+    if (pl_word) { idx->bufs.push_back(pl_word); idx->device_bytes += word_bytes; v.pl_word = pl_word; }
+    if (kh_pos) { idx->bufs.push_back(kh_pos); idx->device_bytes += pos_bytes; v.kh_pos = kh_pos; }
+    return MGB_OK;
+}
+
 // Path layout of a graph with the k-mer hash index (IndexView::pl_*, kernels.cuh k_path_*), from the per-edge k-mers
 // of the hash build. Skipped, leaving the seeding walk as it is without it, when the device memory is not there (it
 // keeps the same 16 GB for the aligner's working memory as the hash index) or MGB_NO_PATH_INDEX is set.
@@ -380,7 +414,7 @@ static int build_path_layout(mgb_index *idx, const unsigned long long *kmer) {
     idx->view.pl_text = reinterpret_cast<const unsigned long long*>(a.text);
     idx->view.pl_rc = a.rc; idx->view.pl_stop = a.stop;
     idx->view.pl_n = n_pos;
-    return MGB_OK;
+    return build_layout_words(idx);
 }
 #endif
 
@@ -1450,24 +1484,37 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             a.nodes_f = b.nodes_f; a.nodes_r = b.nodes_r;
             a.sub_first_f = subk ? sk.first_f : nullptr; a.sub_last_f = sk.last_f; a.sub_len_f = subk ? sk.len_f : nullptr;
             a.sub_first_r = sk.first_r; a.sub_last_r = sk.last_r; a.sub_len_r = subk && both ? sk.len_r : nullptr;
-            a.read_list = d_list; a.n_list = (uint32_t)list.size();
+            a.read_list = d_list; a.n_list = (uint32_t)list.size(); a.n_list_dev = nullptr;
             a.arena = d_arena; a.arena_stride = stride;
             a.hdr = d_hdr; a.heap = d_heap; a.heap_cap = heap_cap; a.heap_used = d_used; a.next = d_next;
             unsigned long long used = 0;
 #if !defined(MGB_HOST_EMU)
             cudaEventRecord(ev[3], st.s);
 #endif
+            // reads k_align gets (after run_exact: known on the host once the pass is done, or at once when read back)
+            uint32_t n_align = a.n_list;
+            bool align_dev = false;         // k_align reads the length of its list from the device
             if (run_exact) {
-                // k_align takes only the reads left over; their count sizes its grid
+                // k_align takes only the reads left over. On pass 0 it reads their count from the device and the host
+                // launches the grid it sized for the whole list without waiting; retry passes read the count back
+                // and size the grid by it. MGB_DEBUG reads it back on pass 0 too, for its lines.
                 if ((rc = launch_exact_reads(index, ea, st))) break;
-                uint32_t n_rest[2] = { 0, 0 };          // and after k_prepare_exact, the length of its list
-                if ((rc = d2h(n_rest, d_next + 1, listed ? 8 : 4, st))) break;
 #if !defined(MGB_HOST_EMU)
-                CUDA_TRY(cudaStreamSynchronize(st.s));
+                align_dev = pass == 0;
 #endif
-                if (listed && dbg_time)
+                uint32_t n_rest[2] = { 0, 0 };          // and after k_prepare_exact, the length of its list
+                if (!align_dev || dbg_time) {
+                    if ((rc = d2h(n_rest, d_next + 1, listed ? 8 : 4, st))) break;
+#if !defined(MGB_HOST_EMU)
+                    CUDA_TRY(cudaStreamSynchronize(st.s));
+#endif
+                }
+                if (listed && dbg_time) {
                     std::fprintf(stderr, "[mgb] reads %u+%u k_prepare_exact answered %u, left over %u\n", lo, n_reads,
                                  n_reads - n_rest[1], n_rest[1]);
+                    std::fprintf(stderr, "[mgb] reads %u+%u k_exact_reads answered %u, left to k_align %u\n", lo, n_reads,
+                                 n_rest[1] - n_rest[0], n_rest[0]);
+                }
 #if defined(MGB_PREP_TIMERS) && !defined(MGB_HOST_EMU)
                 if (listed && dbg_time) {
                     unsigned long long ph[PREP_N_PHASES];
@@ -1479,7 +1526,10 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
                                  ph[PREP_WRITE] / nr, ph[PREP_LEFT] / nr);
                 }
 #endif
-                a.read_list = d_rest; a.n_list = n_rest[0];
+                a.read_list = d_rest;
+                if (align_dev) a.n_list_dev = d_next + 1;      // (a.n_list, the whole list's length, bounds it)
+                else a.n_list = n_rest[0];
+                n_align = n_rest[0];
                 res->stats.kernel_launches += 1;
             }
 #if defined(MGB_HOST_EMU)
@@ -1494,7 +1544,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             if (dbg_time) {         // every pass; per_round: warps launched, each aligning one read of the list at a time
                 char launched[128] = "";          // (one fprintf: pieces on two host threads print at once)
                 if (a.n_list) std::snprintf(launched, sizeof(launched), "; launch k_align grid=%u block=%d per_round=%llu items=%u",
-                                            grid, kern_dna::kAlignThreads, (unsigned long long)grid * wpb, a.n_list);
+                                            grid, kern_dna::kAlignThreads, (unsigned long long)grid * wpb, n_align);
                 std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident), arena %zu bytes per warp%s\n", n_warps,
                              (unsigned long long)index->num_sms * blocks_per_sm * wpb, stride, launched);
             }
@@ -1505,20 +1555,21 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             }
             cudaEventRecord(ev[4], st.s);
             if ((rc = d2h(&used, d_used, 8, st))) break;
+            if (align_dev && !dbg_time && (rc = d2h(&n_align, d_next + 1, 4, st))) break;
             CUDA_TRY(cudaStreamSynchronize(st.s));
             float ms = 0; cudaEventElapsedTime(&ms, ev[3], ev[4]); align_ms += ms;
             cudaEventRecord(ev[3], st.s);
 #endif
             tick("pass: h2d+seed+align kernels");
-            if (a.n_list) res->stats.kernel_launches += 1;
+            if (n_align) res->stats.kernel_launches += 1;       // (a k_align over an empty list aligns nothing)
 #if defined(MGB_PHASE_TIMERS) && !defined(MGB_HOST_EMU)
             {
                 unsigned long long ph[8];
                 cudaMemcpy(ph, a.phase_out, 64, cudaMemcpyDeviceToHost);
                 std::fprintf(stderr, "[phase cycles/read] setup %.0f seeds %.0f fwd %.0f backtrack %.0f align_total %.0f; columns/read: register path %.1f, general path %.1f (reads %u)\n",
-                             (double)ph[0] / a.n_list, (double)ph[1] / a.n_list, (double)ph[2] / a.n_list,
-                             (double)ph[3] / a.n_list, (double)ph[4] / a.n_list, (double)ph[5] / a.n_list,
-                             (double)ph[6] / a.n_list, a.n_list);
+                             (double)ph[0] / n_align, (double)ph[1] / n_align, (double)ph[2] / n_align,
+                             (double)ph[3] / n_align, (double)ph[4] / n_align, (double)ph[5] / n_align,
+                             (double)ph[6] / n_align, n_align);
             }
 #endif
             if (used > heap_cap) used = heap_cap;

@@ -18,6 +18,7 @@
 
 #if !defined(__CUDACC__)
 struct uint2 { uint32_t x, y; };
+struct alignas(16) ulonglong2 { unsigned long long x, y; };
 #endif
 
 namespace mgb {
@@ -70,11 +71,18 @@ struct IndexView {
     //   pl_stop     1 bit per position: pl_node[p] == 0
     //   pl_pos[e]   the position of edge e, kPlNone unless e is a DBG node
     // The arrays end with at least kPlPad filler positions, so readers may run ahead of a path's end.
+    // Two leaner copies for the whole-read gate (exact_path_strand), nullptr when the memory is not there (or the layout
+    // is absent); every reader falls back to the arrays above:
+    //   kh_pos[i]   per hash slot: pl_pos[kh_vals[i]] of an in_graph edge, else kPlNone (an empty slot too)
+    //   pl_word[w]  positions 32w .. 32w + 31 in one 16-byte word: x = pl_text[w], y = pl_stop[w] | pl_rc[w] (high
+    //               half 0), over the same pl_n positions
     const uint32_t *pl_node;
     const uint32_t *pl_pos;
     const unsigned long long *pl_text;
     const uint32_t *pl_rc;
     const uint32_t *pl_stop;
+    const uint32_t *kh_pos;
+    const ulonglong2 *pl_word;
     uint64_t pl_n;
     uint64_t n;                 // number of edges (ids 1..n)
     uint32_t nblk;

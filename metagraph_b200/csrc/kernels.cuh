@@ -141,6 +141,7 @@ struct AlignArgs {
     const uint32_t *sub_first_f, *sub_last_f, *sub_first_r, *sub_last_r;    // k_subk results or nullptr
     const uint8_t *sub_len_f, *sub_len_r;
     const uint32_t *read_list; uint32_t n_list;
+    const unsigned int *n_list_dev;   // non-null: the list's length is *n_list_dev (<= n_list), written by an earlier kernel
     char *arena; size_t arena_stride;
     ReadHdr *hdr; char *heap; uint64_t heap_cap; unsigned long long *heap_used;
     unsigned int *next;
@@ -427,11 +428,20 @@ MGB_HD unsigned long long ldg64(const unsigned long long *p) {
     return *p;
 #endif
 }
+MGB_HD ulonglong2 ldg128(const ulonglong2 *p) {
+#if MGB_DEVICE_CODE
+    return __ldg(p);
+#else
+    return *p;
+#endif
+}
 // The primary strand (0 / 1) of a read if it is answered here (conditions above), else -1; raw / n: its characters
 // and length, *pos: its place p on the path, *score: the alignment's score. One lane, no collectives. The characters
 // are read as aligned 4-byte words (acgt_pack32: up to 35 bytes past the read must be readable) and handled as 2-bit
 // codes 32 at a time; both strands run the same word operations. The path layout is read in chunks of kPathChunk
-// characters, all words of a chunk loaded before any is used.
+// characters, all words of a chunk loaded before any is used. With kh_pos and pl_word (IndexView) a read's index
+// accesses are the two buckets, one kh_pos entry and one 16-byte pl_word per 32 positions, three dependent steps;
+// without them, kh_vals then pl_pos, and pl_stop, pl_rc and pl_text words apart.
 static constexpr int kPathChunk = 160;
 static constexpr int kChunkWords = kPathChunk / 32;
 MGB_HD int exact_path_strand(const PrepExactArgs &a, const uint8_t *raw, int n, uint32_t *pos, score_t *score,
@@ -445,22 +455,32 @@ MGB_HD int exact_path_strand(const PrepExactArgs &a, const uint8_t *raw, int n, 
     const unsigned long long kf = acgt_pack32(raw, &inv) & codes_mask(K);
     const unsigned long long kr = rc_codes32(acgt_pack32(raw + (n - K), &inv)) >> (2 * (32 - K));
     tm.lap(PREP_KEYS);
-    uint64_t ef, er;
+    int s;
+    uint32_t p;
 #if MGB_DEVICE_CODE
     {
         KhProbe pf, pr;                                     // both lookups in flight
         pf.issue(ix, kf, true); pr.issue(ix, kr, true);
         pf.find(ix); pr.find(ix);
-        ef = pf.value(ix); er = pr.value(ix);
+        if ((pf.h >= 0) == (pr.h >= 0)) return -1;          // (a found k-mer's edge is never 0)
+        s = pf.h >= 0 ? 0 : 1;
+        const uint64_t i = s ? pr.slot + pr.h : pf.slot + pf.h;
+        if (ix.kh_pos) {
+            p = __ldg(ix.kh_pos + i);
+        } else {
+            const uint64_t e = __ldg(ix.kh_vals + i);
+            p = in_graph(ix, e) ? __ldg(ix.pl_pos + e) : kPlNone;
+        }
     }
 #else
-    ef = kh_lookup(ix, kf); er = kh_lookup(ix, kr);
+    {
+        const uint64_t ef = kh_lookup(ix, kf), er = kh_lookup(ix, kr);
+        if ((ef != 0) == (er != 0)) return -1;
+        s = ef ? 0 : 1;
+        const uint64_t e = s ? er : ef;
+        p = in_graph(ix, e) ? ix.pl_pos[e] : kPlNone;
+    }
 #endif
-    if ((ef != 0) == (er != 0)) return -1;
-    const int s = ef ? 0 : 1;
-    const uint64_t e = s ? er : ef;
-    if (!in_graph(ix, e)) return -1;
-    const uint32_t p = ldg32(ix.pl_pos + e);
     tm.lap(PREP_LOOKUP);
     if (p == kPlNone) return -1;
     const int nk = n - K + 1;
@@ -471,16 +491,33 @@ MGB_HD int exact_path_strand(const PrepExactArgs &a, const uint8_t *raw, int n, 
         const uint32_t P = p + (uint32_t)i0, w0 = P >> 5;
         const uint32_t se = p + (uint32_t)(i0 + kPathChunk < nk ? i0 + kPathChunk : nk);
         const uint32_t te = p + (uint32_t)(i0 + kPathChunk < n ? i0 + kPathChunk : n);
-        uint32_t st[kChunkWords + 1], rc[kChunkWords + 1];
+        uint32_t sr[kChunkWords + 1];                       // pl_stop | pl_rc
         unsigned long long tx[kChunkWords + 1];
+        if (ix.pl_word) {
 #if MGB_DEVICE_CODE
-        #pragma unroll
+            #pragma unroll
 #endif
-        for (int t = 0; t <= kChunkWords; ++t) {
-            const uint32_t q = (w0 + (uint32_t)t) << 5;
-            st[t] = q < se ? ldg32(ix.pl_stop + w0 + t) : 0u;
-            rc[t] = q < se ? ldg32(ix.pl_rc + w0 + t) : 0u;
-            tx[t] = q < te ? ldg64(ix.pl_text + w0 + t) : 0ull;
+            for (int t = 0; t <= kChunkWords; ++t) {
+                const uint32_t q = (w0 + (uint32_t)t) << 5;
+                const ulonglong2 w = q < te ? ldg128(ix.pl_word + w0 + t) : ulonglong2{ 0ull, 0ull };
+                tx[t] = w.x;
+                sr[t] = q < se ? (uint32_t)w.y : 0u;
+            }
+        } else {
+            uint32_t st[kChunkWords + 1], rc[kChunkWords + 1];
+#if MGB_DEVICE_CODE
+            #pragma unroll
+#endif
+            for (int t = 0; t <= kChunkWords; ++t) {
+                const uint32_t q = (w0 + (uint32_t)t) << 5;
+                st[t] = q < se ? ldg32(ix.pl_stop + w0 + t) : 0u;
+                rc[t] = q < se ? ldg32(ix.pl_rc + w0 + t) : 0u;
+                tx[t] = q < te ? ldg64(ix.pl_text + w0 + t) : 0ull;
+            }
+#if MGB_DEVICE_CODE
+            #pragma unroll
+#endif
+            for (int t = 0; t <= kChunkWords; ++t) sr[t] = st[t] | rc[t];
         }
         uint32_t stop = 0;
 #if MGB_DEVICE_CODE
@@ -491,7 +528,7 @@ MGB_HD int exact_path_strand(const PrepExactArgs &a, const uint8_t *raw, int n, 
             if (q < se) {
                 uint32_t m = q < P ? ~0u << (P - q) : ~0u;
                 if (se - q < 32) m &= (1u << (se - q)) - 1u;
-                stop |= (st[t] | rc[t]) & m;
+                stop |= sr[t] & m;
             }
         }
         tm.lap(PREP_STOPRC);
@@ -1191,8 +1228,17 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
 #endif
 static constexpr int kAlignThreads = MGB_ALIGN_THREADS;
 static constexpr int kWarpsPerBlock = kAlignThreads / kWarp;   // reads in flight per block of k_align
-// one warp per read
+// one warp per read; a warp that finds the list done before its first read touches nothing (the host may launch more
+// warps than a list whose length only the device knows needs)
+__device__ __forceinline__ unsigned int align_take(const AlignArgs &a) {
+    unsigned int t = 0;
+    if (wlane() == 0) t = atomicAdd(a.next, 1u);
+    return wbcast(t, 0);
+}
 __global__ void __launch_bounds__(kAlignThreads, MGB_ALIGN_MIN_BLOCKS) k_align(const __grid_constant__ AlignArgs a) {
+    const uint32_t n_list = a.n_list_dev ? __ldg(a.n_list_dev) : a.n_list;
+    unsigned int t = align_take(a);
+    if (t >= n_list) return;
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) / kWarp;
     char *arena = a.arena + (size_t)warp * a.arena_stride;
     extern __shared__ __align__(16) char smem_raw[];
@@ -1201,13 +1247,7 @@ __global__ void __launch_bounds__(kAlignThreads, MGB_ALIGN_MIN_BLOCKS) k_align(c
     // the warp's arena and on-chip working set: base + offsets from the kernel parameters
     const WarpMem mem { arena, &a.lay };
     const WarpSmem sm { smem, &a.slay };
-    while (true) {
-        unsigned int t = 0;
-        if (wlane() == 0) t = atomicAdd(a.next, 1u);
-        t = wbcast(t, 0);
-        if (t >= a.n_list) break;
-        align_read(a, a.read_list[t], mem, sm);
-    }
+    for (; t < n_list; t = align_take(a)) align_read(a, a.read_list[t], mem, sm);
 }
 
 // Grid of a read-path kernel (k_prepare, k_prepare_exact, k_premap, k_seed, k_seed_hash, k_subk, k_exact_reads, k_align):
@@ -1668,6 +1708,21 @@ __global__ void __launch_bounds__(256) k_path_place(PathArgs a) {
     }
 }
 #undef MGB_EDGE_LOOP
+// IndexView::kh_pos and pl_word from the finished hash index and path layout in `ix` (either output may be null: not
+// built)
+__global__ void __launch_bounds__(256) k_layout_words(IndexView ix, uint32_t *kh_pos, ulonglong2 *pl_word) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, nt = (uint64_t)gridDim.x * blockDim.x;
+    if (kh_pos) {
+        for (uint64_t i = t; i < ix.kh_slots; i += nt) {
+            const uint64_t e = ix.kh_keys[i] ? ix.kh_vals[i] : 0u;
+            kh_pos[i] = in_graph(ix, e) ? ix.pl_pos[e] : kPlNone;
+        }
+    }
+    if (pl_word) {
+        for (uint64_t w = t; w < ix.pl_n / 32; w += nt)
+            pl_word[w] = make_ulonglong2(ix.pl_text[w], ix.pl_stop[w] | ix.pl_rc[w]);
+    }
+}
 __global__ void __launch_bounds__(256) k_radj_pack(RadjArgs a, uint32_t multi_shift) {
     uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     uint64_t nt = (uint64_t)gridDim.x * blockDim.x;
