@@ -1269,6 +1269,9 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
         if (!rc && both) rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, st);
         ReadHdr *d_hdr = nullptr;
         if (!rc) rc = bufs.alloc(&d_hdr, (size_t)n_reads + 1);
+#if defined(MGB_PROBE_NO_WRITES)
+        if (!rc) rc = dev_zero(d_hdr, ((size_t)n_reads + 1) * sizeof(ReadHdr), st);     // k_prepare_exact stores none
+#endif
         // query length k_align stages on chip (0: none; MGB_TEST_LQ: test knob that forces the unstaged path)
         const int lq = b.L_max + 1 <= 512 ? (int)((b.L_max + 1 + 15) & ~15u) : 0;
         int lq_v = lq;

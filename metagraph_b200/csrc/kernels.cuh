@@ -465,12 +465,18 @@ MGB_HD int exact_path_strand(const PrepExactArgs &a, const uint8_t *raw, int n, 
         if ((pf.h >= 0) == (pr.h >= 0)) return -1;          // (a found k-mer's edge is never 0)
         s = pf.h >= 0 ? 0 : 1;
         const uint64_t i = s ? pr.slot + pr.h : pf.slot + pf.h;
+#if defined(MGB_PROBE_NO_LAYOUT)
+        // probe build (scripts/build_variant.sh), wrong results by design: no load after the buckets (no kh_pos,
+        // kh_vals, pl_pos or layout words), every read whose primary k-mer is found passes the layout checks at p = 0
+        p = 0; (void)i;
+#else
         if (ix.kh_pos) {
             p = __ldg(ix.kh_pos + i);
         } else {
             const uint64_t e = __ldg(ix.kh_vals + i);
             p = in_graph(ix, e) ? __ldg(ix.pl_pos + e) : kPlNone;
         }
+#endif
     }
 #else
     {
@@ -493,6 +499,10 @@ MGB_HD int exact_path_strand(const PrepExactArgs &a, const uint8_t *raw, int n, 
         const uint32_t te = p + (uint32_t)(i0 + kPathChunk < n ? i0 + kPathChunk : n);
         uint32_t sr[kChunkWords + 1];                       // pl_stop | pl_rc
         unsigned long long tx[kChunkWords + 1];
+#if defined(MGB_PROBE_NO_LAYOUT) && MGB_DEVICE_CODE
+        (void)se; (void)te;
+        for (int t = 0; t <= kChunkWords; ++t) { tx[t] = 0ull; sr[t] = 0u; }
+#else
         if (ix.pl_word) {
 #if MGB_DEVICE_CODE
             #pragma unroll
@@ -519,6 +529,7 @@ MGB_HD int exact_path_strand(const PrepExactArgs &a, const uint8_t *raw, int n, 
 #endif
             for (int t = 0; t <= kChunkWords; ++t) sr[t] = st[t] | rc[t];
         }
+#endif
         uint32_t stop = 0;
 #if MGB_DEVICE_CODE
         #pragma unroll
@@ -557,6 +568,9 @@ MGB_HD int exact_path_strand(const PrepExactArgs &a, const uint8_t *raw, int n, 
             }
         }
         tm.lap(PREP_TEXT);
+#if defined(MGB_PROBE_NO_LAYOUT) && MGB_DEVICE_CODE
+        diff = 0;
+#endif
         if (stop || bad || diff) return -1;
     }
     const score_t full = cnt[0] * a.ex.diag['A'] + cnt[1] * a.ex.diag['C'] + cnt[2] * a.ex.diag['G']
@@ -600,13 +614,15 @@ MGB_HD void exact_path_write(const PrepExactArgs &a, const uint8_t *raw, int L, 
     const uint32_t nw = exact_read_bytes(a.ex, L) / 8;
     for (uint32_t wi = (uint32_t)lane; wi < nw; wi += (uint32_t)width) o[wi] = exact_path_word(a, raw, L, s, p, score, wi);
 }
-// ... and its header, exact_record_write's
+// ... and word qi (< 5) of its header, exact_record_write's: status, n_aln | heap_off | num_seeds, num_extensions |
+// num_explored_nodes, dp_columns | dp_cells
+static_assert(sizeof(ReadHdr) == 40 && MGB_READ_OK == 0, "ReadHdr is five words");
+MGB_HD unsigned long long exact_path_hdr_word(const ExactArgs &a, int L, uint64_t off, int qi) {
+    return qi == 0 ? 1ull << 32 : qi == 1 ? off : qi == 2 ? (uint32_t)(L - (int)a.k + 1) | 1ull << 32 : 0ull;
+}
 MGB_HD void exact_path_hdr(const ExactArgs &a, uint32_t r, int L, uint64_t off) {
-    ReadHdr h;
-    h.status = MGB_READ_OK; h.n_aln = 1; h.heap_off = off;
-    h.stats.num_seeds = (uint32_t)(L - (int)a.k + 1); h.stats.num_extensions = 1;
-    h.stats.num_explored_nodes = 0; h.stats.dp_columns = 0; h.stats.dp_cells = 0;
-    a.hdr[r] = h;
+    unsigned long long *h = reinterpret_cast<unsigned long long*>(a.hdr + r);
+    for (int qi = 0; qi < 5; ++qi) h[qi] = exact_path_hdr_word(a, L, off, qi);
 }
 
 // One refinement level of the suffix-range table (boss.hpp:651-655 index order: the appended
@@ -1438,10 +1454,18 @@ __device__ __forceinline__ C tile_alloc(uint32_t v, C *ctr, uint32_t *s_sum, C *
 // reads per block and round, one read per thread. The block first copies the tile's characters to shared memory with
 // coalesced 16-byte loads (a tile longer than a.stage_bytes is read from global memory through the same code). The
 // answered reads of a tile take one heap allocation (a record that does not fit makes its read a left-over one), the
-// left-over reads one append to a.list; each thread writes its read's header, then each warp writes its answered records
-// (one store per lane and 8-byte word, no loads but node ids) and prepares its left-over reads (prepare_read), one after
-// the other, 32 lanes each. Persistent grid.
+// left-over reads one append to a.list. A warp whose reads are all answered with records of one size writes its headers
+// and records as runs of words across its lanes (no loads but node ids; DESIGN.md §3.3); other warps write a header per
+// thread and the records one after the other, 32 lanes each. Each warp then prepares its left-over reads (prepare_read),
+// one after the other. Persistent grid.
 static constexpr int kPrepExactThreads = 256;
+#if defined(MGB_PROBE_NO_WRITES)
+// probe build (scripts/build_variant.sh), wrong results by design: no header or record stores (the host zeroes the
+// headers, so every answered read comes back with no alignment)
+static constexpr bool kPrepWrites = false;
+#else
+static constexpr bool kPrepWrites = true;
+#endif
 static_assert(kPrepExactThreads == 256, "prep_stage_bytes sizes tiles of 256 reads");
 // MGB_PREP_TIMERS builds: a warp's sums of the phase cycles added to a.phase_out
 __device__ __forceinline__ void prep_timer_flush(const PrepExactArgs &a, const PrepTimer &tm) {
@@ -1497,13 +1521,62 @@ __global__ void __launch_bounds__(kPrepExactThreads, 5) k_prepare_exact(const __
         const uint32_t slot = tile_alloc<kWarps>(left ? 1u : 0u, a.n_list, s_left, s_slot);
         if (left) a.list[slot] = r;
         tm.lap(PREP_ALLOC);
-        // ---- the answered reads' headers, one per thread, then their records, a warp per record and a lane per word
-        if (s >= 0) exact_path_hdr(a.ex, r, L, off);
-        for (unsigned todo = __ballot_sync(0xffffffffu, s >= 0); todo; todo &= todo - 1) {
-            const int j = __ffs(todo) - 1;
-            exact_path_write(a, reinterpret_cast<const uint8_t*>(__shfl_sync(0xffffffffu, (unsigned long long)raw, j)),
-                             __shfl_sync(0xffffffffu, L, j), __shfl_sync(0xffffffffu, s, j), __shfl_sync(0xffffffffu, p, j),
-                             __shfl_sync(0xffffffffu, score, j), __shfl_sync(0xffffffffu, off, j), lane, 32);
+        // ---- the answered reads' headers and records. The allocation goes in thread order, so a warp's answered
+        // records are one run of the heap. A warp whose 32 reads are all answered with records of one size (without
+        // node ids: lengths that round up to one multiple of 8) writes its headers as one run of 16-byte chunks, each
+        // lane its own record's OutAln, and the rest of its records as one run of 8-byte words from lane 0's offset,
+        // lane i words i, i + 32, ...; other warps write a header per thread and the records one after the other.
+        const unsigned ans = __ballot_sync(0xffffffffu, s >= 0);
+        const uint32_t R = __shfl_sync(0xffffffffu, bytes, 0);
+        unsigned long long *hw = reinterpret_cast<unsigned long long*>(a.ex.hdr + (r - lane));
+        if (kPrepWrites && __all_sync(0xffffffffu, s >= 0 && bytes == R) && ((uintptr_t)hw & 15) == 0) {
+            // the header array and so the warp's 1280 bytes of headers start on a 16-byte boundary
+            #pragma unroll
+            for (int c = lane; c < 96; c += 32) {                    // 80 chunks; every lane takes part in the shuffles
+                const int q = c < 80 ? 2 * c : 0, i0 = q / 5, i1 = (q + 1) / 5;
+                ulonglong2 v;
+                v.x = exact_path_hdr_word(a.ex, __shfl_sync(0xffffffffu, L, i0), __shfl_sync(0xffffffffu, off, i0), q % 5);
+                v.y = exact_path_hdr_word(a.ex, __shfl_sync(0xffffffffu, L, i1), __shfl_sync(0xffffffffu, off, i1),
+                                          (q + 1) % 5);
+                if (c < 80) reinterpret_cast<ulonglong2*>(hw)[c] = v;
+            }
+            // each lane its own record's OutAln (words 0-3); then word g of the records' words 4 .. nw - 1 is word
+            // 4 + g % nb of lane g / nb's record, every lane taking nb of them (past word 0 the score is not used)
+            unsigned long long *o = reinterpret_cast<unsigned long long*>(a.ex.heap + off);
+            const ulonglong2 h0 = make_ulonglong2(exact_path_word(a, raw, L, s, p, score, 0), exact_path_word(a, raw, L, s, p, score, 1));
+            const ulonglong2 h1 = make_ulonglong2(exact_path_word(a, raw, L, s, p, score, 2), exact_path_word(a, raw, L, s, p, score, 3));
+            if (((uintptr_t)o & 15) == 0) {
+                reinterpret_cast<ulonglong2*>(o)[0] = h0; reinterpret_cast<ulonglong2*>(o)[1] = h1;
+            } else {
+                o[0] = h0.x; o[1] = h0.y; o[2] = h1.x; o[3] = h1.y;
+            }
+            o = reinterpret_cast<unsigned long long*>(a.ex.heap + __shfl_sync(0xffffffffu, off, 0)) + 4;
+            // each word's record: its read's place in the tile, and its length and strand, from the record's lane. They
+            // go in one shuffle when both fit in 16 bits: a staged tile is smaller than 64 KB, and every L is below R
+            // (warp-uniform, so is the choice)
+            const uint32_t ro = (uint32_t)(raw - tile), ls = (uint32_t)L << 1 | (uint32_t)s, nw = R >> 3, nb = nw - 4;
+            const bool packed = staged && R < (1u << 15);
+            uint32_t j = (uint32_t)lane / nb, wi = (uint32_t)lane - j * nb;
+            for (uint32_t g = (uint32_t)lane; g < 32 * nb; g += 32) {
+                uint32_t rj, lj;
+                if (packed) {
+                    const uint32_t x = __shfl_sync(0xffffffffu, ro << 16 | ls, j);
+                    rj = x >> 16; lj = x & 0xFFFFu;
+                } else {
+                    rj = __shfl_sync(0xffffffffu, ro, j); lj = __shfl_sync(0xffffffffu, ls, j);
+                }
+                const uint32_t pj = a.ex.result_nodes ? 0u : __shfl_sync(0xffffffffu, p, j);
+                o[j * nw + wi] = exact_path_word(a, tile + rj, (int)(lj >> 1), (int)(lj & 1u), pj, 0, 4 + wi);
+                for (wi += 32; wi >= nb; wi -= nb) ++j;
+            }
+        } else if (kPrepWrites && ans) {
+            if (s >= 0) exact_path_hdr(a.ex, r, L, off);
+            for (unsigned todo = ans; todo; todo &= todo - 1) {
+                const int j = __ffs(todo) - 1;
+                exact_path_write(a, reinterpret_cast<const uint8_t*>(__shfl_sync(0xffffffffu, (unsigned long long)raw, j)),
+                                 __shfl_sync(0xffffffffu, L, j), __shfl_sync(0xffffffffu, s, j), __shfl_sync(0xffffffffu, p, j),
+                                 __shfl_sync(0xffffffffu, score, j), __shfl_sync(0xffffffffu, off, j), lane, 32);
+            }
         }
         tm.lap(PREP_WRITE);
         for (unsigned todo = __ballot_sync(0xffffffffu, left); todo; todo &= todo - 1)

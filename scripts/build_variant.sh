@@ -1,6 +1,10 @@
 #!/bin/bash
 # builds metagraph_b200/_lib/libmgb_<tag>.so with extra nvcc flags (probes of kernel variants; select with MGB_LIB)
 #   scripts/build_variant.sh timers -DMGB_PHASE_TIMERS
+#   scripts/build_variant.sh prep -DMGB_PREP_TIMERS          (k_prepare_exact's phase split, printed under MGB_DEBUG)
+# Probes that bound a phase of k_prepare_exact by leaving it out (wrong results by design; time them with
+# scripts/kernel_split.py): -DMGB_PROBE_NO_WRITES (no header or record stores), -DMGB_PROBE_NO_LAYOUT (no load after the
+# hash buckets: no kh_pos, kh_vals / pl_pos or layout words; every read whose k-mer is found passes at p = 0)
 set -e
 tag=$1; shift
 cd "$(dirname "$0")/.."
