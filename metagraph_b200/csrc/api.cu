@@ -10,6 +10,7 @@
 #include <atomic>
 #include <thread>
 #include <chrono>
+#include <cctype>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -824,7 +825,9 @@ int launch_seed(const mgb_index_t *index, const Batch &b, uint32_t n_strands, St
                 uint8_t *summary, uint64_t *n_launches = nullptr, const uint32_t *list = nullptr,
                 const unsigned int *n_list = nullptr) {
     SeedArgs a { index->view, b.cf, b.cr, b.offsets, b.koff, b.nodes_f, b.nodes_r, b.n_reads, n_strands, 0, nullptr, nullptr,
-                 summary, list, n_list };
+                 summary, list, n_list, 0 };
+    // MGB_TEST_SEED_MODE=walk|wide: test knob, k_seed_hash's walk or short-list mode whatever the list's length
+    if (const char *e = std::getenv("MGB_TEST_SEED_MODE")) a.seed_mode = !std::strcmp(e, "walk") ? 1 : !std::strcmp(e, "wide") ? 2 : 0;
     uint64_t items = (uint64_t)b.n_reads * n_strands;
     // first pass (k_premap): rules out the k-mers the suffix-range table has no node for; the node arrays
     // are zero-filled, so the second pass only visits what is left
@@ -1179,6 +1182,95 @@ struct Piece {
     ~Piece() { for (HostBuf b : heaps) hostbuf_release(b); if (text.p) hostbuf_release(text); }
 };
 
+// MGB_DEBUG, when k_prepare_exact ran and at most 8 reads reach k_align on pass 0: one line per such read with what
+// turned it down at each whole-read gate, read back from the device. exact_path_strand (kernels.cuh, conditions 1-4):
+// the length limit, whether the position-0 k-mer of each strand has a node (f0 / r0), the primary's place p on the path,
+// the first k-mer offset from p with a pl_stop or pl_rc bit, the first character that is not A/C/G/T or differs from
+// pl_text, and the score. exact_read_strand: the length limit, the summary bits (answered only as 0x6 or 0x9) and the
+// score against the threshold. Host code, never on a timed path.
+static void debug_left_over(const IndexView &ix, const PrepExactArgs &pa, const ExactArgs &ea, const char *seqs,
+                            const uint64_t *offsets, const std::vector<uint64_t> &koff, const Batch &b,
+                            const uint8_t *summary, const uint32_t *d_rest, uint32_t n, uint32_t lo, uint32_t n_reads,
+                            Stream &st) {
+    std::vector<uint32_t> rest(n);
+    if (d2h(rest.data(), d_rest, 4ull * n, st)) return;
+#if !defined(MGB_HOST_EMU)
+    if (cudaStreamSynchronize(st.s) != cudaSuccess) return;
+#endif
+    const int k = (int)ix.k;
+    for (uint32_t r : rest) {
+        const char *raw = seqs + offsets[r];
+        const int L = (int)(offsets[r + 1] - offsets[r]), nk = L - k + 1;
+        std::string path = "length", read = "length";
+        uint8_t bits = 0;
+        if (summary) d2h(&bits, summary + r, 1, st);
+        uint64_t n0[2] = { 0, 0 };
+        uint32_t p = kPlNone;
+        if (nk > 0) {
+            d2h(&n0[0], b.nodes_f + koff[r], 8, st);
+            d2h(&n0[1], b.nodes_r + koff[r], 8, st);
+        }
+#if !defined(MGB_HOST_EMU)
+        cudaStreamSynchronize(st.s);
+#endif
+        const int s = (n0[0] != 0) == (n0[1] != 0) ? -1 : n0[0] ? 0 : 1;
+        // the primary strand's characters, upper case (N: not A/C/G/T); Σ diag over them
+        std::string q(L > 0 ? L : 0, 'N');
+        for (int i = 0; i < L; ++i) {
+            const char c = (char)std::toupper((unsigned char)(s == 1 ? raw[L - 1 - i] : raw[i]));
+            const char *at = std::strchr("ACGT", c);
+            q[i] = !c || !at ? 'N' : s == 1 ? "TGCA"[at - "ACGT"] : c;
+        }
+        long score = ea.end_bonus;
+        for (char c : q) score += ea.diag[(uint8_t)c & 0x7F];
+        if (nk > 0 && L <= (int)pa.ex.max_len) {
+            if (s < 0) {
+                path = "probe";
+            } else {
+                if (ix.pl_n) d2h(&p, ix.pl_pos + n0[s], 4, st);
+#if !defined(MGB_HOST_EMU)
+                cudaStreamSynchronize(st.s);
+#endif
+                if (p == kPlNone) {
+                    path = "no path position";
+                } else {
+                    const uint32_t w0 = p >> 5, w1 = (p + (uint32_t)L + 31) >> 5;
+                    std::vector<uint32_t> sw(w1 - w0 + 1), rw(w1 - w0 + 1);
+                    std::vector<unsigned long long> tw(w1 - w0 + 1);
+                    d2h(sw.data(), ix.pl_stop + w0, 4ull * sw.size(), st);
+                    d2h(rw.data(), ix.pl_rc + w0, 4ull * rw.size(), st);
+                    d2h(tw.data(), ix.pl_text + w0, 8ull * tw.size(), st);
+#if !defined(MGB_HOST_EMU)
+                    cudaStreamSynchronize(st.s);
+#endif
+                    int stop = -1, rcb = -1, bad = -1, diff = -1;
+                    for (int t = nk - 1; t >= 0; --t) {
+                        const uint32_t x = p + (uint32_t)t - (w0 << 5);
+                        if ((sw[x >> 5] >> (x & 31)) & 1u) stop = t;
+                        if ((rw[x >> 5] >> (x & 31)) & 1u) rcb = t;
+                    }
+                    for (int i = L - 1; i >= 0; --i) {
+                        const char *acgt = std::strchr("ACGT", q[i]);
+                        const uint32_t x = p + (uint32_t)i - (w0 << 5);
+                        if (q[i] == 'N') bad = i;
+                        else if ((int)((tw[x >> 5] >> (2 * (x & 31))) & 3u) != (int)(acgt - "ACGT")) diff = i;
+                    }
+                    char buf[160];
+                    std::snprintf(buf, sizeof(buf), "p=%u stop@%d rc@%d invalid@%d mismatch@%d", p, stop, rcb, bad, diff);
+                    path = stop >= 0 || rcb >= 0 || bad >= 0 || diff >= 0 ? buf
+                         : score < pa.ex.min_score ? std::string(buf) + " threshold" : std::string(buf) + " (answers)";
+                }
+            }
+        }
+        if (nk > 0 && L <= (int)ea.max_len) {
+            read = bits == 0x6 || bits == 0x9 ? (score < ea.min_score ? "threshold" : "(answers)") : "summary bits";
+        }
+        std::fprintf(stderr, "[mgb] reads %u+%u left to k_align: read %u L=%d f0=%d r0=%d | exact_path_strand: %s | "
+                     "exact_read_strand: summary=0x%x score=%ld min=%d: %s\n", lo, n_reads, r, L,
+                     n0[0] != 0, n0[1] != 0, path.c_str(), bits, score, ea.min_score, read.c_str());
+    }
+}
+
 static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const char *all_seqs,
                        const uint64_t *all_offsets, uint32_t lo, uint32_t n_reads, Piece *res) {
     // MGB_DEBUG=1: wall-clock split of the call on stderr
@@ -1380,11 +1472,15 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
 #endif
 
         // align passes: all reads with scale 1, overflowed reads again with larger arenas
-        std::vector<uint32_t> list(n_reads);
-        for (uint32_t r = 0; r < n_reads; ++r) list[r] = r;
+        // The pass's reads. Pass 0 after k_prepare_exact takes its list from the device and needs the host's copy of all
+        // n_reads only once it is done: filling it first would delay the launches behind it.
+        std::vector<uint32_t> list;
+        auto all_reads = [&] { list.resize(n_reads); for (uint32_t r = 0; r < n_reads; ++r) list[r] = r; };
+        if (!prep_exact) all_reads();
+        uint32_t n_pass = n_reads;
         uint32_t scale = 1;
         float align_ms = 0, d2h_ms = 0; (void)align_ms; (void)d2h_ms;
-        for (int pass = 0; !rc && !list.empty(); ++pass, scale *= 4) {
+        for (int pass = 0; !rc && n_pass; ++pass, scale *= 4) {
             if (pass == 6) { rc = fail(MGB_ERR_OVERFLOW, "a read exceeded the largest per-read work arena"); break; }
             Caps caps = choose_caps(b.L_max, dcfg, index->view.k, scale);
             size_t stride = arena_bytes(caps);
@@ -1437,13 +1533,13 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
                 if (mem_warps < wpb) mem_warps = wpb;
                 if (n_warps64 > mem_warps) n_warps64 = mem_warps / wpb * wpb;
             }
-            if (n_warps64 > ((uint64_t)list.size() + wpb - 1) / wpb * wpb) n_warps64 = ((uint64_t)list.size() + wpb - 1) / wpb * wpb;
+            if (n_warps64 > ((uint64_t)n_pass + wpb - 1) / wpb * wpb) n_warps64 = ((uint64_t)n_pass + wpb - 1) / wpb * wpb;
             n_warps64 = kern_dna::read_path_grid(n_warps64 / wpb) * wpb;    // (MGB_TEST_MAX_BLOCKS)
             uint32_t n_warps = (uint32_t)n_warps64;
 #endif
             // pass 0 after k_prepare_exact: its heap, counters and list of reads left over are in place already
             const bool listed = pass == 0 && prep_exact;
-            const uint64_t heap_cap = listed ? pa.ex.heap_cap : heap_cap_of(list.size(), scale);
+            const uint64_t heap_cap = listed ? pa.ex.heap_cap : heap_cap_of(n_pass, scale);
             char *d_arena = nullptr, *d_heap = nullptr; uint32_t *d_list = nullptr, *d_rest = nullptr;
             unsigned long long *d_used = nullptr; unsigned int *d_next = nullptr;
             if ((rc = pass_bufs.alloc(&d_arena, stride * n_warps))) break;
@@ -1451,15 +1547,15 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
                 d_heap = pa.ex.heap; d_list = pa.list; d_used = pa.ex.heap_used; d_next = next0; d_rest = rest0;
             } else {
                 if ((rc = heap_bufs.alloc(&d_heap, heap_cap))) break;
-                if ((rc = heap_bufs.alloc(&d_list, list.size()))) break;
+                if ((rc = heap_bufs.alloc(&d_list, n_pass))) break;
                 if ((rc = heap_bufs.alloc(&d_used, 1))) break;
                 if ((rc = heap_bufs.alloc(&d_next, 2))) break;    // k_align's next read; the reads k_exact_reads leaves
-                if (exact_reads && (rc = heap_bufs.alloc(&d_rest, list.size()))) break;
+                if (exact_reads && (rc = heap_bufs.alloc(&d_rest, n_pass))) break;
             }
             ta.heap[pass] = d_heap;
             tick("pass: arena/heap alloc");
             if (!listed) {
-                if ((rc = h2d(d_list, list.data(), list.size() * 4, st))) break;
+                if ((rc = h2d(d_list, list.data(), (size_t)n_pass * 4, st))) break;
                 if ((rc = dev_zero(d_used, 8, st))) break;
                 if ((rc = dev_zero(d_next, 8, st))) break;
             }
@@ -1468,7 +1564,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             std::memset(&ea, 0, sizeof(ea));
             if (exact_reads) {
                 exact_args(caps, &ea);
-                ea.list = d_list; ea.n_list = (uint32_t)list.size(); ea.n_list_dev = listed ? pa.n_list : nullptr;
+                ea.list = d_list; ea.n_list = n_pass; ea.n_list_dev = listed ? pa.n_list : nullptr;
                 ea.rest = d_rest; ea.n_rest = d_next + 1;
                 ea.heap = d_heap; ea.heap_cap = heap_cap; ea.heap_used = d_used;
             }
@@ -1487,7 +1583,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             a.nodes_f = b.nodes_f; a.nodes_r = b.nodes_r;
             a.sub_first_f = subk ? sk.first_f : nullptr; a.sub_last_f = sk.last_f; a.sub_len_f = subk ? sk.len_f : nullptr;
             a.sub_first_r = sk.first_r; a.sub_last_r = sk.last_r; a.sub_len_r = subk && both ? sk.len_r : nullptr;
-            a.read_list = d_list; a.n_list = (uint32_t)list.size(); a.n_list_dev = nullptr;
+            a.read_list = d_list; a.n_list = n_pass; a.n_list_dev = nullptr;
             a.arena = d_arena; a.arena_stride = stride;
             a.hdr = d_hdr; a.heap = d_heap; a.heap_cap = heap_cap; a.heap_used = d_used; a.next = d_next;
             unsigned long long used = 0;
@@ -1517,6 +1613,9 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
                                  n_reads - n_rest[1], n_rest[1]);
                     std::fprintf(stderr, "[mgb] reads %u+%u k_exact_reads answered %u, left to k_align %u\n", lo, n_reads,
                                  n_rest[1] - n_rest[0], n_rest[0]);
+                    if (n_rest[0] <= 8)
+                        debug_left_over(index->view, pa, ea, seqs, offsets, koff, b, summary, d_rest, n_rest[0], lo,
+                                        n_reads, st);
                 }
 #if defined(MGB_PREP_TIMERS) && !defined(MGB_HOST_EMU)
                 if (listed && dbg_time) {
@@ -1598,6 +1697,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             // classify this pass; alignments are materialised in read order after the last pass
             std::vector<uint32_t> retry;
             const uint32_t heap_id = text ? (uint32_t)pass : (uint32_t)res->heaps.size() - 1;
+            if (list.size() != n_pass) all_reads();
             for (uint32_t r : list) {
                 const ReadHdr &h = hdr_host[r];
                 if (h.status == MGB_READ_OVERFLOW) { MGB_EMU_HIT(EMU_READ_OVERFLOW); retry.push_back(r); continue; }
@@ -1612,6 +1712,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             }
             res->stats.num_reads_retried += retry.size();
             list.swap(retry);
+            n_pass = (uint32_t)list.size();
             tick("pass: classify");
         }
         // text route: every read's pass goes up (its heap offset is in d_hdr already), then the text comes down

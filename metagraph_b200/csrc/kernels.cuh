@@ -61,6 +61,9 @@ struct SeedArgs {
     // k_seed_hash only: the reads to seed, list[0 .. *n_list) (built on the device by k_prepare_exact); nullptr: all
     // n_reads reads
     const uint32_t *list; const unsigned int *n_list;
+    // k_seed_hash only: 0 picks the walk or the short-list mode by the number of reads; 1 / 2 force the walk / the
+    // short-list mode (MGB_TEST_SEED_MODE=walk|wide, test knob)
+    uint32_t seed_mode;
 };
 
 MGB_HD void seed_item(const SeedArgs &a, uint64_t item) {
@@ -1075,6 +1078,71 @@ struct PathWalk {
     MGB_D void step(const IndexView &ix) { ++q; load(ix, false); }
 };
 
+// k_seed_hash's short-list mode: one read per warp, every k-mer of the read looked up in the hash index on its own
+// (map_to_edge for each k-mer, the lookup the walk below saves loads on), kSeedWideDepth lookups in flight per lane.
+// A k-mer's node id is its edge if that is in_graph, else 0 (so is a window with an invalid character); the summary
+// bits come from a warp-wide OR. There is no chain of dependent loads: a read costs about one round trip per
+// kSeedWideDepth * 32 k-mers, where the walk's lane waits on one adjacency record or bucket per k-mer once it leaves the
+// path layout. Kept out of line so that the walk's code and registers stay as they are. Warp w takes items w,
+// w + warps, ...
+static constexpr int kSeedWideDepth = 4;
+// the short-list mode runs when the items are at most kSeedWideRounds per warp of the grid (DESIGN.md §3.2)
+#ifndef MGB_SEED_WIDE_ROUNDS
+#define MGB_SEED_WIDE_ROUNDS 1
+#endif
+static constexpr uint32_t kSeedWideRounds = MGB_SEED_WIDE_ROUNDS;
+__device__ __noinline__ void seed_hash_wide(const SeedArgs &a, uint32_t n_items) {
+    const IndexView &ix = a.ix;
+    const int K = (int)ix.k;
+    const uint32_t sigma = ix.sigma;
+    const int ns = (int)a.n_strands;
+    const int lane = (int)(threadIdx.x & 31);
+    const uint32_t warps = gridDim.x * blockDim.x / kWarp;
+    for (uint32_t it = (blockIdx.x * blockDim.x + threadIdx.x) / kWarp; it < n_items; it += warps) {
+        const uint32_t r = a.list ? __ldg(a.list + it) : it;
+        const uint64_t b = a.offsets[r];
+        const int L = (int)(a.offsets[r + 1] - b);
+        const int nk = L >= K ? L - K + 1 : 0;
+        const uint64_t ko = a.koff[r];
+        const int n = ns * nk;                        // item j: k-mer j % nk of strand j / nk
+        uint32_t seen = 0;                            // SeedArgs::summary bits of this lane's k-mers
+        for (int base = 0; base < n; base += kWarp * kSeedWideDepth) {
+            KhProbe p[kSeedWideDepth];
+            #pragma unroll
+            for (int d = 0; d < kSeedWideDepth; ++d) {
+                const int j = base + d * kWarp + lane;
+                const int s = j >= nk ? 1 : 0, i = j - s * nk;
+                bool ok = j < n;
+                unsigned long long key = 0;
+                if (ok) {
+                    const uint8_t *c = (s ? a.cr : a.cf) + b + i;
+                    for (int t = 0; t < K; ++t) {
+                        const uint32_t x = __ldg(c + t);
+                        ok = ok && x >= 1 && x < sigma;
+                        key |= (unsigned long long)((x - 1) & 3u) << (2 * t);
+                    }
+                }
+                p[d].issue(ix, key, ok);
+            }
+            #pragma unroll
+            for (int d = 0; d < kSeedWideDepth; ++d) p[d].find(ix);
+            #pragma unroll
+            for (int d = 0; d < kSeedWideDepth; ++d) {
+                const int j = base + d * kWarp + lane;
+                if (j < n) {
+                    const int s = j >= nk ? 1 : 0, i = j - s * nk;
+                    const uint64_t found = p[d].value(ix);
+                    const bool store = found != 0 && in_graph(ix, found);
+                    ((s ? a.nodes_r : a.nodes_f) + ko)[i] = store ? found : 0;
+                    seen |= (store ? 2u : 1u) << (2 * s);
+                }
+            }
+        }
+        seen = __reduce_or_sync(0xffffffffu, seen);
+        if (a.summary && lane == 0) a.summary[r] = (uint8_t)seen;
+    }
+}
+
 // BOSS::map_to_edges (boss.cpp:996-1045) on graphs with the k-mer hash index (DNA block layout, k <= 31), one read per
 // lane. A strand walked in order costs one load per k-mer: the adjacency record of the previous k-mer's edge while the
 // walk is warm (boss.cpp:1024-1043), the k-mer's bucket (+ the value on a hit) when it is cold (map_to_edge,
@@ -1101,6 +1169,8 @@ struct PathWalk {
 //
 // Steps are written with selects rather than branches: lanes in different regimes issue together. Persistent grid:
 // lane t of n_lanes takes the reads t + n_lanes * round, or those entries of a.list (the reads k_prepare_exact left over).
+// A short list (at most kSeedWideRounds reads per warp of the grid, decided alike by every thread) goes to
+// seed_hash_wide instead: a lane's walk is a chain of dependent loads, and with few reads nothing hides its latency.
 __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash(const __grid_constant__ SeedArgs a) {
     const IndexView &ix = a.ix;
     const int K = (int)ix.k;
@@ -1110,6 +1180,10 @@ __global__ void __launch_bounds__(kSeedThreads, MGB_SEED_MIN_BLOCKS) k_seed_hash
     const bool two = a.n_strands == 2;
     const uint32_t lanes = gridDim.x * blockDim.x;
     const uint32_t n_items = a.list ? *a.n_list : a.n_reads;
+    if (a.seed_mode == 2 || (a.seed_mode == 0 && n_items <= kSeedWideRounds * (lanes / kWarp))) {
+        seed_hash_wide(a, n_items);
+        return;
+    }
     for (uint32_t it = blockIdx.x * blockDim.x + threadIdx.x; it < n_items; it += lanes) {
         const uint32_t r = a.list ? __ldg(a.list + it) : it;
         const uint64_t b = a.offsets[r];
