@@ -168,6 +168,10 @@ enum EmuPath : int {
     EMU_UNSTAGED_READ,        // a read whose strands are not staged on chip (L + 1 > lq)
     EMU_GENERAL_COLUMN,       // a child column computed by the general path
     EMU_READ_OVERFLOW,        // a read marked MGB_READ_OVERFLOW (retried with a larger arena)
+    EMU_RAM_STOP_GENERAL,     // the general loop ends an extension on max_ram_per_alignment
+    EMU_NODES_STOP_GENERAL,   // the general loop ends an extension on max_nodes_per_seq_char
+    EMU_RAM_STOP_CHAIN,       // chain_loop ends an extension on max_ram_per_alignment
+    EMU_NODES_STOP_CHAIN,     // chain_loop ends an extension on max_nodes_per_seq_char
     EMU_N_PATHS
 };
 extern "C" unsigned long long mgb_emu_path_hits[EMU_N_PATHS];
@@ -2233,10 +2237,12 @@ struct ReadAligner {
                 if (parS[par.max_pos - par.trim] < best_score) {
                     double node_counter = (double)n_cols;
                     if (node_counter / wlen >= cfg.max_nodes_per_seq_char) {
+                        MGB_EMU_HIT(EMU_NODES_STOP_GENERAL);
                         heap_n = 0; nn_n = 0;            // global_xdrop
                         continue;
                     }
                     if ((double)table_size_bytes / 1000000 > cfg.max_ram_per_alignment) {
+                        MGB_EMU_HIT(EMU_RAM_STOP_GENERAL);
                         heap_n = 0; nn_n = 0;
                         continue;
                     }
@@ -2599,8 +2605,12 @@ struct ReadAligner {
 
         while (!stop) {                                    // every exit sets stop
             if (c_maxval < best_score) {
-                if ((double)ncols / wlen >= cfg.max_nodes_per_seq_char) { stop = 1; break; }      // global_xdrop
-                if ((double)table_bytes / 1000000 > cfg.max_ram_per_alignment) { stop = 1; break; }
+                if ((double)ncols / wlen >= cfg.max_nodes_per_seq_char) {                           // global_xdrop
+                    MGB_EMU_HIT(EMU_NODES_STOP_CHAIN); stop = 1; break;
+                }
+                if ((double)table_bytes / 1000000 > cfg.max_ram_per_alignment) {
+                    MGB_EMU_HIT(EMU_RAM_STOP_CHAIN); stop = 1; break;
+                }
             }
             if (!c_bm) { stop = 1; break; }                    // no band: no children
             const int begin = ffs32(c_bm) - 1 + c_trim;

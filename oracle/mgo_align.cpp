@@ -679,6 +679,10 @@ SeederOutput run_seeder(const DBGSuccinct &graph, const DBGAlignerConfig &config
 // ---------------------------------------------------------------------------
 // Extender (aligner_extender_methods.{hpp,cpp})
 // ---------------------------------------------------------------------------
+// Stop-test trace of the calling thread (mgo_align_budget_trace): while set, the extender appends
+// (table_size_bytes_, table.size(), window.size()) every time it evaluates the node and RAM budgets.
+thread_local std::vector<uint64_t> *budget_trace = nullptr;
+
 namespace {
 
 constexpr size_t kPadding = 5;
@@ -1040,6 +1044,11 @@ class Extender {
                     double node_counter = config_.global_xdrop ? table.size()
                                                                : next_offset - seed_offset;
                     if (S[col.max_pos - col.trim] < best_score) {
+                        if (budget_trace) {
+                            budget_trace->push_back(table_size_bytes_);
+                            budget_trace->push_back(table.size());
+                            budget_trace->push_back(window.size());
+                        }
                         if (node_counter / window.size() >= config_.max_nodes_per_seq_char) {
                             if (config_.global_xdrop) {
                                 queue = std::priority_queue<TableIt>();

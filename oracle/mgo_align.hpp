@@ -198,6 +198,11 @@ class DBGAligner {
     DBGAlignerConfig config_;
 };
 
+// Not in the reference: when non-null, the extender of the calling thread appends one triple
+// (table_size_bytes_, table.size(), window.size()) each time it evaluates its node and RAM budgets
+// (the stop tests of DefaultColumnExtender::extend). Test infrastructure for the budget tests.
+extern thread_local std::vector<uint64_t> *budget_trace;
+
 // cli/align.cpp:254-307 (TSV branch) + alignment.hpp:418-435
 std::string format_alignment(const std::string &header, const AlignmentResults &paths,
                              score_t min_path_score);

@@ -265,6 +265,33 @@ char* mgo_align_tsv(void *gp, const char *alphabet, const mgo_config_t *cfg,
     return buf;
 }
 
+// Aligns `n` reads on the calling thread as mgo_align_tsv does and reports every evaluation of the extender's
+// node and RAM budgets (DefaultColumnExtender::extend: the column's best cell is below the best score so far).
+// Each evaluation is a triple (table_size_bytes_, table.size(), window.size()); read_ends[i] is the number of
+// triples of reads 0..i. Returns a malloc'd array of all triples, or NULL if the aligner threw.
+uint64_t* mgo_align_budget_trace(void *gp, const char *alphabet, const mgo_config_t *cfg, const char **seqs,
+                                 uint64_t n, uint64_t *read_ends) {
+    auto *g = static_cast<DBGSuccinct*>(gp);
+    const Alphabet &a = alph_of(alphabet);
+    std::vector<uint64_t> trace;
+    try {
+        DBGAligner aligner(*g, to_config(*cfg, a));
+        std::vector<std::pair<std::string, std::string>> batch;
+        for (uint64_t i = 0; i < n; ++i) batch.emplace_back(std::string(), seqs[i]);
+        uint64_t i = 0;
+        budget_trace = &trace;
+        // align_batch finishes a read before it moves on to the next one
+        aligner.align_batch(batch, [&](const std::string&, AlignmentResults&&) { read_ends[i++] = trace.size() / 3; });
+        budget_trace = nullptr;
+    } catch (...) {
+        budget_trace = nullptr;
+        return nullptr;
+    }
+    auto *out = static_cast<uint64_t*>(std::malloc(std::max<size_t>(1, trace.size()) * sizeof(uint64_t)));
+    std::copy(trace.begin(), trace.end(), out);
+    return out;
+}
+
 void mgo_free(void *p) { std::free(p); }
 
 } // extern "C"

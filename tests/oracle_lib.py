@@ -53,6 +53,8 @@ def lib():
         L.mgo_seeds.argtypes = [vp, cp, vp, cp, u64, i, vp, u64, vp]
         L.mgo_align_tsv.restype = vp
         L.mgo_align_tsv.argtypes = [vp, cp, vp, ctypes.POINTER(cp), ctypes.POINTER(cp), u64, i, i, vp]
+        L.mgo_align_budget_trace.restype = ctypes.POINTER(u64)
+        L.mgo_align_budget_trace.argtypes = [vp, cp, vp, ctypes.POINTER(cp), u64, vp]
         L.mgo_free.argtypes = [vp]
         _lib = L
     return _lib
@@ -171,6 +173,23 @@ class OracleGraph:
         lines = txt.split("\n")
         assert lines[-1] == ""
         return lines[:-1]
+
+    def budget_trace(self, cfg, reads):
+        """Every evaluation of the extender's node and RAM budgets, per read: a list with one (n, 3) uint64 array
+        per read whose rows are (table_size_bytes_, table.size(), window.size()) at the stop tests."""
+        import numpy as np
+        c = cfg.to_c()
+        n = len(reads)
+        S = (ctypes.c_char_p * n)(*[s.encode() if isinstance(s, str) else s for s in reads])
+        ends = np.zeros(max(1, n), np.uint64)
+        p = lib().mgo_align_budget_trace(self.h, self.alphabet, ctypes.byref(c), S, n, ends.ctypes.data)
+        if not p:
+            raise RuntimeError("oracle aligner failed")
+        total = int(ends[n - 1]) if n else 0
+        flat = np.ctypeslib.as_array(p, shape=(max(1, 3 * total),))[:3 * total].reshape(total, 3).copy()
+        lib().mgo_free(ctypes.cast(p, ctypes.c_void_p))
+        bounds = [0] + [int(e) for e in ends[:n]]
+        return [flat[bounds[i]:bounds[i + 1]] for i in range(n)]
 
 
 def is_low_complexity(seq):

@@ -67,7 +67,7 @@ def check_mt(lib, both):
     return got
 
 
-def random_case(lib, seed, k, G, nreads, L, rate, cfg, mask=False, nseq=1):
+def random_case(lib, seed, k, G, nreads, L, rate, cfg, mask=False, nseq=1, oracle_stats=None):
     rng = np.random.default_rng(seed)
     seqs = ["".join(np.array(list("ACGT"))[rng.integers(0, 4, G)])]
     seqs += [mutate(rng, seqs[0], 0.02) for _ in range(nseq - 1)]
@@ -89,7 +89,7 @@ def random_case(lib, seed, k, G, nreads, L, rate, cfg, mask=False, nseq=1):
             r = r[:len(r) // 2] + "N" + r[len(r) // 2 + 1:]
         reads.append(r)
     reads += ["", "A", "ACGT" * 3, "N" * 40]          # empty / shorter than k / all-invalid
-    exp = g.align_tsv(cfg, reads, with_nodes=True)
+    exp = g.align_tsv(cfg, reads, with_nodes=True, stats=oracle_stats)
     got, stats = run_lines(idx, cfg, reads)
     bad = [i for i in range(len(reads)) if exp[i] != got[i]]
     assert not bad, (seed, bad[:3], exp[bad[0]], got[bad[0]])
@@ -114,7 +114,7 @@ def whole_read_hits(lib):
 
 # the aligner's spill / migration sites the host-emulation build counts (align_core.cuh EmuPath, same order)
 EMU_PATHS = ("queue_migrate", "nn_migrate", "column_migrate", "arena_column", "unstaged_read", "general_column",
-             "read_overflow")
+             "read_overflow", "ram_stop_general", "nodes_stop_general", "ram_stop_chain", "nodes_stop_chain")
 
 
 def path_hits(lib):
