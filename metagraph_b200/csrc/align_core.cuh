@@ -172,6 +172,7 @@ enum EmuPath : int {
     EMU_NODES_STOP_GENERAL,   // the general loop ends an extension on max_nodes_per_seq_char
     EMU_RAM_STOP_CHAIN,       // chain_loop ends an extension on max_ram_per_alignment
     EMU_NODES_STOP_CHAIN,     // chain_loop ends an extension on max_nodes_per_seq_char
+    EMU_CONV_MOVE,            // conv_grow: a convergence-table entry outgrows its segment and moves to a new one
     EMU_N_PATHS
 };
 extern "C" unsigned long long mgb_emu_path_hits[EMU_N_PATHS];
@@ -1598,6 +1599,7 @@ struct ReadAligner {
             int seg_start = imax(0, new_start - 16);
             int seg_cap = imin(L + 1, new_end + 16) - seg_start;
             if (cells_used + seg_cap > caps.max_conv_cells) { overflow = true; return false; }
+            MGB_EMU_HIT(EMU_CONV_MOVE);
             score_t *src = cells + en->seg_off, *dst = cells + cells_used;
             wsync();
             for (int p = old_start + wlane(); p < old_end; p += kWarp)

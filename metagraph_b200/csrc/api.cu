@@ -1401,7 +1401,8 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
         // MGB_TEST_NO_PREPARE_EXACT: test knob, the route off.
         PrepExactArgs pa;
         std::memset(&pa, 0, sizeof(pa));
-        unsigned int *next0 = nullptr;      // k_align's next read, the reads k_exact_reads leaves, the length of pa.list
+        unsigned int *next0 = nullptr;      // k_align's next read, the reads k_exact_reads leaves, the length of pa.list,
+                                            // k_align's next arena
         uint32_t *rest0 = nullptr;
         const bool prep_exact = !rc && exact_reads && index->view.kh_slots && index->view.pl_n
                                 && exact_max_len(choose_caps(b.L_max, dcfg, k, 1)) >= k
@@ -1482,7 +1483,13 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
         float align_ms = 0, d2h_ms = 0; (void)align_ms; (void)d2h_ms;
         for (int pass = 0; !rc && n_pass; ++pass, scale *= 4) {
             if (pass == 6) { rc = fail(MGB_ERR_OVERFLOW, "a read exceeded the largest per-read work arena"); break; }
-            Caps caps = choose_caps(b.L_max, dcfg, index->view.k, scale);
+            // the arena fits the longest read of the pass: on a retry pass the reads that overflowed, not the batch
+            uint32_t L_pass = b.L_max;
+            if (pass > 0) {
+                L_pass = 0;
+                for (uint32_t r : list) L_pass = std::max<uint32_t>(L_pass, (uint32_t)(offsets[r + 1] - offsets[r]));
+            }
+            Caps caps = choose_caps(L_pass, dcfg, index->view.k, scale);
             size_t stride = arena_bytes(caps);
             // on-chip working set per warp: the column buffers hold the widest column the x-drop band
             // allows (choose_caps' estimate; at least 64 cells, the register path of the extender needs 40) of
@@ -1501,7 +1508,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             DevBufs pass_bufs(st, wsg.w, 32);          // slot 32: the arena
             DevBufs &heap_bufs = pass_keep.emplace_back(st, wsg.w, text ? 40 + 8 * (size_t)pass : 33);
 #if defined(MGB_HOST_EMU)
-            uint32_t n_warps = 1;
+            const uint32_t n_arenas = 1;
 #else
             int blocks_per_sm = 0;
             const size_t smem_block = smem_per_warp * kern_dna::kWarpsPerBlock;
@@ -1526,30 +1533,32 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             if (blocks_per_sm < 1) blocks_per_sm = 1;
             const uint64_t wpb = kern_dna::kWarpsPerBlock;        // warps (reads in flight) per block
             uint64_t n_warps64 = (uint64_t)index->num_sms * blocks_per_sm * wpb;
-            if (stride * n_warps64 > pass_bufs.capacity_of_next()) {
-                size_t free_b = 0, total_b = 0;
-                cudaMemGetInfo(&free_b, &total_b);
-                uint64_t mem_warps = (uint64_t)(free_b * 0.6 + pass_bufs.capacity_of_next()) / (stride ? stride : 1);
-                if (mem_warps < wpb) mem_warps = wpb;
-                if (n_warps64 > mem_warps) n_warps64 = mem_warps / wpb * wpb;
-            }
             if (n_warps64 > ((uint64_t)n_pass + wpb - 1) / wpb * wpb) n_warps64 = ((uint64_t)n_pass + wpb - 1) / wpb * wpb;
             n_warps64 = kern_dna::read_path_grid(n_warps64 / wpb) * wpb;    // (MGB_TEST_MAX_BLOCKS)
-            uint32_t n_warps = (uint32_t)n_warps64;
+            // one arena per warp that can take a read, and as many as fit in 60 % of the free memory (at least one)
+            uint64_t n_arenas64 = std::min<uint64_t>(n_warps64, n_pass);
+            if (stride * n_arenas64 > pass_bufs.capacity_of_next()) {
+                size_t free_b = 0, total_b = 0;
+                cudaMemGetInfo(&free_b, &total_b);
+                const uint64_t mem_arenas = (uint64_t)(free_b * 0.6 + pass_bufs.capacity_of_next()) / (stride ? stride : 1);
+                n_arenas64 = std::max<uint64_t>(1, std::min(n_arenas64, mem_arenas));
+                n_warps64 = std::min(n_warps64, (n_arenas64 + wpb - 1) / wpb * wpb);
+            }
+            uint32_t n_warps = (uint32_t)n_warps64, n_arenas = (uint32_t)n_arenas64;
 #endif
             // pass 0 after k_prepare_exact: its heap, counters and list of reads left over are in place already
             const bool listed = pass == 0 && prep_exact;
             const uint64_t heap_cap = listed ? pa.ex.heap_cap : heap_cap_of(n_pass, scale);
             char *d_arena = nullptr, *d_heap = nullptr; uint32_t *d_list = nullptr, *d_rest = nullptr;
             unsigned long long *d_used = nullptr; unsigned int *d_next = nullptr;
-            if ((rc = pass_bufs.alloc(&d_arena, stride * n_warps))) break;
+            if ((rc = pass_bufs.alloc(&d_arena, stride * n_arenas))) break;
             if (listed) {
                 d_heap = pa.ex.heap; d_list = pa.list; d_used = pa.ex.heap_used; d_next = next0; d_rest = rest0;
             } else {
                 if ((rc = heap_bufs.alloc(&d_heap, heap_cap))) break;
                 if ((rc = heap_bufs.alloc(&d_list, n_pass))) break;
                 if ((rc = heap_bufs.alloc(&d_used, 1))) break;
-                if ((rc = heap_bufs.alloc(&d_next, 2))) break;    // k_align's next read; the reads k_exact_reads leaves
+                if ((rc = heap_bufs.alloc(&d_next, 4))) break;    // k_align's next read and arena; the reads k_exact_reads leaves
                 if (exact_reads && (rc = heap_bufs.alloc(&d_rest, n_pass))) break;
             }
             ta.heap[pass] = d_heap;
@@ -1557,7 +1566,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             if (!listed) {
                 if ((rc = h2d(d_list, list.data(), (size_t)n_pass * 4, st))) break;
                 if ((rc = dev_zero(d_used, 8, st))) break;
-                if ((rc = dev_zero(d_next, 8, st))) break;
+                if ((rc = dev_zero(d_next, 16, st))) break;
             }
             // the read-dependent part of the gate (exact_read_strand); max_len keeps what k_align's own exit required
             ExactArgs ea;
@@ -1584,7 +1593,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             a.sub_first_f = subk ? sk.first_f : nullptr; a.sub_last_f = sk.last_f; a.sub_len_f = subk ? sk.len_f : nullptr;
             a.sub_first_r = sk.first_r; a.sub_last_r = sk.last_r; a.sub_len_r = subk && both ? sk.len_r : nullptr;
             a.read_list = d_list; a.n_list = n_pass; a.n_list_dev = nullptr;
-            a.arena = d_arena; a.arena_stride = stride;
+            a.arena = d_arena; a.arena_stride = stride; a.n_arenas = n_arenas;
             a.hdr = d_hdr; a.heap = d_heap; a.heap_cap = heap_cap; a.heap_used = d_used; a.next = d_next;
             unsigned long long used = 0;
 #if !defined(MGB_HOST_EMU)
@@ -1643,12 +1652,13 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
             used = *d_used;
 #else
             const uint32_t grid = (uint32_t)(std::min<uint64_t>(n_warps, ((uint64_t)a.n_list + wpb - 1) / wpb * wpb) / wpb);
-            if (dbg_time) {         // every pass; per_round: warps launched, each aligning one read of the list at a time
+            if (dbg_time) {         // every pass; per_round: warps launched with an arena, each aligning one read at a time
                 char launched[128] = "";          // (one fprintf: pieces on two host threads print at once)
                 if (a.n_list) std::snprintf(launched, sizeof(launched), "; launch k_align grid=%u block=%d per_round=%llu items=%u",
-                                            grid, kern_dna::kAlignThreads, (unsigned long long)grid * wpb, n_align);
-                std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident), arena %zu bytes per warp%s\n", n_warps,
-                             (unsigned long long)index->num_sms * blocks_per_sm * wpb, stride, launched);
+                                            grid, kern_dna::kAlignThreads,
+                                            (unsigned long long)std::min<uint64_t>((uint64_t)grid * wpb, n_arenas), n_align);
+                std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident), arena %zu bytes per warp, %u arenas%s\n",
+                             n_warps, (unsigned long long)index->num_sms * blocks_per_sm * wpb, stride, n_arenas, launched);
             }
             if (a.n_list) {
                 CUDA_TRY(index->view.wide ? kern_any::launch_align(grid, smem_block, st.s, a)

@@ -146,8 +146,9 @@ struct AlignArgs {
     const uint32_t *read_list; uint32_t n_list;
     const unsigned int *n_list_dev;   // non-null: the list's length is *n_list_dev (<= n_list), written by an earlier kernel
     char *arena; size_t arena_stride;
+    uint32_t n_arenas;          // arenas at `arena`: k_align hands them to its warps in the order they start
     ReadHdr *hdr; char *heap; uint64_t heap_cap; unsigned long long *heap_used;
-    unsigned int *next;
+    unsigned int *next;         // next[0]: the next read of the list; next[3]: the next arena
 };
 
 // aligns read r with the warp's arena and on-chip working set and writes its record and alignments
@@ -1320,17 +1321,20 @@ static constexpr int kAlignThreads = MGB_ALIGN_THREADS;
 static constexpr int kWarpsPerBlock = kAlignThreads / kWarp;   // reads in flight per block of k_align
 // one warp per read; a warp that finds the list done before its first read touches nothing (the host may launch more
 // warps than a list whose length only the device knows needs)
-__device__ __forceinline__ unsigned int align_take(const AlignArgs &a) {
+__device__ __forceinline__ unsigned int align_take(const AlignArgs &a, int which = 0) {
     unsigned int t = 0;
-    if (wlane() == 0) t = atomicAdd(a.next, 1u);
+    if (wlane() == 0) t = atomicAdd(a.next + which, 1u);
     return wbcast(t, 0);
 }
 __global__ void __launch_bounds__(kAlignThreads, MGB_ALIGN_MIN_BLOCKS) k_align(const __grid_constant__ AlignArgs a) {
     const uint32_t n_list = a.n_list_dev ? __ldg(a.n_list_dev) : a.n_list;
+    // the warp's arena, numbered in the order the warps start rather than by warp id: a pass allocates one arena per
+    // read at most, and fewer when device memory holds fewer; a warp left without one aligns nothing
+    const unsigned int slot = align_take(a, 3);
+    if (slot >= a.n_arenas) return;
     unsigned int t = align_take(a);
     if (t >= n_list) return;
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) / kWarp;
-    char *arena = a.arena + (size_t)warp * a.arena_stride;
+    char *arena = a.arena + (size_t)slot * a.arena_stride;
     extern __shared__ __align__(16) char smem_raw[];
     char *smem = smem_raw + (threadIdx.x / kWarp) * a.slay.total;
     init_arena(a, arena);

@@ -114,7 +114,7 @@ def whole_read_hits(lib):
 
 # the aligner's spill / migration sites the host-emulation build counts (align_core.cuh EmuPath, same order)
 EMU_PATHS = ("queue_migrate", "nn_migrate", "column_migrate", "arena_column", "unstaged_read", "general_column",
-             "read_overflow", "ram_stop_general", "nodes_stop_general", "ram_stop_chain", "nodes_stop_chain")
+             "read_overflow", "ram_stop_general", "nodes_stop_general", "ram_stop_chain", "nodes_stop_chain", "conv_move")
 
 
 def path_hits(lib):
