@@ -205,6 +205,31 @@ enum { MGB_TEXT_TSV = 1, MGB_TEXT_JSON = 2 };
 int mgb_align_batch_text(const mgb_index_t *index, const mgb_config_t *config, const char *seqs,
                          const uint64_t *offsets, const char *headers, const uint64_t *header_offsets,
                          uint32_t n_reads, int format, mgb_results_t **out);
+/* `metagraph align FILE` from the bytes of the file: parses the complete FASTA/FASTQ records of buf[0, bytes) as
+ * kseq_read does (seq_io/sequence_io.hpp:349-438), aligns them and renders their text as mgb_align_batch_text does.
+ * buf starts at a record start; at_eof = 1 for the last chunk of a file. *consumed = bytes up to the end of the last
+ * complete record: the caller keeps buf[*consumed, bytes) for the front of the next chunk, and grows its buffer when
+ * *consumed is 0 and at_eof is 0. *ended = 1 when a malformed record ended the input as it ends FastaParser's
+ * iteration: the caller reads no more of this file. comment_delim: NULL = the header is the name only, otherwise
+ * `--header-comment-delim` (cli/align.cpp:430-435). flags: MGB_FASTX_FWD_AND_REVERSE = `--fwd-and-reverse`, every
+ * record followed by its reverse complement under the same header. format: MGB_TEXT_TSV / MGB_TEXT_JSON.
+ * The records are parsed on the device when the chunk is a FASTA chunk without '+' lines or a 4-line FASTQ chunk and
+ * is shorter than 4 GiB; other chunks are parsed on the host. Either way the bytes are the same. */
+enum { MGB_FASTX_FWD_AND_REVERSE = 1 };
+int mgb_align_fastx_text(const mgb_index_t *index, const mgb_config_t *config, const char *buf, uint64_t bytes,
+                         int at_eof, const char *comment_delim, int flags, int format,
+                         uint64_t *consumed, int *ended, mgb_results_t **out);
+/* Diagnostic entry, not needed to align files: the reads and headers mgb_align_fastx_text aligns for the same
+ * arguments, without aligning them, so that the device parser can be checked against the host restatement and either
+ * parser can be timed on its own. device_route = 1:
+ * parsed as mgb_align_fastx_text parses them on index's device; *refused = 1 when the chunk left the device route and
+ * the host restatement parsed it. device_route = 0: the host restatement (index may be NULL). The arrays are the
+ * caller's: seqs of max_seq_bytes, names of max_name_bytes, offsets and name_offsets of max_records + 1 entries;
+ * MGB_ERR_OVERFLOW when the records do not fit. */
+int mgb_fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes, int at_eof, const char *comment_delim,
+                    int flags, int device_route, char *seqs, uint64_t max_seq_bytes, uint64_t *offsets, char *names,
+                    uint64_t max_name_bytes, uint64_t *name_offsets, uint64_t max_records, uint64_t *n_records,
+                    uint64_t *consumed, int *ended, int *refused);
 /* The text block of a result set of mgb_align_batch_text (owned by it); MGB_ERR_INVALID_ARGUMENT for a record set. */
 int mgb_results_text(const mgb_results_t *results, const char **text, uint64_t *bytes);
 

@@ -84,6 +84,12 @@ def load_library(path=None):
     L.mgb_align_batch.argtypes = [vp, ctypes.POINTER(mgb_config_t), vp, vp, u32, ctypes.POINTER(vp)]
     L.mgb_align_batch_text.restype = i
     L.mgb_align_batch_text.argtypes = [vp, ctypes.POINTER(mgb_config_t), vp, vp, vp, vp, u32, i, ctypes.POINTER(vp)]
+    L.mgb_align_fastx_text.restype = i
+    L.mgb_align_fastx_text.argtypes = [vp, ctypes.POINTER(mgb_config_t), vp, u64, i, cp, i, i, ctypes.POINTER(u64),
+                                       ctypes.POINTER(i), ctypes.POINTER(vp)]
+    L.mgb_fastx_parse.restype = i
+    L.mgb_fastx_parse.argtypes = [vp, vp, u64, i, cp, i, i, vp, u64, vp, vp, u64, vp, u64, ctypes.POINTER(u64),
+                                  ctypes.POINTER(u64), ctypes.POINTER(i), ctypes.POINTER(i)]
     L.mgb_results_text.restype = i
     L.mgb_results_text.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(u64)]
     L.mgb_results_num_reads.restype = u32
@@ -133,6 +139,7 @@ REQUIRED_SYMBOLS = [
     "mgb_results_alignments", "mgb_results_stats", "mgb_results_free", "mgb_results_export_bytes",
     "mgb_results_export", "mgb_results_import", "mgb_boss_build", "mgb_boss_free",
     "mgb_boss_mask_dummy", "mgb_set_pipeline_pieces", "mgb_set_host_threads", "mgb_dbg_load", "mgb_dbg_last_error", "mgb_boss_last_error", "mgb_config_check", "mgb_dbg_load_suffix_ranges", "mgb_dbg_free_suffix_ranges", "mgb_index_set_mode",
-    "mgb_align_batch_text", "mgb_results_text",
+    "mgb_align_batch_text", "mgb_results_text", "mgb_align_fastx_text", "mgb_fastx_parse",
 ]
 MGB_TEXT_TSV, MGB_TEXT_JSON = 1, 2
+MGB_FASTX_FWD_AND_REVERSE = 1

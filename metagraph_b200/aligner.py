@@ -480,5 +480,62 @@ class B200Aligner:
         finally:
             self.free_raw(res)
 
+    def align_fastx_text_raw(self, buf, at_eof=True, comment_delim=None, fwd_and_reverse=False, json=False):
+        """Runs mgb_align_fastx_text on one chunk of FASTA/FASTQ bytes (a uint8 array or bytes); returns (results
+        handle, consumed, ended)."""
+        c = self.config.to_c() if not isinstance(self.config, mgb_config_t) else self.config
+        arr = np.frombuffer(buf, np.uint8) if isinstance(buf, (bytes, bytearray, memoryview)) else buf
+        res, consumed, ended = ctypes.c_void_p(), ctypes.c_uint64(), ctypes.c_int()
+        fmt = _lib.MGB_TEXT_JSON if json else _lib.MGB_TEXT_TSV
+        flags = _lib.MGB_FASTX_FWD_AND_REVERSE if fwd_and_reverse else 0
+        delim = None if comment_delim is None else _as_bytes(comment_delim)
+        _lib.check(self._L, self._L.mgb_align_fastx_text(self.graph.handle, ctypes.byref(c), arr.ctypes.data, len(arr),
+                                                         int(bool(at_eof)), delim, flags, fmt, ctypes.byref(consumed),
+                                                         ctypes.byref(ended), ctypes.byref(res)))
+        return res, consumed.value, bool(ended.value)
+
+    def align_fastx_text(self, buf, at_eof=True, comment_delim=None, fwd_and_reverse=False, json=False):
+        """What `metagraph align` prints for the complete FASTA/FASTQ records of buf, rendered on the device.
+        Returns (text, consumed, ended): bytes of buf up to the end of the last complete record, and whether a
+        malformed record ended the input (see mgb_align_fastx_text)."""
+        res, consumed, ended = self.align_fastx_text_raw(buf, at_eof, comment_delim, fwd_and_reverse, json)
+        try:
+            self.last_stats = self.stats_of(res)
+            return self.text_of(res), consumed, ended
+        finally:
+            self.free_raw(res)
+
     def align(self, query):
         return self.align_batch([("", query)])[0]
+
+
+def _as_bytes(x):
+    return x.encode("latin1") if isinstance(x, str) else bytes(x)
+
+
+def parse_fastx(buf, at_eof=True, comment_delim=None, fwd_and_reverse=False, index=None, lib=None):
+    """The records mgb_align_fastx_text aligns for these arguments (mgb_fastx_parse): with index, as its device
+    parses them; without, by the host restatement of kseq_read. Returns (headers, reads, consumed, ended, refused),
+    headers and reads as lists of bytes; refused: the device route left the chunk to the host restatement."""
+    L = index._L if index is not None else _lib.load_library(lib)
+    data = bytes(buf)
+    arr = np.frombuffer(data, np.uint8) if data else np.zeros(1, np.uint8)
+    delim = None if comment_delim is None else _as_bytes(comment_delim)
+    copies = 2 if fwd_and_reverse else 1
+    # every record starts at a '>' or '@' byte
+    max_rec = copies * (data.count(b">") + data.count(b"@") + 1)
+    max_seq = copies * len(data) + 1
+    max_name = copies * (len(data) + max_rec * len(delim or b"")) + 1
+    seqs, names = np.zeros(max_seq, np.uint8), np.zeros(max_name, np.uint8)
+    offs, noffs = np.zeros(max_rec + 1, np.uint64), np.zeros(max_rec + 1, np.uint64)
+    n, consumed, ended, refused = ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_int(), ctypes.c_int()
+    _lib.check(L, L.mgb_fastx_parse(index.handle if index is not None else None, arr.ctypes.data, len(data),
+                                    int(bool(at_eof)), delim, _lib.MGB_FASTX_FWD_AND_REVERSE if fwd_and_reverse else 0,
+                                    int(index is not None), seqs.ctypes.data, max_seq, offs.ctypes.data,
+                                    names.ctypes.data, max_name, noffs.ctypes.data, max_rec, ctypes.byref(n),
+                                    ctypes.byref(consumed), ctypes.byref(ended), ctypes.byref(refused)))
+    n = n.value
+    sb, nb = seqs.tobytes(), names.tobytes()
+    reads = [sb[int(offs[i]):int(offs[i + 1])] for i in range(n)]
+    headers = [nb[int(noffs[i]):int(noffs[i + 1])] for i in range(n)]
+    return headers, reads, consumed.value, bool(ended.value), bool(refused.value)

@@ -45,6 +45,8 @@
 #define MGB_KERNEL_NS kern_dna
 #include "kernels.cuh"
 #include "format_core.cuh"
+#include "fastx_core.cuh"
+#include "fastx_host.hpp"
 #include "host_common.hpp"
 #include "index_build.hpp"
 
@@ -770,9 +772,11 @@ struct Batch {                 // device-resident read batch
     uint64_t *offsets = nullptr, *koff = nullptr, *nodes_f = nullptr, *nodes_r = nullptr;
 };
 
+// dev_seqs: seqs is device memory (the file route's parsed reads, 16-byte aligned, 64 bytes of slack after the last
+// read) and is read in place
 int upload_batch(const mgb_index_t *index, const char *seqs, const uint64_t *offsets, uint32_t n_reads,
                  bool need_rc_nodes, Stream &st, DevBufs &bufs, Batch *b, std::vector<uint64_t> *koff_host,
-                 mgb_stats_t *stats) {
+                 mgb_stats_t *stats, bool dev_seqs = false) {
     const uint32_t k = index->view.k;
     b->n_reads = n_reads;
     b->total_chars = offsets[n_reads];
@@ -787,7 +791,8 @@ int upload_batch(const mgb_index_t *index, const char *seqs, const uint64_t *off
     b->total_kmers = (*koff_host)[n_reads];
     int rc;
     const size_t pad = 64;
-    if ((rc = bufs.alloc(&b->seqs, b->total_chars + pad))) return rc;
+    if (dev_seqs) b->seqs = const_cast<char*>(seqs);
+    else if ((rc = bufs.alloc(&b->seqs, b->total_chars + pad))) return rc;
     if ((rc = bufs.alloc(&b->qf, b->total_chars + pad))) return rc;
     if ((rc = bufs.alloc(&b->qr, b->total_chars + pad))) return rc;
     if ((rc = bufs.alloc(&b->cf, b->total_chars + pad))) return rc;
@@ -796,10 +801,10 @@ int upload_batch(const mgb_index_t *index, const char *seqs, const uint64_t *off
     if ((rc = bufs.alloc(&b->koff, (size_t)n_reads + 1))) return rc;
     if ((rc = bufs.alloc(&b->nodes_f, b->total_kmers + 1))) return rc;
     if (need_rc_nodes && (rc = bufs.alloc(&b->nodes_r, b->total_kmers + 1))) return rc;
-    if ((rc = h2d(b->seqs, seqs, b->total_chars, st))) return rc;
+    if (!dev_seqs && (rc = h2d(b->seqs, seqs, b->total_chars, st))) return rc;
     if ((rc = h2d(b->offsets, offsets, ((size_t)n_reads + 1) * 8, st))) return rc;
     if ((rc = h2d(b->koff, koff_host->data(), ((size_t)n_reads + 1) * 8, st))) return rc;
-    stats->h2d_bytes += b->total_chars + 2 * ((size_t)n_reads + 1) * 8;
+    stats->h2d_bytes += (dev_seqs ? 0 : b->total_chars) + 2 * ((size_t)n_reads + 1) * 8;
     return 0;
 }
 
@@ -1071,6 +1076,162 @@ int render_text(const mgb_index_t *index, TextArgs &ta, DevBufs &tb, Stream &st,
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------
+// file route (mgb_align_fastx_text): one chunk of FASTA/FASTQ bytes parsed into reads and headers on the device
+// (fastx_core.cuh). The parsed arrays stay in the workspace of the call; only their offsets come back.
+// ---------------------------------------------------------------------------------------
+struct FastxDev {
+    bool refused = false;                      // the chunk has neither parallel form: the host restatement parses it
+    char *seqs = nullptr, *names = nullptr;    // device arrays
+    std::vector<uint64_t> offsets, name_offsets;
+    uint64_t consumed = 0;
+};
+
+// exclusive scan of off[0, n) in place, total at off[n] (fastx_core.cuh k_fastx_scan_up / _down; the tile sums, a
+// thousandth of the elements, by k_text_scan's one block)
+int scan_u64(uint64_t *off, uint32_t n, Stream &st, DevBufs &bufs) {
+#if defined(MGB_HOST_EMU)
+    (void)st; (void)bufs;
+    uint64_t t = 0;
+    for (uint32_t i = 0; i < n; ++i) { const uint64_t v = off[i]; off[i] = t; t += v; }
+    off[n] = t;
+#else
+    const uint32_t n_tiles = (n + kFastxScanTile - 1) / kFastxScanTile;
+    uint64_t *tile_sum = nullptr;
+    if (int rc = bufs.alloc(&tile_sum, (size_t)n_tiles + 1)) return rc;
+    if (n_tiles) k_fastx_scan_up<<<n_tiles, 256, 0, st.s>>>(off, n, tile_sum);
+    k_text_scan<<<1, 1024, 0, st.s>>>(tile_sum, n_tiles);
+    k_fastx_scan_down<<<n_tiles ? n_tiles : 1, 256, 0, st.s>>>(off, n, tile_sum, n_tiles);
+    CUDA_TRY(cudaGetLastError());
+#endif
+    return 0;
+}
+
+int fastx_parse_dev(const mgb_index_t *index, const char *buf, uint64_t bytes, bool at_eof, const char *delim,
+                    bool fwd_rev, Stream &st, DevBufs &bufs, FastxDev *out, mgb_stats_t *stats) {
+    if (bytes >= 0xffffffffull || (delim && std::strlen(delim) > kFastxMaxDelim)) { out->refused = true; return 0; }
+    int rc;
+    FastxArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.n = (uint32_t)bytes; a.at_eof = at_eof; a.fwd_rev = fwd_rev;
+    a.n_tiles = (uint32_t)((bytes + kFastxTile - 1) / kFastxTile);
+    if (delim) { a.has_delim = 1; a.dlen = (uint32_t)std::strlen(delim); std::memcpy(a.delim, delim, a.dlen); }
+    uint8_t *d_buf = nullptr;
+    if ((rc = bufs.alloc(&d_buf, (size_t)a.n_tiles * kFastxTile + 16))) return rc;
+    if ((rc = bufs.alloc(&a.tile_nl, (size_t)a.n_tiles + 1))) return rc;
+    if ((rc = bufs.alloc(&a.sum, 1))) return rc;
+    if (bytes && (rc = h2d(d_buf, buf, bytes, st))) return rc;
+    if ((rc = dev_zero(a.sum, sizeof(FastxSummary), st))) return rc;
+    a.buf = d_buf;
+    stats->h2d_bytes += bytes;
+    [[maybe_unused]] const unsigned tiles_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(a.n_tiles, (uint64_t)index->num_sms * 8));
+    // line ends
+    uint64_t n_nl = 0;
+#if defined(MGB_HOST_EMU)
+    for (uint32_t t = 0; t < a.n_tiles; ++t) {
+        uint64_t c = 0;
+        for (uint32_t i = t * kFastxTile; i < a.n && i < (t + 1) * kFastxTile; ++i) c += buf[i] == '\n';
+        a.tile_nl[t] = c;
+    }
+#else
+    if (a.n_tiles) {
+        k_fastx_count<<<tiles_grid, 256, 0, st.s>>>(a);
+        CUDA_TRY(cudaGetLastError());
+    }
+#endif
+    if ((rc = scan_u64(a.tile_nl, a.n_tiles, st, bufs))) return rc;
+    if ((rc = d2h(&n_nl, a.tile_nl + a.n_tiles, 8, st))) return rc;
+#if !defined(MGB_HOST_EMU)
+    CUDA_TRY(cudaStreamSynchronize(st.s));
+#endif
+    a.n_nl = (uint32_t)n_nl;
+    a.n_lines = a.n_nl + (bytes && buf[bytes - 1] != '\n' ? 1 : 0);
+    if ((rc = bufs.alloc(&a.nl, (size_t)a.n_nl + 1))) return rc;
+    [[maybe_unused]] const unsigned lines_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)a.n_lines + 255) / 256,
+                                                                                   (uint64_t)index->num_sms * 8));
+    FastxSummary sum;
+    std::memset(&sum, 0, sizeof(sum));
+#if defined(MGB_HOST_EMU)
+    {
+        uint64_t o = 0;
+        for (uint32_t i = 0; i < a.n; ++i) if (buf[i] == '\n') a.nl[o++] = i;
+        a.nl[a.n_nl] = a.n;
+        for (uint32_t i = 0; i < a.n_lines; ++i) {
+            bool hdr;
+            fastx_classify_line(a, i, &sum.flags, &hdr, &sum.q_cut);
+            if (hdr) { ++sum.n_hdr; sum.last_hdr = fastx_line_begin(a, i) + 1; }
+        }
+    }
+#else
+    if (a.n_tiles) k_fastx_lines<<<tiles_grid, 256, 0, st.s>>>(a);
+    else k_fastx_lines<<<1, 32, 0, st.s>>>(a);        // (nl[0] = 0 for an empty chunk)
+    if (a.n_lines) k_fastx_classify<<<lines_grid, 256, 0, st.s>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    if ((rc = d2h(&sum, a.sum, sizeof(sum), st))) return rc;
+    CUDA_TRY(cudaStreamSynchronize(st.s));
+#endif
+    stats->kernel_launches += 6;
+    stats->d2h_bytes += 8 + sizeof(sum);
+    if ((sum.flags & kFastxFastaBad) && (sum.flags & kFastxFastqBad)) { out->refused = true; return 0; }
+    a.fastq = (sum.flags & kFastxFastaBad) != 0;
+    uint32_t n_rec;
+    if (a.fastq) {
+        n_rec = (at_eof ? a.n_lines : a.n_nl) / 4;
+        out->consumed = sum.q_cut ? sum.q_cut - 1 : bytes;
+    } else {
+        n_rec = at_eof ? sum.n_hdr : sum.n_hdr ? sum.n_hdr - 1 : 0;
+        out->consumed = at_eof ? bytes : sum.last_hdr ? sum.last_hdr - 1 : 0;
+    }
+    const uint64_t copies = fwd_rev ? 2 : 1, n_out = copies * n_rec;
+    if (n_out > 0xffffffffull) return fail(MGB_ERR_OVERFLOW, "more than 2^32 - 1 records in one chunk");
+    out->offsets.assign(n_out + 1, 0);
+    out->name_offsets.assign(n_out + 1, 0);
+    // the packed arrays: at most `copies` times the chunk's bytes (and a delimiter per record), and the slack the read
+    // kernels' word loads go past the last read
+    if ((rc = bufs.alloc(&out->seqs, copies * bytes + 128))) return rc;
+    if ((rc = bufs.alloc(&out->names, copies * (bytes + (uint64_t)n_rec * a.dlen) + 128))) return rc;
+    if (!n_rec) return 0;
+    a.n_rec = n_rec;
+    a.seqs = out->seqs; a.names = out->names;
+    if ((rc = bufs.alloc(&a.lh, (size_t)a.n_lines + 1))) return rc;
+    if ((rc = bufs.alloc(&a.ls, (size_t)a.n_lines + 1))) return rc;
+    if ((rc = bufs.alloc(&a.ln, (size_t)a.n_lines + 1))) return rc;
+    if (!a.fastq && (rc = bufs.alloc(&a.rec_line, (size_t)sum.n_hdr + 1))) return rc;
+    if ((rc = bufs.alloc(&a.offsets, n_out + 1))) return rc;
+    if ((rc = bufs.alloc(&a.name_offsets, n_out + 1))) return rc;
+#if defined(MGB_HOST_EMU)
+    for (uint32_t i = 0; i < a.n_lines; ++i) fastx_role_line(a, i);
+#else
+    k_fastx_roles<<<lines_grid, 256, 0, st.s>>>(a);
+    CUDA_TRY(cudaGetLastError());
+#endif
+    if ((rc = scan_u64(a.lh, a.n_lines, st, bufs)) || (rc = scan_u64(a.ls, a.n_lines, st, bufs))
+        || (rc = scan_u64(a.ln, a.n_lines, st, bufs)))
+        return rc;
+#if defined(MGB_HOST_EMU)
+    if (!a.fastq) {
+        for (uint32_t i = 0; i < a.n_lines; ++i) if (a.lh[i + 1] != a.lh[i]) a.rec_line[a.lh[i]] = i;
+        a.rec_line[a.lh[a.n_lines]] = a.n_lines;
+    }
+    for (uint32_t r = 0; r < n_rec; ++r) fastx_gather_record(a, r);
+#else
+    if (!a.fastq) k_fastx_records<<<lines_grid, 256, 0, st.s>>>(a);
+    {
+        const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n_rec + 7) / 8, (uint64_t)index->num_sms * 16));
+        k_fastx_gather<<<grid, 256, 0, st.s>>>(a);       // a warp per record
+    }
+    CUDA_TRY(cudaGetLastError());
+#endif
+    stats->kernel_launches += a.fastq ? 11 : 12;
+    if ((rc = d2h(out->offsets.data(), a.offsets, (n_out + 1) * 8, st))) return rc;
+    if ((rc = d2h(out->name_offsets.data(), a.name_offsets, (n_out + 1) * 8, st))) return rc;
+#if !defined(MGB_HOST_EMU)
+    CUDA_TRY(cudaStreamSynchronize(st.s));
+#endif
+    stats->d2h_bytes += 16 * (n_out + 1);
+    return 0;
+}
+
 } // namespace
 
 extern "C" {
@@ -1174,6 +1335,7 @@ struct Piece {
     int text_format = 0;
     int32_t min_path_score = 0;
     const char *names = nullptr; const uint64_t *name_offsets = nullptr;
+    bool dev_input = false;          // reads and headers are device memory (the file route), offsets host memory
     HostBuf text;
     uint64_t text_bytes = 0;
     mgb_stats_t stats;
@@ -1287,12 +1449,15 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
     std::memset(&res->stats, 0, sizeof(res->stats));
     res->lo = lo; res->n_reads = n_reads;
     // offsets relative to the first character of the piece
+    // (device-resident reads: the piece starts at the 16-byte word that holds its first character, as the kernels'
+    // word reads assume)
     std::vector<uint64_t> offs_local;
     const uint64_t *offsets = all_offsets + lo;
-    const char *seqs = all_seqs ? all_seqs + all_offsets[lo] : nullptr;
+    const uint64_t base = res->dev_input ? all_offsets[lo] & ~15ull : all_offsets[lo];
+    const char *seqs = all_seqs ? all_seqs + base : nullptr;
     if (all_offsets[lo]) {
         offs_local.resize((size_t)n_reads + 1);
-        for (uint32_t r = 0; r <= n_reads; ++r) offs_local[r] = all_offsets[lo + r] - all_offsets[lo];
+        for (uint32_t r = 0; r <= n_reads; ++r) offs_local[r] = all_offsets[lo + r] - base;
         offsets = offs_local.data();
     }
     const bool text = res->text_format != 0;
@@ -1327,19 +1492,19 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
         cudaEventRecord(ev[0], st.s);
 #endif
         tick("setup");
-        rc = upload_batch(index, seqs, offsets, n_reads, both, st, bufs, &b, &koff, &res->stats);
+        rc = upload_batch(index, seqs, offsets, n_reads, both, st, bufs, &b, &koff, &res->stats, res->dev_input);
         // text route: the headers go up with the reads (workspace slots from 96 on: above every pass's heap, below)
         DevBufs text_bufs(st, wsg.w, 96);
         TextArgs ta;
         std::memset(&ta, 0, sizeof(ta));
         if (!rc && text) {
             const uint64_t name_bytes = name_offs[n_reads];
-            char *d_names = nullptr; uint64_t *d_name_off = nullptr;
-            if (!rc) rc = text_bufs.alloc(&d_names, name_bytes + 64);
+            char *d_names = res->dev_input ? const_cast<char*>(names) : nullptr; uint64_t *d_name_off = nullptr;
+            if (!rc && !res->dev_input) rc = text_bufs.alloc(&d_names, name_bytes + 64);
             if (!rc) rc = text_bufs.alloc(&d_name_off, (size_t)n_reads + 1);
-            if (!rc && name_bytes) rc = h2d(d_names, names, name_bytes, st);
+            if (!rc && name_bytes && !res->dev_input) rc = h2d(d_names, names, name_bytes, st);
             if (!rc) rc = h2d(d_name_off, name_offs, ((size_t)n_reads + 1) * 8, st);
-            res->stats.h2d_bytes += name_bytes + ((size_t)n_reads + 1) * 8;
+            res->stats.h2d_bytes += (res->dev_input ? 0 : name_bytes) + ((size_t)n_reads + 1) * 8;
             ta.seqs = b.seqs; ta.offsets = b.offsets; ta.names = d_names; ta.name_off = d_name_off;
             ta.n_reads = n_reads; ta.k = index->view.k; ta.json = res->text_format == MGB_TEXT_JSON;
             ta.result_nodes = dcfg.result_nodes; ta.min_path_score = res->min_path_score;
@@ -1622,7 +1787,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
                                  n_reads - n_rest[1], n_rest[1]);
                     std::fprintf(stderr, "[mgb] reads %u+%u k_exact_reads answered %u, left to k_align %u\n", lo, n_reads,
                                  n_rest[1] - n_rest[0], n_rest[0]);
-                    if (n_rest[0] <= 8)
+                    if (n_rest[0] <= 8 && !res->dev_input)
                         debug_left_over(index->view, pa, ea, seqs, offsets, koff, b, summary, d_rest, n_rest[0], lo,
                                         n_reads, st);
                 }
@@ -1815,9 +1980,10 @@ int mgb_config_check(const mgb_index_t *index, const mgb_config_t *config) {
 } // extern "C"
 
 // mgb_align_batch (text_format 0) and mgb_align_batch_text (MGB_TEXT_TSV / MGB_TEXT_JSON, with the headers)
+// dev_input: seqs and names are device memory (the file route's parsed chunk), the offsets host memory
 static int align_batch(const mgb_index_t *index, const mgb_config_t *config, const char *seqs, const uint64_t *offsets,
                        const char *names, const uint64_t *name_offsets, uint32_t n_reads, int text_format,
-                       mgb_results_t **out) {
+                       mgb_results_t **out, bool dev_input = false) {
     DevConfig dcfg;
     std::string err;
     int rc = lower_config(*config, index->view.k, index->alphabet, &dcfg, &err);
@@ -1876,6 +2042,7 @@ static int align_batch(const mgb_index_t *index, const mgb_config_t *config, con
         pieces[i].text_format = text_format;
         pieces[i].min_path_score = config->min_path_score;
         pieces[i].names = names; pieces[i].name_offsets = name_offsets;
+        pieces[i].dev_input = dev_input;
     }
     if (n_pieces == 1) {
         rc = align_range(index, dcfg, seqs, offsets, 0, n_reads, &pieces[0]);
@@ -1982,6 +2149,122 @@ int mgb_align_batch_text(const mgb_index_t *index, const mgb_config_t *config, c
     for (uint32_t r = 0; r < n_reads; ++r)
         if (header_offsets[r + 1] < header_offsets[r]) return fail(MGB_ERR_INVALID_ARGUMENT, "header offsets must be non-decreasing");
     return align_batch(index, config, seqs, offsets, headers, header_offsets, n_reads, format, out);
+}
+
+// the chunk's records on the device route, or the host restatement's when the device route refuses the chunk
+// (or device_route is false); *parse: the file route's own copies and launches
+static int fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes, bool at_eof, const char *delim,
+                       bool fwd_rev, bool device_route, Stream &st, DevBufs &bufs, FastxDev *dev, FastxRecords *host,
+                       uint64_t *consumed, int *ended, mgb_stats_t *parse) {
+    *consumed = 0; *ended = 0;
+    dev->refused = !device_route;
+    if (device_route) {
+        const int rc = fastx_parse_dev(index, buf, bytes, at_eof, delim, fwd_rev, st, bufs, dev, parse);
+        if (rc) return rc;
+    }
+    if (dev->refused) fastx_parse_host(buf, bytes, at_eof, delim, fwd_rev, host, consumed, ended);
+    else *consumed = dev->consumed;
+    return MGB_OK;
+}
+
+// a workspace of the index held for the duration of a call (the parsed chunk lives in it)
+struct CallWorkspace {
+    const mgb_index_t *ix; Workspace *w; Stream st;
+    explicit CallWorkspace(const mgb_index_t *i) : ix(i), w(i->ws_acquire()) {}
+    ~CallWorkspace() { ix->ws_release(w); }
+    int ready() {
+#if !defined(MGB_HOST_EMU)
+        CUDA_TRY(cudaSetDevice(ix->device));
+        if (int rc = w->ready()) return rc;
+        st.s = w->stream;
+#endif
+        return MGB_OK;
+    }
+};
+
+int mgb_align_fastx_text(const mgb_index_t *index, const mgb_config_t *config, const char *buf, uint64_t bytes,
+                         int at_eof, const char *comment_delim, int flags, int format, uint64_t *consumed, int *ended,
+                         mgb_results_t **out) {
+    if (!index || !config || !consumed || !ended || !out || (!buf && bytes)) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (format != MGB_TEXT_TSV && format != MGB_TEXT_JSON)
+        return fail(MGB_ERR_INVALID_ARGUMENT, "format must be MGB_TEXT_TSV or MGB_TEXT_JSON");
+    if (flags & ~MGB_FASTX_FWD_AND_REVERSE) return fail(MGB_ERR_INVALID_ARGUMENT, "unknown flags");
+    CallWorkspace cw(index);
+    int rc = cw.ready();
+    if (rc) return rc;
+    DevBufs bufs(cw.st, cw.w, 0);
+    FastxDev dev;
+    FastxRecords host;
+    mgb_stats_t parse;
+    std::memset(&parse, 0, sizeof(parse));
+    const bool fwd_rev = flags & MGB_FASTX_FWD_AND_REVERSE;
+    rc = fastx_parse(index, buf, bytes, at_eof != 0, comment_delim, fwd_rev, true, cw.st, bufs, &dev, &host, consumed,
+                     ended, &parse);
+    if (rc) return rc;
+    const std::vector<uint64_t> &offs = dev.refused ? host.offsets : dev.offsets;
+    if (offs.size() - 1 > 0xffffffffull) return fail(MGB_ERR_OVERFLOW, "more than 2^32 - 1 records in one chunk");
+    const uint32_t n = (uint32_t)(offs.size() - 1);
+    rc = dev.refused ? align_batch(index, config, host.seqs.data(), host.offsets.data(), host.names.data(),
+                                   host.name_offsets.data(), n, format, out)
+                     : align_batch(index, config, dev.seqs, dev.offsets.data(), dev.names, dev.name_offsets.data(), n,
+                                   format, out, true);
+    if (rc) return rc;
+    mgb_stats_t &t = (*out)->stats;
+    t.h2d_bytes += parse.h2d_bytes; t.d2h_bytes += parse.d2h_bytes; t.kernel_launches += parse.kernel_launches;
+    return MGB_OK;
+}
+
+int mgb_fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes, int at_eof, const char *comment_delim,
+                    int flags, int device_route, char *seqs, uint64_t max_seq_bytes, uint64_t *offsets, char *names,
+                    uint64_t max_name_bytes, uint64_t *name_offsets, uint64_t max_records, uint64_t *n_records,
+                    uint64_t *consumed, int *ended, int *refused) {
+    if ((device_route && !index) || (!buf && bytes) || !seqs || !offsets || !names || !name_offsets || !n_records
+        || !consumed || !ended || !refused)
+        return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (flags & ~MGB_FASTX_FWD_AND_REVERSE) return fail(MGB_ERR_INVALID_ARGUMENT, "unknown flags");
+    FastxDev dev;
+    FastxRecords host;
+    mgb_stats_t parse;
+    std::memset(&parse, 0, sizeof(parse));
+    const bool fwd_rev = flags & MGB_FASTX_FWD_AND_REVERSE;
+    auto fits = [&](const std::vector<uint64_t> &o, const std::vector<uint64_t> &no) {
+        return o.size() - 1 <= max_records && o.back() <= max_seq_bytes && no.back() <= max_name_bytes;
+    };
+    if (!device_route) {
+        Stream st;
+        DevBufs none(st, nullptr, 0);
+        fastx_parse(index, buf, bytes, at_eof != 0, comment_delim, fwd_rev, false, st, none, &dev, &host, consumed,
+                    ended, &parse);
+    } else {
+        CallWorkspace cw(index);
+        int rc = cw.ready();
+        if (rc) return rc;
+        DevBufs bufs(cw.st, cw.w, 0);
+        if ((rc = fastx_parse(index, buf, bytes, at_eof != 0, comment_delim, fwd_rev, true, cw.st, bufs, &dev, &host,
+                              consumed, ended, &parse)))
+            return rc;
+        if (!dev.refused) {
+            if (!fits(dev.offsets, dev.name_offsets)) return fail(MGB_ERR_OVERFLOW, "output arrays too small");
+            if ((rc = d2h(seqs, dev.seqs, dev.offsets.back(), cw.st))) return rc;
+            if ((rc = d2h(names, dev.names, dev.name_offsets.back(), cw.st))) return rc;
+#if !defined(MGB_HOST_EMU)
+            CUDA_TRY(cudaStreamSynchronize(cw.st.s));
+#endif
+            std::memcpy(offsets, dev.offsets.data(), dev.offsets.size() * 8);
+            std::memcpy(name_offsets, dev.name_offsets.data(), dev.name_offsets.size() * 8);
+            *n_records = dev.offsets.size() - 1;
+            *refused = 0;
+            return MGB_OK;
+        }
+    }
+    *refused = device_route ? 1 : 0;
+    if (!fits(host.offsets, host.name_offsets)) return fail(MGB_ERR_OVERFLOW, "output arrays too small");
+    std::memcpy(seqs, host.seqs.data(), host.seqs.size());
+    std::memcpy(names, host.names.data(), host.names.size());
+    std::memcpy(offsets, host.offsets.data(), host.offsets.size() * 8);
+    std::memcpy(name_offsets, host.name_offsets.data(), host.name_offsets.size() * 8);
+    *n_records = host.offsets.size() - 1;
+    return MGB_OK;
 }
 
 int mgb_results_text(const mgb_results_t *results, const char **text, uint64_t *bytes) {
