@@ -420,13 +420,13 @@ struct ReadAligner {
         return c.fmt == FMT_FULL ? sv == cellE(c, j) : (cell_flags(c, j) & CF_INS) != 0;
     }
     MGB_HD bool bt_ins_ext(const ColMeta &c, int j) {
-        return c.fmt == FMT_FULL ? cellE(c, j) == cellE(c, j - 1) + cfg.gap_ext : (cell_flags(c, j) & CF_INS_EXT) != 0;
+        return c.fmt == FMT_FULL ? cellE(c, j) == wadd(cellE(c, j - 1), cfg.gap_ext) : (cell_flags(c, j) & CF_INS_EXT) != 0;
     }
     MGB_HD bool bt_is_del(const ColMeta &c, int j, score_t sv) {
         return c.fmt == FMT_FULL ? sv == cellF(c, j) : (cell_flags(c, j) & CF_DEL) != 0;
     }
     MGB_HD bool bt_del_ext(const ColMeta &c, const ColMeta &p, int pos) {
-        return c.fmt == FMT_FULL ? cellF(c, pos - c.trim) == cellF(p, pos - p.trim) + c.score + cfg.gap_ext
+        return c.fmt == FMT_FULL ? cellF(c, pos - c.trim) == wadd(wadd(cellF(p, pos - p.trim), c.score), cfg.gap_ext)
                                  : (cell_flags(c, pos - c.trim) & CF_DEL_EXT) != 0;
     }
 
@@ -1850,7 +1850,7 @@ struct ReadAligner {
     // extend_ins_end (extender.cpp:293-328); returns the new size. `sc` may migrate to the arena.
     MGB_HD int extend_ins_end(Scratch &sc, int size, int max_size, score_t cutoff) {
         if (size >= max_size) return size;
-        score_t ins = imax(sc.S[size - 1] + cfg.gap_open, sc.E[size - 1] + cfg.gap_ext);
+        score_t ins = imax(wadd(sc.S[size - 1], cfg.gap_open), wadd(sc.E[size - 1], cfg.gap_ext));
         if (ins < cutoff) return size;
         const uint32_t diff = (uint32_t)ins - (uint32_t)cutoff;              // ins >= cutoff
         const uint32_t extra = cfg.gap_ext < 0 ? diff / (uint32_t)(-cfg.gap_ext) : 0x7fffffffu;
@@ -1867,7 +1867,7 @@ struct ReadAligner {
             sc = big;
         }
         for (int t = wlane(); t < cnt + 5; t += kWarp) {
-            score_t v = t < cnt ? ins + t * cfg.gap_ext : kNinf;
+            score_t v = t < cnt ? wadd(ins, t * cfg.gap_ext) : kNinf;
             sc.S[size + t] = v; sc.E[size + t] = v; sc.F[size + t] = kNinf;
         }
         wsync();
@@ -1880,27 +1880,27 @@ struct ReadAligner {
                               int n, int prof_base, score_t cutoff, int code, score_t add, bool use_del) {
         const int n4 = (n + 3) & ~3;
         const score_t go = cfg.gap_open, ge = cfg.gap_ext;
-        int carry = kNinf + ge;                        // a[-1] = E[0] + ge, E[0] = ninf
+        int carry = wadd(kNinf, ge);                       // a[-1] = E[0] + ge, E[0] = ninf
         for (int base = 0; base < n4; base += kWarp) {
             int j = base + wlane();
             bool act = j < n4;
             score_t mval = kNinf, del = kNinf;
             if (act) {
                 score_t match = kNinf;
-                if (j) match = pS[j - 1] + prof_score(s, prof_base + j, code) + add;
-                if (use_del) del = imax(pS[j] + go, pF[j] + ge) + add;
+                if (j) match = wadd(wadd(pS[j - 1], prof_score(s, prof_base + j, code)), add);
+                if (use_del) del = wadd(imax(wadd(pS[j], go), wadd(pF[j], ge)), add);
                 mval = imax(match, del);
             }
             // a[j] = m[j] + go - j*ge ; E[j+1] = prefmax(a)[j] + j*ge
-            int a = act ? mval + go - j * ge : INT32_MIN;
+            int a = act ? wsub(wadd(mval, go), j * ge) : INT32_MIN;
             int incl = wscan_max(a);
             incl = imax(incl, carry);
             int excl = wshfl_up1(incl, carry);         // prefix max over i < j (incl. a[-1])
             if (act) {
-                score_t e_j = j ? excl + (j - 1) * ge : kNinf;    // E[j]
+                score_t e_j = j ? wadd(excl, (j - 1) * ge) : kNinf;    // E[j]
                 score_t sv = imax(mval, e_j);
                 sc.F[j] = del;
-                sc.E[j + 1] = incl + j * ge;                      // E[j + 1]
+                sc.E[j + 1] = wadd(incl, j * ge);                      // E[j + 1]
                 sc.S[j] = sv > cutoff - 1 ? sv : kNinf;
             }
             carry = wbcast(incl, kWarp - 1);
@@ -1908,7 +1908,7 @@ struct ReadAligner {
         wsync();
         if (size0 > imax(1, n)) {                      // scalar tail (:284-289)
             int j = size0 - 1;
-            score_t t = imax(pS[j - 1] + add + prof_score(s, prof_base + j, code), sc.E[j]);
+            score_t t = imax(wadd(wadd(pS[j - 1], add), prof_score(s, prof_base + j, code)), sc.E[j]);
             if (t >= cutoff) sc.S[j] = t;
             wsync();
         }
@@ -1981,9 +1981,9 @@ struct ReadAligner {
             const score_t pf_j = act ? pF[j] : kNinf;
             pr[c] = prof(j);
             psm1[c] = prev; pfv[c] = pf_j;
-            const score_t match = (act && j) ? prev + pr[c] + add : kNinf;
+            const score_t match = (act && j) ? wadd(wadd(prev, pr[c]), add) : kNinf;
             // (DPX add-max forms of max(S + go, F + ge) and of the running maximum)
-            const score_t del = (act && use_del) ? iaddmax(ps_j, go, pf_j + ge) + add : kNinf;
+            const score_t del = (act && use_del) ? wadd(iaddmax(ps_j, go, wadd(pf_j, ge)), add) : kNinf;
             mval[c] = imax(match, del);
             r.F[c] = act ? del : kNinf;
             // a[j] = m[j] + go - j*ge ; E[j+1] = prefmax(a)[j] + j*ge
@@ -1992,19 +1992,19 @@ struct ReadAligner {
             prev = ps_j;                                   // pS[j] for cell j + 1 (valid while j + 1 <= n4)
         }
         // prefix max over the previous lanes (incl. a[-1] = E[0] + ge, E[0] = ninf)
-        const int lane_incl = imax(wscan_max(loc), kNinf + ge);
-        const int lane_excl = wshfl_up1(lane_incl, kNinf + ge);
+        const int lane_incl = imax(wscan_max(loc), wadd(kNinf, ge));
+        const int lane_excl = wshfl_up1(lane_incl, wadd(kNinf, ge));
 #if MGB_DEVICE_CODE
 #pragma unroll
 #endif
         for (int c = 0; c < kCPL; ++c) {
             const int j = j0 + c;
             const int excl = c ? imax(lane_excl, aloc[c ? c - 1 : 0]) : lane_excl;      // prefix max over i < j
-            const score_t E_j = (j >= 1 && j <= n4) ? excl + (j - 1) * ge : kNinf;
+            const score_t E_j = (j >= 1 && j <= n4) ? wadd(excl, (j - 1) * ge) : kNinf;
             score_t S_j = kNinf;
             if (j < n4) { const score_t sv = imax(mval[c], E_j); S_j = sv > cutoff - 1 ? sv : kNinf; }
             if (size0 > imax(1, n) && j == size0 - 1) {                                 // scalar tail (:284-289)
-                const score_t tt = imax(psm1[c] + add + pr[c], E_j);
+                const score_t tt = imax(wadd(wadd(psm1[c], add), pr[c]), E_j);
                 if (tt >= cutoff) S_j = tt;
             }
             r.S[c] = S_j; r.E[c] = E_j;
@@ -2013,7 +2013,7 @@ struct ReadAligner {
         int size = size0;
         if (size0 < max_size) {
             const score_t s_last = cell_bcast(r.S, size0 - 1), e_last = cell_bcast(r.E, size0 - 1);
-            const score_t ins = imax(s_last + go, e_last + ge);
+            const score_t ins = imax(wadd(s_last, go), wadd(e_last, ge));
             if (ins >= cutoff) {
                 const uint32_t diff = (uint32_t)ins - (uint32_t)cutoff;                  // ins >= cutoff
                 const uint32_t extra = ge_shift >= 0 ? diff >> ge_shift
@@ -2028,7 +2028,7 @@ struct ReadAligner {
                     const int j = j0 + c;
                     if (j >= size0) {
                         const bool in = j < size0 + cnt;
-                        r.S[c] = in ? ins + (j - size0) * ge : kNinf;
+                        r.S[c] = in ? wadd(ins, (j - size0) * ge) : kNinf;
                         r.E[c] = r.S[c]; r.F[c] = kNinf;
                     }
                 }
@@ -2041,8 +2041,8 @@ struct ReadAligner {
 #pragma unroll
 #endif
         for (int c = 0; c < kCPL; ++c) {
-            r.fl[c] = (uint8_t)((r.S[c] == r.E[c] ? CF_INS : 0) | (r.E[c] == e_prev + ge ? CF_INS_EXT : 0)
-                              | (r.S[c] == r.F[c] ? CF_DEL : 0) | (r.F[c] == pfv[c] + add + ge ? CF_DEL_EXT : 0));
+            r.fl[c] = (uint8_t)((r.S[c] == r.E[c] ? CF_INS : 0) | (r.E[c] == wadd(e_prev, ge) ? CF_INS_EXT : 0)
+                              | (r.S[c] == r.F[c] ? CF_DEL : 0) | (r.F[c] == wadd(wadd(pfv[c], add), ge) ? CF_DEL_EXT : 0));
             e_prev = r.E[c];
         }
         return size;
@@ -2380,7 +2380,7 @@ struct ReadAligner {
                         const int j = j0 + c;
                         const bool cell = j < size;
                         if (cell && r.S[c] == max_val) bd = imin(bd, iabs(j + begin - diag_i));
-                        if (!in_seed && cell && r.S[c] + cx[s].ps[start + begin + j] >= extension_cutoff) he = true;
+                        if (!in_seed && cell && wadd(r.S[c], cx[s].ps[start + begin + j]) >= extension_cutoff) he = true;
                     }
                     const int gd = wreduce_min(bd);
                     int bj = 0x7fffffff;
@@ -2492,7 +2492,7 @@ struct ReadAligner {
                     if (v != kNinf) mn = imin(mn, v);
                     int d = iabs(j + begin - diag_i);
                     if (v > bs || (v == bs && d < bd)) { bs = v; bd = d; bj = j; }
-                    if (v + cx[s].ps[start + begin + j] >= extension_cutoff) he = true;
+                    if (wadd(v, cx[s].ps[start + begin + j]) >= extension_cutoff) he = true;
                 }
                 min_cell_score = imin(min_cell_score, wreduce_min(mn));
                 score_t gbs = wreduce_max(bs);
@@ -2694,7 +2694,7 @@ struct ReadAligner {
                 const int j = j0 + c;
                 const bool cell = j < size;
                 if (cell && r.S[c] == max_val) bkey = imin(bkey, (iabs(j + begin - diag_i) << 5) | j);
-                if (!in_seed && cell && r.S[c] + ps[start + begin + j] >= ext_cut) he = true;
+                if (!in_seed && cell && wadd(r.S[c], ps[start + begin + j]) >= ext_cut) he = true;
             }
             const int max_pos = (wreduce_min(bkey) & 31) + begin;
             // ---- convergence filter, first half (update_seed_filter, :100-156): find the node's entry. Cases
@@ -2868,12 +2868,12 @@ struct ReadAligner {
                         score_t sv = cellS(col, pos), sp = cellS(par, pos_p);
                         if (sv == kNinf || sp == kNinf) continue;
                         score_t end_bonus = start_pos == last_pos ? right_end_bonus : 0;
-                        if (sv + end_bonus >= min_start_score) {
-                            bool is_match = sv == sp + col.score + prof_score(s, seed_clipping + start_pos, code)
+                        if (wadd(sv, end_bonus) >= min_start_score) {
+                            bool is_match = sv == wadd(wadd(sp, col.score), prof_score(s, seed_clipping + start_pos, code))
                                 && prof_is_match(s, seed_clipping + start_pos, code);
                             if (is_match || start_pos == last_pos || col.is_tip) {
                                 BtStart &o = which ? b : a;
-                                o.score = sv + end_bonus;
+                                o.score = wadd(sv, end_bonus);
                                 o.neg_off_diag = -iabs(start_pos - col.offset + seed_off_m1);
                                 o.neg_i = -(int)i; o.pos = start_pos;
                             }
@@ -2968,7 +2968,7 @@ struct ReadAligner {
                             const bool ins = bt_is_ins(c_t, ci, sv) && (t || cur_op == 0xffu || cur_op != OP_D);
                             const int code = encode_char(c_t.c);
                             good = sv != kNinf && !ins
-                                && sv == cellS(p_t, pi) + c_t.score + prof_score(s, seed_clipping + pos_t, code);
+                                && sv == wadd(wadd(cellS(p_t, pi), c_t.score), prof_score(s, seed_clipping + pos_t, code));
                             is_m = prof_is_match(s, seed_clipping + pos_t, code);
                         }
                     }
@@ -3038,8 +3038,8 @@ struct ReadAligner {
                         --pos;
                     }
                 } else if (pos && pos >= trim_p + 1
-                        && sv == cellS(par, pos - trim_p - 1) + col.score
-                                + prof_score(s, seed_clipping + pos, code)) {
+                        && sv == wadd(wadd(cellS(par, pos - trim_p - 1), col.score),
+                                      prof_score(s, seed_clipping + pos, code))) {
                     ++n_trace;
                     if (n_seq >= (int)caps.aln_seq) { overflow = true; return 0; }
                     m.bt_seq()[n_seq++] = col.c;
@@ -3084,7 +3084,7 @@ struct ReadAligner {
             if (n_trace >= min_trace_length && n_path && path_back_nonzero) {
                 const ColMeta cj = j ? col : m.cols()[0];
                 score_t cur_cell_score = cellS(cj, pos - cj.trim);
-                best_score = imax(best_score, score - cur_cell_score);
+                best_score = imax(best_score, wsub(score, cur_cell_score));
                 if ((int64_t)score - min_cell_score < best_score) break;
 
                 const ColMeta root = m.cols()[0];

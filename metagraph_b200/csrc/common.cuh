@@ -107,12 +107,18 @@ inline int nth_set32(uint32_t x, int t) {
 }
 #endif
 
-// max(a + b, c): one DPX instruction (VIADDMNMX) on the device
+// a + b and a - b modulo 2^32. Past the scores the reference keeps in range (ninf plus more than one penalty, DESIGN.md
+// §5) its epi32 column update wraps; these wrap the same way, with no undefined behaviour in the host build.
+MGB_HOSTDEV int wadd(int a, int b) { return (int)((uint32_t)a + (uint32_t)b); }
+MGB_HOSTDEV int wsub(int a, int b) { return (int)((uint32_t)a - (uint32_t)b); }
+
+// max(a + b, c), a + b modulo 2^32: one DPX instruction (VIADDMNMX) on the device
 MGB_HD int iaddmax(int a, int b, int c) {
 #if MGB_DEVICE_CODE
     return __viaddmax_s32(a, b, c);
 #else
-    return a + b > c ? a + b : c;
+    const int t = wadd(a, b);
+    return t > c ? t : c;
 #endif
 }
 MGB_HOSTDEV int imin(int a, int b) { return a < b ? a : b; }

@@ -141,6 +141,12 @@ inline int lower_config(const mgb_config_t &c, uint32_t k, int alphabet, DevConf
                 if (g != q && c.score_matrix[g][q] >= m) ok = false;
             }
         }
+        // ... and ninf less a mismatch (or gap open), a gap open and an extension stays in int32: past that the reference's
+        // column update wraps (DESIGN.md §5) and the argument for the shortcut does not hold
+        int lo = c.gap_opening_penalty;
+        for (int a = 0; a < 128; ++a)
+            for (int b = 0; b < 128; ++b) lo = std::min(lo, (int)c.score_matrix[a][b]);
+        ok = ok && (int64_t)kNinf + lo + c.gap_opening_penalty + c.gap_extension_penalty >= INT32_MIN;
         d->exact_shortcut = ok ? 1 : 0;
     }
     d->sigma = at.sigma; d->has_complement = at.has_complement ? 1 : 0;

@@ -732,6 +732,9 @@ struct DPTColumn {
 };
 constexpr size_t kSizeofDPTColumn = 136; // sizeof(DefaultColumnExtender::DPTColumn) on LP64/libstdc++
 
+// simde_mm_add_epi32 lane: adds modulo 2^32 (the scalar statements of extender.cpp stay plain int adds)
+inline score_t add_epi32(score_t a, score_t b) { return (score_t)((uint32_t)a + (uint32_t)b); }
+
 // extender.cpp:209-290, lane-for-lane
 void update_column(size_t prev_end, const score_t *S_prev_v, const score_t *F_prev_v,
                    PVec &S_v, PVec &E_v, PVec &F_v, const score_t *profile_scores,
@@ -744,18 +747,18 @@ void update_column(size_t prev_end, const score_t *S_prev_v, const score_t *F_pr
         score_t match[4], del_score[4];
         for (size_t l = 0; l < 4; ++l) {
             if (j) {
-                match[l] = S_prev_v[j + l - 1] + profile_scores[j + l] + init_score;
+                match[l] = add_epi32(add_epi32(S_prev_v[j + l - 1], profile_scores[j + l]), init_score);
             } else if (l) {
-                match[l] = S_prev_v[l - 1] + profile_scores[l] + init_score;
+                match[l] = add_epi32(add_epi32(S_prev_v[l - 1], profile_scores[l]), init_score);
             } else {
                 match[l] = ninf;
             }
             del_score[l] = offset > 1
-                ? std::max(S_prev_v[j + l] + gap_open, F_prev_v[j + l] + gap_extend) + init_score
+                ? add_epi32(std::max(add_epi32(S_prev_v[j + l], gap_open), add_epi32(F_prev_v[j + l], gap_extend)), init_score)
                 : ninf;
             F_v[j + l] = del_score[l];
             match[l] = std::max(match[l], del_score[l]);
-            E_v[j + l + 1] = match[l] + gap_open;
+            E_v[j + l + 1] = add_epi32(match[l], gap_open);
         }
         E_v[j + 1] = std::max(E_v[j] + gap_extend, E_v[j + 1]);
         E_v[j + 2] = std::max(E_v[j + 1] + gap_extend, E_v[j + 2]);
