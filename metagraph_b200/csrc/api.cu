@@ -18,6 +18,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <numeric>
 #include <string>
 #include <vector>
 #if defined(_OPENMP)
@@ -35,6 +36,16 @@
 #else
     return 1;
 #endif
+}
+
+// memcpy of n bytes in 4 MiB chunks, on host_team() threads when there are more than four chunks
+static void parallel_copy(char *dst, const char *src, uint64_t n) {
+    const int64_t chunks = (int64_t)((n + (1 << 22) - 1) >> 22);
+    #pragma omp parallel for schedule(static) num_threads(host_team()) if (chunks > 4)
+    for (int64_t c = 0; c < chunks; ++c) {
+        const uint64_t o = (uint64_t)c << 22;
+        std::memcpy(dst + o, src + o, std::min<uint64_t>(1ull << 22, n - o));
+    }
 }
 
 #include "../../include/mgb.h"
@@ -61,6 +72,14 @@ namespace {
 thread_local std::string g_err;
 
 int fail(int code, const std::string &msg) { g_err = msg; return code; }
+
+void add_stats(mgb_stats_t &t, const mgb_stats_t &u) {
+    t.num_seeds += u.num_seeds; t.num_extensions += u.num_extensions;
+    t.num_explored_nodes += u.num_explored_nodes; t.dp_cells += u.dp_cells; t.dp_columns += u.dp_columns;
+    t.num_reads_retried += u.num_reads_retried; t.seed_kernel_ms += u.seed_kernel_ms;
+    t.align_kernel_ms += u.align_kernel_ms; t.h2d_ms += u.h2d_ms; t.d2h_ms += u.d2h_ms;
+    t.h2d_bytes += u.h2d_bytes; t.d2h_bytes += u.d2h_bytes; t.kernel_launches += u.kernel_launches;
+}
 
 
 #if !defined(MGB_HOST_EMU)
@@ -91,6 +110,9 @@ namespace {
 // ---------------------------------------------------------------------------------------
 // device memory helpers
 // ---------------------------------------------------------------------------------------
+// sync: waits for the stream's work (MGB_ERR_CUDA with the CUDA error text if it failed); record / elapsed_ms: the
+// workspace's events ev[i], which the device timers of mgb_stats_t are measured between. The emulation runs every
+// operation when it is issued, so these do nothing there.
 #if defined(MGB_HOST_EMU)
 struct Stream { int dummy; };
 inline int dev_alloc(void **p, size_t bytes, Stream&) { *p = std::calloc(1, bytes ? bytes : 1); return *p ? 0 : MGB_ERR_CUDA; }
@@ -98,8 +120,11 @@ inline void dev_free(void *p, Stream&) { std::free(p); }
 inline int h2d(void *d, const void *h, size_t bytes, Stream&) { std::memcpy(d, h, bytes); return 0; }
 inline int d2h(void *h, const void *d, size_t bytes, Stream&) { std::memcpy(h, d, bytes); return 0; }
 inline int dev_zero(void *d, size_t bytes, Stream&) { std::memset(d, 0, bytes); return 0; }
+inline int sync(Stream&) { return 0; }
+inline void record(Stream&, int) {}
+inline float elapsed_ms(Stream&, int, int) { return 0; }
 #else
-struct Stream { cudaStream_t s; };
+struct Stream { cudaStream_t s = nullptr; cudaEvent_t *ev = nullptr; };
 inline int dev_alloc(void **p, size_t bytes, Stream &st) {
     cudaError_t e = cudaMallocAsync(p, bytes ? bytes : 16, st.s);
     if (e != cudaSuccess) { g_err = std::string("cudaMallocAsync: ") + cudaGetErrorString(e); return MGB_ERR_CUDA; }
@@ -121,6 +146,13 @@ inline int dev_zero(void *d, size_t bytes, Stream &st) {
     if (e != cudaSuccess) { g_err = std::string("memset: ") + cudaGetErrorString(e); return MGB_ERR_CUDA; }
     return 0;
 }
+inline int sync(Stream &st) {
+    cudaError_t e = cudaStreamSynchronize(st.s);
+    if (e != cudaSuccess) return fail(MGB_ERR_CUDA, std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e));
+    return 0;
+}
+inline void record(Stream &st, int i) { cudaEventRecord(st.ev[i], st.s); }
+inline float elapsed_ms(Stream &st, int from, int to) { float ms = 0; cudaEventElapsedTime(&ms, st.ev[from], st.ev[to]); return ms; }
 #endif
 
 // Host buffers that receive the packed results. On the device build they are pinned and
@@ -163,23 +195,19 @@ inline void hostbuf_release(HostBuf b) { g_pinned_pool.release(b); }
 // Device working memory of one call. On the device build the buffers belong to a Workspace that the
 // index keeps between calls (slot i = the i-th request of the call): cudaMalloc of GB-sized arenas per
 // call is slow, and stream-ordered pools stall when two streams trade memory back and forth.
+// Every DevBufs takes consecutive slots of one region, and an allocation past the region's end fails, in both builds.
+constexpr int kMaxPasses = 6;          // align_range gives up on a read after six passes
+struct Region { const char *name; size_t base, end; };
+constexpr Region kBatchSlots { "batch", 0, 32 };              // the batch's buffers; the file route's parse
+constexpr Region kArenaSlots { "arena", 32, 33 };             // the align pass's arena
+constexpr Region kPassHeapSlots { "pass heap", 33, 40 };      // record route: the heap, list and counters of a pass
+// text route: every pass keeps its heap on the device until the text is rendered
+inline Region text_heap_slots(int pass) { return { "text heap", 40 + 8 * (size_t)pass, 48 + 8 * (size_t)pass }; }
+constexpr Region kTextSlots { "text", 96, SIZE_MAX };         // text route: the headers and the text
+static_assert(40 + 8 * kMaxPasses <= kTextSlots.base, "the text heaps end below the text region");
+
 #if defined(MGB_HOST_EMU)
 struct Workspace {};
-struct DevBufs {               // frees everything it owns on scope exit
-    Stream &st;
-    std::vector<void*> ptrs;
-    DevBufs(Stream &s, Workspace*, size_t) : st(s) {}
-    ~DevBufs() { for (void *p : ptrs) dev_free(p, st); }
-    template <class T> int alloc(T **p, size_t count) {
-        void *v = nullptr;
-        int rc = dev_alloc(&v, count * sizeof(T), st);
-        if (rc) return rc;
-        ptrs.push_back(v);
-        *p = (T*)v;
-        return 0;
-    }
-    size_t capacity_of_next() const { return 0; }
-};
 #else
 struct Workspace {
     std::vector<void*> ptr;
@@ -217,21 +245,32 @@ struct Workspace {
         return 0;
     }
 };
-struct DevBufs {
+#endif
+struct DevBufs {               // (the emulation build frees what it took on scope exit)
     Stream &st;
     Workspace *ws;
+    Region region;
     size_t slot;
-    DevBufs(Stream &s, Workspace *w, size_t slot_base) : st(s), ws(w), slot(slot_base) {}
+    std::vector<void*> owned;
+    DevBufs(Stream &s, Workspace *w, Region r) : st(s), ws(w), region(r), slot(r.base) {}
+    ~DevBufs() { for (void *p : owned) dev_free(p, st); }
     template <class T> int alloc(T **p, size_t count) {
+        if (slot >= region.end) return fail(MGB_ERR_CUDA, std::string("workspace region '") + region.name + "' is full");
         void *v = nullptr;
-        int rc = ws->get(slot++, count * sizeof(T), &v);
-        if (rc) return rc;
+#if defined(MGB_HOST_EMU)
+        ++slot;
+        if (int rc = dev_alloc(&v, count * sizeof(T), st)) return rc;
+        owned.push_back(v);
+#else
+        if (int rc = ws->get(slot++, count * sizeof(T), &v)) return rc;
+#endif
         *p = (T*)v;
         return 0;
     }
+#if !defined(MGB_HOST_EMU)
     size_t capacity_of_next() const { return slot < ws->cap.size() ? ws->cap[slot] : 0; }
-};
 #endif
+};
 
 } // namespace
 
@@ -300,6 +339,29 @@ struct mgb_results {
     }
     mgb_stats_t stats;
 };
+
+namespace {
+// A workspace of the index held for the duration of a call, with its stream and events. ready() makes the index's
+// device current. The destructor waits for the call's work on the stream before the workspace goes back; that wait is
+// unchecked, so the call's own result and error text stand.
+struct CallWorkspace {
+    const mgb_index_t *ix; Workspace *w; Stream st; bool ready_ = false;
+    explicit CallWorkspace(const mgb_index_t *i) : ix(i), w(i->ws_acquire()) {}
+    ~CallWorkspace() {
+        if (ready_) { const std::string err = g_err; sync(st); g_err = err; }
+        ix->ws_release(w);
+    }
+    int ready() {
+#if !defined(MGB_HOST_EMU)
+        CUDA_TRY(cudaSetDevice(ix->device));
+        if (int rc = w->ready()) return rc;
+        st.s = w->stream; st.ev = w->ev;
+#endif
+        ready_ = true;
+        return MGB_OK;
+    }
+};
+} // namespace
 
 #if !defined(MGB_HOST_EMU)
 // IndexView::pl_word (0.5 bytes per position) and kh_pos (4 bytes per hash slot), the whole-read gate's leaner copies of
@@ -928,8 +990,6 @@ int launch_prepare_exact(const mgb_index_t *index, const PrepExactArgs &a, Strea
 // align passes left in their heaps (format_core.cuh). Independent of the index layout and the graph mode, so compiled
 // in this translation unit only.
 // ---------------------------------------------------------------------------------------
-constexpr int kMaxPasses = 6;          // align_range gives up on a read after six passes
-
 struct TextArgs {
     const char *seqs; const uint64_t *offsets;       // the piece's raw reads
     const char *names; const uint64_t *name_off;     // and their headers
@@ -1040,10 +1100,9 @@ int render_text(const mgb_index_t *index, TextArgs &ta, DevBufs &tb, Stream &st,
         k_text_size<<<grid, 256, 0, st.s>>>(ta);
         k_text_scan<<<1, 1024, 0, st.s>>>(ta.off, ta.n_reads);
         CUDA_TRY(cudaGetLastError());
-        if ((rc = d2h(&total, ta.off + ta.n_reads, 8, st))) return rc;
-        CUDA_TRY(cudaStreamSynchronize(st.s));
     }
 #endif
+    if ((rc = d2h(&total, ta.off + ta.n_reads, 8, st)) || (rc = sync(st))) return rc;
     stats->kernel_launches += 2;
     stats->d2h_bytes += 8;
     *host = hostbuf_acquire(total);
@@ -1069,9 +1128,7 @@ int render_text(const mgb_index_t *index, TextArgs &ta, DevBufs &tb, Stream &st,
         if ((rc = d2h(host->p + lo, ta.out, ta.hi - ta.lo, st))) return rc;
         stats->kernel_launches += 1;
     }
-#if !defined(MGB_HOST_EMU)
-    CUDA_TRY(cudaStreamSynchronize(st.s));
-#endif
+    if ((rc = sync(st))) return rc;
     stats->d2h_bytes += total;
     return 0;
 }
@@ -1140,10 +1197,7 @@ int fastx_parse_dev(const mgb_index_t *index, const char *buf, uint64_t bytes, b
     }
 #endif
     if ((rc = scan_u64(a.tile_nl, a.n_tiles, st, bufs))) return rc;
-    if ((rc = d2h(&n_nl, a.tile_nl + a.n_tiles, 8, st))) return rc;
-#if !defined(MGB_HOST_EMU)
-    CUDA_TRY(cudaStreamSynchronize(st.s));
-#endif
+    if ((rc = d2h(&n_nl, a.tile_nl + a.n_tiles, 8, st)) || (rc = sync(st))) return rc;
     a.n_nl = (uint32_t)n_nl;
     a.n_lines = a.n_nl + (bytes && buf[bytes - 1] != '\n' ? 1 : 0);
     if ((rc = bufs.alloc(&a.nl, (size_t)a.n_nl + 1))) return rc;
@@ -1168,8 +1222,8 @@ int fastx_parse_dev(const mgb_index_t *index, const char *buf, uint64_t bytes, b
     if (a.n_lines) k_fastx_classify<<<lines_grid, 256, 0, st.s>>>(a);
     CUDA_TRY(cudaGetLastError());
     if ((rc = d2h(&sum, a.sum, sizeof(sum), st))) return rc;
-    CUDA_TRY(cudaStreamSynchronize(st.s));
 #endif
+    if ((rc = sync(st))) return rc;
     stats->kernel_launches += 6;
     stats->d2h_bytes += 8 + sizeof(sum);
     if ((sum.flags & kFastxFastaBad) && (sum.flags & kFastxFastqBad)) { out->refused = true; return 0; }
@@ -1224,12 +1278,28 @@ int fastx_parse_dev(const mgb_index_t *index, const char *buf, uint64_t bytes, b
 #endif
     stats->kernel_launches += a.fastq ? 11 : 12;
     if ((rc = d2h(out->offsets.data(), a.offsets, (n_out + 1) * 8, st))) return rc;
-    if ((rc = d2h(out->name_offsets.data(), a.name_offsets, (n_out + 1) * 8, st))) return rc;
-#if !defined(MGB_HOST_EMU)
-    CUDA_TRY(cudaStreamSynchronize(st.s));
-#endif
+    if ((rc = d2h(out->name_offsets.data(), a.name_offsets, (n_out + 1) * 8, st)) || (rc = sync(st))) return rc;
     stats->d2h_bytes += 16 * (n_out + 1);
     return 0;
+}
+
+// k-mer to node ids of every read on `strands` strands: the forward strand's into out_f, the reverse complement's into
+// *out_r (resized to the batch's k-mers); *koff: where each read's k-mers start
+static int map_nodes(const mgb_index_t *index, const char *seqs, const uint64_t *offsets, uint32_t n, uint32_t strands,
+                     uint64_t *out_f, std::vector<uint64_t> *out_r, std::vector<uint64_t> *koff) {
+    CallWorkspace cw(index);
+    if (int rc = cw.ready()) return rc;
+    DevBufs bufs(cw.st, cw.w, kBatchSlots);
+    Batch b; mgb_stats_t stats; std::memset(&stats, 0, sizeof(stats));
+    int rc = upload_batch(index, seqs, offsets, n, strands == 2, cw.st, bufs, &b, koff, &stats);
+    if (!rc) rc = dev_zero(b.nodes_f, (b.total_kmers + 1) * 8, cw.st);
+    if (!rc && strands == 2) rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, cw.st);
+    if (!rc) rc = launch_prepare(index, b, cw.st, index->num_sms);
+    if (!rc) rc = launch_seed(index, b, strands, cw.st, bufs, nullptr);
+    if (!rc) rc = d2h(out_f, b.nodes_f, b.total_kmers * 8, cw.st);
+    if (!rc && strands == 2) { out_r->resize(b.total_kmers + 1); rc = d2h(out_r->data(), b.nodes_r, b.total_kmers * 8, cw.st); }
+    if (!rc) rc = sync(cw.st);
+    return rc;
 }
 
 } // namespace
@@ -1239,110 +1309,35 @@ extern "C" {
 int mgb_map_to_nodes(const mgb_index_t *index, const char *seqs, const uint64_t *offsets,
                      uint32_t n_seqs, uint64_t *out_nodes) {
     if (!index || !seqs || !offsets || !out_nodes) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
-    Stream st;
-    int rc = 0;
-    struct WsGuard { const mgb_index_t *ix; Workspace *w; ~WsGuard() { ix->ws_release(w); } } wsg{ index, index->ws_acquire() };
-#if !defined(MGB_HOST_EMU)
-    CUDA_TRY(cudaSetDevice(index->device));
-    if ((rc = wsg.w->ready())) return rc;
-    st.s = wsg.w->stream;
-#endif
-    {
-        DevBufs bufs(st, wsg.w, 0);
-        Batch b; std::vector<uint64_t> koff; mgb_stats_t stats; std::memset(&stats, 0, sizeof(stats));
-        // PRIMARY graph: CanonicalDBG::map_to_nodes_sequentially (canonical_dbg.cpp:55-146) = both strands mapped in
-        // the stored graph; a k-mer missing on its own strand takes the id of its reverse complement + n
-        const bool primary = index->view.mode == 2;
-        std::vector<uint64_t> rev;
-        rc = upload_batch(index, seqs, offsets, n_seqs, primary, st, bufs, &b, &koff, &stats);
-        if (!rc) rc = dev_zero(b.nodes_f, (b.total_kmers + 1) * 8, st);
-        if (!rc && primary) rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, st);
-        if (!rc) rc = launch_prepare(index, b, st, index->num_sms);
-        if (!rc) rc = launch_seed(index, b, primary ? 2 : 1, st, bufs, nullptr);
-        if (!rc) rc = d2h(out_nodes, b.nodes_f, b.total_kmers * 8, st);
-        if (!rc && primary) { rev.resize(b.total_kmers + 1); rc = d2h(rev.data(), b.nodes_r, b.total_kmers * 8, st); }
-#if !defined(MGB_HOST_EMU)
-        if (!rc) { cudaError_t e = cudaStreamSynchronize(st.s); if (e != cudaSuccess) rc = fail(MGB_ERR_CUDA, cudaGetErrorString(e)); }
-#endif
-        if (!rc && primary) {
-            const uint64_t n = index->view.n;
-            for (uint32_t r = 0; r < n_seqs; ++r) {
-                const uint64_t lo = koff[r], nk = koff[r + 1] - koff[r];
-                for (uint64_t i = 0; i < nk; ++i) {
-                    const uint64_t rv = rev[lo + nk - 1 - i];
-                    if (!out_nodes[lo + i] && rv) out_nodes[lo + i] = rv + n;
-                }
+    // PRIMARY graph: CanonicalDBG::map_to_nodes_sequentially (canonical_dbg.cpp:55-146) = both strands mapped in
+    // the stored graph; a k-mer missing on its own strand takes the id of its reverse complement + n
+    const bool primary = index->view.mode == 2;
+    std::vector<uint64_t> rev, koff;
+    if (int rc = map_nodes(index, seqs, offsets, n_seqs, primary ? 2 : 1, out_nodes, &rev, &koff)) return rc;
+    if (primary) {
+        const uint64_t n = index->view.n;
+        for (uint32_t r = 0; r < n_seqs; ++r) {
+            const uint64_t lo = koff[r], nk = koff[r + 1] - koff[r];
+            for (uint64_t i = 0; i < nk; ++i) {
+                const uint64_t rv = rev[lo + nk - 1 - i];
+                if (!out_nodes[lo + i] && rv) out_nodes[lo + i] = rv + n;
             }
         }
     }
-#if !defined(MGB_HOST_EMU)
-    cudaStreamSynchronize(st.s);
-#endif
-    return rc;
+    return MGB_OK;
 }
 
 int mgb_map_to_nodes_strands(const mgb_index_t *index, const char *seqs, const uint64_t *offsets,
                              uint32_t n_seqs, uint64_t *out_fwd, uint64_t *out_rc) {
     if (!index || !seqs || !offsets || !out_fwd || !out_rc) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
     if (!index->at.has_complement) return fail(MGB_ERR_BAD_CONFIG, "a reverse-complement strand needs a DNA graph");
-    Stream st;
-    int rc = 0;
-    struct WsGuard { const mgb_index_t *ix; Workspace *w; ~WsGuard() { ix->ws_release(w); } } wsg{ index, index->ws_acquire() };
-#if !defined(MGB_HOST_EMU)
-    CUDA_TRY(cudaSetDevice(index->device));
-    if ((rc = wsg.w->ready())) return rc;
-    st.s = wsg.w->stream;
-#endif
-    {
-        DevBufs bufs(st, wsg.w, 0);
-        Batch b; std::vector<uint64_t> koff; mgb_stats_t stats; std::memset(&stats, 0, sizeof(stats));
-        rc = upload_batch(index, seqs, offsets, n_seqs, true, st, bufs, &b, &koff, &stats);
-        if (!rc) rc = dev_zero(b.nodes_f, (b.total_kmers + 1) * 8, st);
-        if (!rc) rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, st);
-        if (!rc) rc = launch_prepare(index, b, st, index->num_sms);
-        if (!rc) rc = launch_seed(index, b, 2, st, bufs, nullptr);
-        if (!rc) rc = d2h(out_fwd, b.nodes_f, b.total_kmers * 8, st);
-        if (!rc) rc = d2h(out_rc, b.nodes_r, b.total_kmers * 8, st);
-#if !defined(MGB_HOST_EMU)
-        if (!rc) { cudaError_t e = cudaStreamSynchronize(st.s); if (e != cudaSuccess) rc = fail(MGB_ERR_CUDA, cudaGetErrorString(e)); }
-#endif
-    }
-#if !defined(MGB_HOST_EMU)
-    cudaStreamSynchronize(st.s);
-#endif
-    return rc;
+    std::vector<uint64_t> rev, koff;
+    if (int rc = map_nodes(index, seqs, offsets, n_seqs, 2, out_fwd, &rev, &koff)) return rc;
+    std::memcpy(out_rc, rev.data(), 8 * koff[n_seqs]);
+    return MGB_OK;
 }
 
 } // extern "C"
-
-// One contiguous range of reads [lo, lo + n) of a batch, processed start to finish on its own
-// stream: upload, prepare + seed, align passes, download, materialisation. Pieces of one batch are
-// independent (IDBGAligner::align_batch treats every query separately, dbg_aligner.cpp:251-355), so
-// the download and unpacking of one piece overlap the kernels of the next.
-struct Piece {
-    uint32_t lo = 0, n_reads = 0;
-    // views into the arrays of the enclosing mgb_results: entries of reads [lo, lo + n_reads), and a
-    // region of n_reads * num_alternative_paths records that receives n_alns of them (piece-local
-    // indices in `first`)
-    uint64_t *first = nullptr;
-    uint32_t *count = nullptr;
-    mgb_alignment_t *alns = nullptr;
-    uint64_t n_alns = 0;
-    std::vector<HostBuf> heaps;
-    std::vector<uint64_t> heap_bytes;
-    uint64_t *src_off = nullptr; uint32_t *src_heap = nullptr;   // views into the enclosing mgb_results
-    // text route (mgb_align_batch_text): format (0: records), the batch's headers, and the piece's text
-    int text_format = 0;
-    int32_t min_path_score = 0;
-    const char *names = nullptr; const uint64_t *name_offsets = nullptr;
-    bool dev_input = false;          // reads and headers are device memory (the file route), offsets host memory
-    HostBuf text;
-    uint64_t text_bytes = 0;
-    mgb_stats_t stats;
-    int rc = 0;
-    std::string err;
-    ~Piece() { for (HostBuf b : heaps) hostbuf_release(b); if (text.p) hostbuf_release(text); }
-};
 
 // MGB_DEBUG, when k_prepare_exact ran and at most 8 reads reach k_align on pass 0: one line per such read with what
 // turned it down at each whole-read gate, read back from the device. exact_path_strand (kernels.cuh, conditions 1-4):
@@ -1355,10 +1350,7 @@ static void debug_left_over(const IndexView &ix, const PrepExactArgs &pa, const 
                             const uint8_t *summary, const uint32_t *d_rest, uint32_t n, uint32_t lo, uint32_t n_reads,
                             Stream &st) {
     std::vector<uint32_t> rest(n);
-    if (d2h(rest.data(), d_rest, 4ull * n, st)) return;
-#if !defined(MGB_HOST_EMU)
-    if (cudaStreamSynchronize(st.s) != cudaSuccess) return;
-#endif
+    if (d2h(rest.data(), d_rest, 4ull * n, st) || sync(st)) return;
     const int k = (int)ix.k;
     for (uint32_t r : rest) {
         const char *raw = seqs + offsets[r];
@@ -1372,9 +1364,7 @@ static void debug_left_over(const IndexView &ix, const PrepExactArgs &pa, const 
             d2h(&n0[0], b.nodes_f + koff[r], 8, st);
             d2h(&n0[1], b.nodes_r + koff[r], 8, st);
         }
-#if !defined(MGB_HOST_EMU)
-        cudaStreamSynchronize(st.s);
-#endif
+        sync(st);
         const int s = (n0[0] != 0) == (n0[1] != 0) ? -1 : n0[0] ? 0 : 1;
         // the primary strand's characters, upper case (N: not A/C/G/T); Σ diag over them
         std::string q(L > 0 ? L : 0, 'N');
@@ -1390,9 +1380,7 @@ static void debug_left_over(const IndexView &ix, const PrepExactArgs &pa, const 
                 path = "probe";
             } else {
                 if (ix.pl_n) d2h(&p, ix.pl_pos + n0[s], 4, st);
-#if !defined(MGB_HOST_EMU)
-                cudaStreamSynchronize(st.s);
-#endif
+                sync(st);
                 if (p == kPlNone) {
                     path = "no path position";
                 } else {
@@ -1402,9 +1390,7 @@ static void debug_left_over(const IndexView &ix, const PrepExactArgs &pa, const 
                     d2h(sw.data(), ix.pl_stop + w0, 4ull * sw.size(), st);
                     d2h(rw.data(), ix.pl_rc + w0, 4ull * rw.size(), st);
                     d2h(tw.data(), ix.pl_text + w0, 8ull * tw.size(), st);
-#if !defined(MGB_HOST_EMU)
-                    cudaStreamSynchronize(st.s);
-#endif
+                    sync(st);
                     int stop = -1, rcb = -1, bad = -1, diff = -1;
                     for (int t = nk - 1; t >= 0; --t) {
                         const uint32_t x = p + (uint32_t)t - (w0 << 5);
@@ -1433,487 +1419,587 @@ static void debug_left_over(const IndexView &ix, const PrepExactArgs &pa, const 
     }
 }
 
-static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const char *all_seqs,
-                       const uint64_t *all_offsets, uint32_t lo, uint32_t n_reads, Piece *res) {
-    // MGB_DEBUG=1: wall-clock split of the call on stderr
-    const bool dbg_time = std::getenv("MGB_DEBUG") != nullptr;
-    auto t_last = std::chrono::steady_clock::now();
-    auto tick = [&](const char *what) {
-        if (!dbg_time) return;
-        auto now = std::chrono::steady_clock::now();
+// What is the same for every piece of one mgb_align_batch / mgb_align_batch_text call
+struct Call {
+    const mgb_index_t *index;
+    const DevConfig &dcfg;
+    const char *seqs; const uint64_t *offsets;          // the batch's reads
+    const char *names; const uint64_t *name_offsets;    // text route: their headers
+    int text_format;                                    // 0: records; MGB_TEXT_TSV / MGB_TEXT_JSON
+    int32_t min_path_score;
+    bool dev_input;          // reads and headers are device memory (the file route), offsets host memory
+};
+
+// One contiguous range of reads [lo, lo + n) of a batch, processed start to finish on its own
+// stream: upload, prepare + seed, align passes, download, materialisation. Pieces of one batch are
+// independent (IDBGAligner::align_batch treats every query separately, dbg_aligner.cpp:251-355), so
+// the download and unpacking of one piece overlap the kernels of the next.
+struct Piece {
+    uint32_t lo = 0, n_reads = 0;
+    // views into the arrays of the enclosing mgb_results: entries of reads [lo, lo + n_reads), and a
+    // region of n_reads * num_alternative_paths records that receives n_alns of them (piece-local
+    // indices in `first`)
+    uint64_t *first = nullptr;
+    uint32_t *count = nullptr;
+    mgb_alignment_t *alns = nullptr;
+    uint64_t n_alns = 0;
+    std::vector<HostBuf> heaps;
+    std::vector<uint64_t> heap_bytes;
+    uint64_t *src_off = nullptr; uint32_t *src_heap = nullptr;   // views into the enclosing mgb_results
+    HostBuf text;                    // text route: the piece's text
+    uint64_t text_bytes = 0;
+    mgb_stats_t stats;
+    int rc = 0; std::string err;
+    ~Piece() { for (HostBuf b : heaps) hostbuf_release(b); if (text.p) hostbuf_release(text); }
+};
+
+// MGB_DEBUG=1: wall-clock split of a piece on stderr
+struct Ticks {
+    bool on; uint32_t lo, n_reads;
+    std::chrono::steady_clock::time_point last = std::chrono::steady_clock::now();
+    void operator()(const char *what) {
+        if (!on) return;
+        const auto now = std::chrono::steady_clock::now();
         std::fprintf(stderr, "[mgb] reads %u+%u %-28s %8.2f ms\n", lo, n_reads, what,
-                     std::chrono::duration<double, std::milli>(now - t_last).count());
-        t_last = now;
-    };
-    int rc = 0;
+                     std::chrono::duration<double, std::milli>(now - last).count());
+        last = now;
+    }
+};
+
+// offsets all[lo .. lo + n] relative to base: in place when base is 0, else rebased into *local
+static const uint64_t *rebase_offsets(const uint64_t *all, uint32_t lo, uint32_t n, uint64_t base,
+                                      std::vector<uint64_t> *local) {
+    if (!base) return all + lo;
+    local->resize((size_t)n + 1);
+    for (uint32_t r = 0; r <= n; ++r) (*local)[r] = all[lo + r] - base;
+    return local->data();
+}
+
+// the packed records of one read (OutAln | node ids unless no_nodes | CIGAR | sequence) as `count` mgb_alignment_t
+static void unpack_records(const char *p, uint32_t count, bool no_nodes, uint32_t read_index, mgb_alignment_t *dst) {
+    for (uint32_t i = 0; i < count; ++i) {
+        const OutAln *o = (const OutAln*)p;
+        mgb_alignment_t al;
+        std::memset(&al, 0, sizeof(al));
+        al.read_index = read_index; al.orientation = (uint8_t)o->orientation; al.score = o->score;
+        al.offset = o->offset; al.query_begin = o->query_begin; al.query_len = o->query_len;
+        al.num_nodes = o->n_nodes; al.sequence_len = o->seq_len; al.num_cigar_ops = o->n_cigar;
+        p += sizeof(OutAln);
+        if (no_nodes) al.nodes = nullptr;
+        else { al.nodes = (const uint64_t*)p; p += 8ull * o->n_nodes; }
+        al.cigar = (const uint32_t*)p; p += (4ull * o->n_cigar + 7) & ~7ull;
+        al.sequence = p; p += ((uint64_t)o->seq_len + 7) & ~7ull;
+        dst[i] = al;
+    }
+}
+
+// output heap of a pass over n reads: generous first guess, doubled on retry passes (MGB_TEST_HEAP0: test knob,
+// pass 0's capacity in bytes)
+static uint64_t heap_cap_of(const Batch &b, const DevConfig &dcfg, uint32_t k, uint64_t n, uint32_t scale) {
+    const uint64_t per_read = sizeof(OutAln) + 9ull * (b.L_max + 64 + k) + 4ull * 64;
+    uint64_t cap = n * per_read * dcfg.num_alternative_paths * scale + 4096;
+    if (const char *e = std::getenv("MGB_TEST_HEAP0")) if (scale == 1) cap = std::min<uint64_t>(cap, std::atoll(e));
+    return cap;
+}
+
+// longest read with a whole-read exact answer: k_align's own exit needed both strands staged on chip
+// (L + 1 <= lq) and room for L characters and L - k + 1 nodes in an alignment slot
+static uint32_t exact_max_len(const Caps &caps, uint32_t k, int lq) {
+    const uint64_t max_len = std::min<uint64_t>({ lq > 0 ? (uint64_t)lq - 1 : 0, caps.aln_seq,
+                                                 (uint64_t)caps.aln_nodes + k - 1 });
+    return caps.aln_cigar >= 1 ? (uint32_t)max_len : 0;
+}
+
+// the configuration part of the whole-read gate (kernels.cuh ExactArgs), over the batch's arrays
+static void exact_args(const Batch &b, const DevConfig &dcfg, uint32_t k, const Caps &caps, int lq,
+                       const uint8_t *summary, ReadHdr *hdr, ExactArgs *ea) {
+    std::memset(ea, 0, sizeof(*ea));
+    ea->k = k;
+    ea->end_bonus = dcfg.left_end_bonus + dcfg.right_end_bonus;
+    ea->min_score = std::max({ 0, (int)dcfg.min_cell_score, (int)dcfg.min_path_score });
+    ea->max_len = exact_max_len(caps, k, lq);
+    ea->result_nodes = dcfg.result_nodes;
+    std::memcpy(ea->diag, dcfg.diag, sizeof(ea->diag));
+    ea->qf = b.qf; ea->qr = b.qr; ea->offsets = b.offsets; ea->koff = b.koff;
+    ea->nodes_f = b.nodes_f; ea->nodes_r = b.nodes_r; ea->summary = summary;
+    ea->hdr = hdr;
+}
+
+// sub-k seeding (min_seed_length < k): the independent index_range lookups run GPU-wide ahead of k_align
+static int launch_subk(const mgb_index_t *index, const SubkArgs &sk, uint32_t L_max, Stream &st) {
+    const uint32_t chunks = (L_max + kSubkChunk - 1) / kSubkChunk;
+#if defined(MGB_HOST_EMU)
+    (void)index; (void)st;
+    for (uint32_t r = 0; r < sk.n_reads; ++r)
+        for (uint32_t s = 0; s < sk.n_strands; ++s)
+            for (uint32_t c = 0; c < chunks; ++c) subk_item(sk, r, s, c);
+#else
+    // one warp per 32 query positions of a strand, 4 warps per block
+    const uint64_t items = (uint64_t)sk.n_reads * sk.n_strands * ((chunks * kSubkChunk + 31) / 32);
+    const uint64_t blocks = std::min<uint64_t>((items + 3) / 4, (uint64_t)index->num_sms * 16);
+    CUDA_TRY(index->view.wide ? kern_any::launch_subk((unsigned)blocks, st.s, sk, chunks)
+                              : kern_dna::launch_subk((unsigned)blocks, st.s, sk, chunks));
+#endif
+    return 0;
+}
+
+// text route: the piece's headers go up with its reads, and the text's arguments are set
+static int upload_headers(const Call &c, const Batch &b, const char *names, const uint64_t *name_offs, Stream &st,
+                          DevBufs &text_bufs, TextArgs *ta, mgb_stats_t *stats) {
+    const uint32_t n_reads = b.n_reads;
+    const uint64_t name_bytes = name_offs[n_reads];
+    char *d_names = c.dev_input ? const_cast<char*>(names) : nullptr; uint64_t *d_name_off = nullptr;
+    int rc = c.dev_input ? 0 : text_bufs.alloc(&d_names, name_bytes + 64);
+    if (!rc) rc = text_bufs.alloc(&d_name_off, (size_t)n_reads + 1);
+    if (!rc && name_bytes && !c.dev_input) rc = h2d(d_names, names, name_bytes, st);
+    if (!rc) rc = h2d(d_name_off, name_offs, ((size_t)n_reads + 1) * 8, st);
+    stats->h2d_bytes += (c.dev_input ? 0 : name_bytes) + ((size_t)n_reads + 1) * 8;
+    ta->seqs = b.seqs; ta->offsets = b.offsets; ta->names = d_names; ta->name_off = d_name_off;
+    ta->n_reads = n_reads; ta->k = c.index->view.k; ta->json = c.text_format == MGB_TEXT_JSON;
+    ta->result_nodes = c.dcfg.result_nodes; ta->min_path_score = c.min_path_score;
+    return rc;
+}
+
+// What prepare_and_seed leaves for the align passes
+struct Seeded {
+    bool exact_reads = false;        // the configuration allows whole-read exact answers (kernels.cuh ExactArgs)
+    bool prep_exact = false;         // k_prepare_exact ran: pass 0's heap, counters and list are in pa / next0 / rest0
+    bool subk = false;               // sub-k seeding ran (sk)
+    uint8_t *summary = nullptr;      // k_seed_hash's per-read summary
+    ReadHdr *hdr = nullptr;          // per read: status, n_aln, heap offset and stats of the pass that answered it
+    PrepExactArgs pa;
+    // k_align's next read, the reads k_exact_reads leaves, the length of pa.list, k_align's next arena
+    unsigned int *next0 = nullptr; uint32_t *rest0 = nullptr;
+    SubkArgs sk;
+};
+
+// query preparation (k_prepare, or k_prepare_exact with its whole-read answers), exact seeding and sub-k seeding;
+// device events 1 and 2 mark the start and the end of the kernels
+static int prepare_and_seed(const Call &c, const Batch &b, int lq, Stream &st, DevBufs &bufs, Seeded *sd,
+                            mgb_stats_t *stats) {
+    const mgb_index_t *index = c.index; const DevConfig &dcfg = c.dcfg;
+    const uint32_t k = index->view.k, n_reads = b.n_reads;
+    const bool both = dcfg.forward_and_reverse_complement;
+    const bool map_nodes = dcfg.max_seed_length >= k;
+    // The seeding kernel of graphs with the k-mer hash index summarises what it stored per read; without it the
+    // whole-read gate reads the node arrays instead.
+    sd->exact_reads = dcfg.exact_shortcut && both && index->view.mode == 0 && dcfg.min_seed_length == k
+                      && dcfg.max_seed_length == k && !dcfg.seed_complexity_filter && dcfg.min_exact_match <= 1.0;
+    int rc;
+    if (sd->exact_reads && index->view.kh_slots && (rc = bufs.alloc(&sd->summary, (size_t)n_reads + 1))) return rc;
+    if ((rc = dev_zero(b.nodes_f, (b.total_kmers + 1) * 8, st))) return rc;
+    if (both && (rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, st))) return rc;
+    if ((rc = bufs.alloc(&sd->hdr, (size_t)n_reads + 1))) return rc;
+#if defined(MGB_PROBE_NO_WRITES)
+    if ((rc = dev_zero(sd->hdr, ((size_t)n_reads + 1) * sizeof(ReadHdr), st))) return rc;     // k_prepare_exact stores none
+#endif
+    // Whole-read exact answers from the raw reads, in place of k_prepare (kernels.cuh PrepExactArgs), on graphs with
+    // the k-mer hash index and the path layout: the reads left over are prepared, seeded and go on as before. Pass 0's
+    // heap, its counters and the list exist before the kernel runs; pass 0 takes them over.
+    // MGB_TEST_NO_PREPARE_EXACT: test knob, the route off.
+    PrepExactArgs &pa = sd->pa;
+    std::memset(&pa, 0, sizeof(pa));
+    sd->prep_exact = sd->exact_reads && index->view.kh_slots && index->view.pl_n
+                     && exact_max_len(choose_caps(b.L_max, dcfg, k, 1), k, lq) >= k
+                     && !std::getenv("MGB_TEST_NO_PREPARE_EXACT");
+    if (sd->prep_exact) {
+        pa.ix = index->view;
+        pa.prep = PrepArgs { b.seqs, b.offsets, b.n_reads, b.qf, b.qr, b.cf, b.cr, {0} };
+        std::memcpy(pa.prep.code_of, index->at.code_of, sizeof(pa.prep.code_of));
+        exact_args(b, dcfg, k, choose_caps(b.L_max, dcfg, k, 1), lq, sd->summary, sd->hdr, &pa.ex);
+        pa.stage_bytes = prep_stage_bytes(b.L_max);
+        pa.ex.heap_cap = heap_cap_of(b, dcfg, k, n_reads, 1);
+        if ((rc = bufs.alloc(&pa.ex.heap, pa.ex.heap_cap)) || (rc = bufs.alloc(&pa.ex.heap_used, 1))
+            || (rc = bufs.alloc(&sd->next0, 4)) || (rc = bufs.alloc(&pa.list, (size_t)n_reads + 1))
+            || (rc = bufs.alloc(&sd->rest0, (size_t)n_reads + 1)) || (rc = dev_zero(pa.ex.heap_used, 8, st))
+            || (rc = dev_zero(sd->next0, 16, st)))
+            return rc;
+        pa.n_list = sd->next0 + 2;
+#if defined(MGB_PREP_TIMERS) && !defined(MGB_HOST_EMU)
+        if ((rc = bufs.alloc(&pa.phase_out, PREP_N_PHASES)) || (rc = dev_zero(pa.phase_out, 8 * PREP_N_PHASES, st))) return rc;
+#endif
+    }
+    record(st, 1);
+    rc = sd->prep_exact ? launch_prepare_exact(index, pa, st) : launch_prepare(index, b, st, index->num_sms);
+    stats->kernel_launches += 1;
+    if (rc) return rc;
+    if (map_nodes && (rc = launch_seed(index, b, both ? 2 : 1, st, bufs, sd->summary, &stats->kernel_launches,
+                                       sd->prep_exact ? pa.list : nullptr, sd->prep_exact ? pa.n_list : nullptr)))
+        return rc;
+    SubkArgs &sk = sd->sk;
+    std::memset(&sk, 0, sizeof(sk));
+    sd->subk = map_nodes && dcfg.min_seed_length < k && b.total_chars && !std::getenv("MGB_TEST_NOSUBK");
+    if (sd->subk) {
+        sk.ix = index->view; sk.cf = b.cf; sk.cr = b.cr; sk.offsets = b.offsets; sk.koff = b.koff;
+        sk.nodes_f = b.nodes_f; sk.nodes_r = b.nodes_r; sk.n_reads = n_reads; sk.n_strands = both ? 2 : 1;
+        sk.min_seed_length = dcfg.min_seed_length;
+        sk.max_len = dcfg.max_seed_length < k - 1 ? dcfg.max_seed_length : k - 1;
+        const size_t nc = b.total_chars + 64;
+        if ((rc = bufs.alloc(&sk.first_f, nc)) || (rc = bufs.alloc(&sk.last_f, nc)) || (rc = bufs.alloc(&sk.len_f, nc)))
+            return rc;
+        if (both && ((rc = bufs.alloc(&sk.first_r, nc)) || (rc = bufs.alloc(&sk.last_r, nc))
+                     || (rc = bufs.alloc(&sk.len_r, nc))))
+            return rc;
+        if ((rc = launch_subk(index, sk, b.L_max, st))) return rc;
+        stats->kernel_launches += 1;
+    }
+    record(st, 2);
+    return 0;
+}
+
+// The shape of one align pass: the per-read caps, arena and on-chip layout, and how many warps and arenas k_align gets
+struct PassPlan {
+    Caps caps; SmemLayout slay;
+    size_t stride = 0, smem_per_warp = 0;      // arena and shared-memory bytes per warp
+    int blocks_per_sm = 1;
+    uint32_t n_warps = 1, n_arenas = 1;
+};
+
+static int pass_plan(const Call &c, const Batch &b, uint32_t L_pass, uint32_t scale, int lq, uint32_t n_pass,
+                     const DevBufs &arena_bufs, PassPlan *p) {
+    const mgb_index_t *index = c.index; const DevConfig &dcfg = c.dcfg;
+    p->caps = choose_caps(L_pass, dcfg, index->view.k, scale);
+    p->stride = arena_bytes(p->caps);
+    // on-chip working set per warp: the column buffers hold the widest column the x-drop band
+    // allows (choose_caps' estimate; at least 64 cells, the register path of the extender needs 40) of
+    // reads up to 248 bp; wider columns spill to the arena scratch
+    uint64_t band_est = (uint64_t)b.L_max + 9;
+    if (dcfg.gap_ext < 0 && dcfg.xdrop < (1 << 20))
+        band_est = std::min<uint64_t>(band_est, 2ull * (dcfg.xdrop / (-dcfg.gap_ext)) + 16 + 8);
+    int bmax = band_est <= 256 ? std::max(64, (int)((band_est + 31) & ~31ull)) : 256;
+    int hcap = 16;
+    // test knobs: force the spill paths (arena scratch, queue migration)
+    if (const char *e = std::getenv("MGB_TEST_BMAX")) bmax = std::atoi(e);
+    if (const char *e = std::getenv("MGB_TEST_HCAP")) hcap = std::atoi(e);
+    p->smem_per_warp = p->slay.carve(bmax, lq, hcap, (int)dcfg.num_alternative_paths, !index->view.wide);
+#if defined(MGB_HOST_EMU)
+    (void)n_pass; (void)arena_bufs;           // one lane aligns the reads one after the other in one arena
+#else
+    const size_t smem_block = p->smem_per_warp * kern_dna::kWarpsPerBlock;
+    {
+        // driver queries serialise against running work: ask once per shared-memory size
+        static std::mutex occ_mu;
+        static std::map<std::pair<int, size_t>, int> occ_cache;
+        std::lock_guard<std::mutex> lk(occ_mu);
+        const int variant = index->view.wide ? 1 : index->view.mode != 0 ? 2 : 0;    // which k_align
+        auto key = std::make_pair(index->device * 4 + variant, smem_block);
+        auto it = occ_cache.find(key);
+        if (it == occ_cache.end()) {
+            // the shared memory limit is a high-water mark per device and kernel: keep the largest
+            size_t mx = smem_block;
+            for (auto &kv : occ_cache) if (kv.first.first == key.first) mx = std::max(mx, kv.first.second);
+            CUDA_TRY(variant == 1 ? kern_any::align_occupancy(mx, smem_block, &p->blocks_per_sm)
+                   : variant == 2 ? kern_canon::align_occupancy(mx, smem_block, &p->blocks_per_sm)
+                                  : kern_dna::align_occupancy(mx, smem_block, &p->blocks_per_sm));
+            occ_cache[key] = p->blocks_per_sm;
+        } else p->blocks_per_sm = it->second;
+    }
+    if (p->blocks_per_sm < 1) p->blocks_per_sm = 1;
+    const uint64_t wpb = kern_dna::kWarpsPerBlock;        // warps (reads in flight) per block
+    uint64_t n_warps = (uint64_t)index->num_sms * p->blocks_per_sm * wpb;
+    if (n_warps > ((uint64_t)n_pass + wpb - 1) / wpb * wpb) n_warps = ((uint64_t)n_pass + wpb - 1) / wpb * wpb;
+    n_warps = kern_dna::read_path_grid(n_warps / wpb) * wpb;    // (MGB_TEST_MAX_BLOCKS)
+    // one arena per warp that can take a read, and as many as fit in 60 % of the free memory (at least one)
+    uint64_t n_arenas = std::min<uint64_t>(n_warps, n_pass);
+    if (p->stride * n_arenas > arena_bufs.capacity_of_next()) {
+        size_t free_b = 0, total_b = 0;
+        cudaMemGetInfo(&free_b, &total_b);
+        const uint64_t mem_arenas = (uint64_t)(free_b * 0.6 + arena_bufs.capacity_of_next()) / (p->stride ? p->stride : 1);
+        n_arenas = std::max<uint64_t>(1, std::min(n_arenas, mem_arenas));
+        n_warps = std::min(n_warps, (n_arenas + wpb - 1) / wpb * wpb);
+    }
+    p->n_warps = (uint32_t)n_warps; p->n_arenas = (uint32_t)n_arenas;
+#endif
+    return 0;
+}
+
+// k_align over a.read_list (its length a.n_list, or *a.n_list_dev when set); n_align: the reads it gets, for MGB_DEBUG
+static int launch_align(const mgb_index_t *index, const AlignArgs &a, const PassPlan &p, uint32_t n_align, bool dbg,
+                        Stream &st) {
+#if defined(MGB_HOST_EMU)
+    (void)index; (void)n_align; (void)dbg; (void)st;
+    const uint32_t n = a.n_list_dev ? *a.n_list_dev : a.n_list;
+    if (n) init_arena(a, a.arena);
+    std::vector<char> smem_emu(p.smem_per_warp + 64);
+    const WarpMem mem_emu { a.arena, &a.lay };
+    const WarpSmem sm_emu { smem_emu.data(), &a.slay };
+    for (uint32_t t = 0; t < n; ++t) align_read(a, a.read_list[t], mem_emu, sm_emu);
+#else
+    const uint64_t wpb = kern_dna::kWarpsPerBlock;
+    const uint32_t grid = (uint32_t)(std::min<uint64_t>(p.n_warps, ((uint64_t)a.n_list + wpb - 1) / wpb * wpb) / wpb);
+    if (dbg) {         // every pass; per_round: warps launched with an arena, each aligning one read at a time
+        char launched[128] = "";          // (one fprintf: pieces on two host threads print at once)
+        if (a.n_list) std::snprintf(launched, sizeof(launched), "; launch k_align grid=%u block=%d per_round=%llu items=%u",
+                                    grid, kern_dna::kAlignThreads,
+                                    (unsigned long long)std::min<uint64_t>((uint64_t)grid * wpb, p.n_arenas), n_align);
+        std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident), arena %zu bytes per warp, %u arenas%s\n",
+                     p.n_warps, (unsigned long long)index->num_sms * p.blocks_per_sm * wpb, p.stride, p.n_arenas, launched);
+    }
+    const size_t smem_block = p.smem_per_warp * kern_dna::kWarpsPerBlock;
+    if (a.n_list) {
+        CUDA_TRY(index->view.wide ? kern_any::launch_align(grid, smem_block, st.s, a)
+               : index->view.mode != 0 ? kern_canon::launch_align(grid, smem_block, st.s, a)
+                                       : kern_dna::launch_align(grid, smem_block, st.s, a));
+    }
+#endif
+    return 0;
+}
+
+// MGB_DEBUG on pass 0 after k_prepare_exact: how many reads each whole-read stage answered, and why the last few
+// were left over
+static void debug_exact_counts(const Call &c, uint32_t lo, const Batch &b, const std::vector<uint64_t> &koff,
+                               const char *seqs, const uint64_t *offsets, const Seeded &sd, const ExactArgs &ea,
+                               const uint32_t n_rest[2], Stream &st) {
+    const uint32_t n_reads = b.n_reads;
+    std::fprintf(stderr, "[mgb] reads %u+%u k_prepare_exact answered %u, left over %u\n", lo, n_reads,
+                 n_reads - n_rest[1], n_rest[1]);
+    std::fprintf(stderr, "[mgb] reads %u+%u k_exact_reads answered %u, left to k_align %u\n", lo, n_reads,
+                 n_rest[1] - n_rest[0], n_rest[0]);
+    if (n_rest[0] <= 8 && !c.dev_input)
+        debug_left_over(c.index->view, sd.pa, ea, seqs, offsets, koff, b, sd.summary, ea.rest, n_rest[0], lo, n_reads, st);
+#if defined(MGB_PREP_TIMERS) && !defined(MGB_HOST_EMU)
+    unsigned long long ph[PREP_N_PHASES];
+    if (cudaMemcpy(ph, sd.pa.phase_out, sizeof(ph), cudaMemcpyDeviceToHost) != cudaSuccess) return;
+    const double nr = n_reads ? (double)n_reads : 1.0;
+    std::fprintf(stderr, "[mgb] k_prepare_exact cycles/read: stage %.0f keys %.0f lookup %.0f stop_rc %.0f "
+                 "text %.0f alloc %.0f write %.0f left %.0f\n", ph[PREP_STAGE] / nr, ph[PREP_KEYS] / nr,
+                 ph[PREP_LOOKUP] / nr, ph[PREP_STOPRC] / nr, ph[PREP_TEXT] / nr, ph[PREP_ALLOC] / nr,
+                 ph[PREP_WRITE] / nr, ph[PREP_LEFT] / nr);
+#endif
+}
+
+// The align passes of a piece so far
+struct PassState {
+    std::vector<uint32_t> list;      // the pass's reads; empty on pass 0 after k_prepare_exact until its launches are in
+    uint32_t n_pass = 0;
+    std::vector<uint32_t> read_heap; // which pass produced the read's alignments
+    float align_ms = 0, d2h_ms = 0;
+    void all_reads(uint32_t n) { list.resize(n); std::iota(list.begin(), list.end(), 0u); }
+};
+
+// One align pass over ps->list: its buffers (or those pass 0 takes over from k_prepare_exact), k_exact_reads and
+// k_align, the download of the headers (and on the record route the heap), and the classification of the reads. The
+// reads that overflowed their arena become ps->list, the next pass's reads.
+static int run_pass(const Call &c, const Batch &b, const Seeded &sd, const PassPlan &p, int pass, uint32_t scale,
+                    int lq, const char *seqs, const uint64_t *offsets, const std::vector<uint64_t> &koff,
+                    DevBufs &arena_bufs, DevBufs &heap_bufs, ReadHdr *hdr_host, Stream &st, Ticks &tick,
+                    PassState *ps, TextArgs *ta, Piece *res) {
+    const mgb_index_t *index = c.index;
+    const uint32_t k = index->view.k, n_reads = b.n_reads, n_pass = ps->n_pass;
+    const bool text = c.text_format != 0;
+    const bool listed = pass == 0 && sd.prep_exact;      // pass 0 after k_prepare_exact
+    const uint64_t heap_cap = listed ? sd.pa.ex.heap_cap : heap_cap_of(b, c.dcfg, k, n_pass, scale);
+    char *d_arena = nullptr, *d_heap = nullptr; uint32_t *d_list = nullptr, *d_rest = nullptr;
+    unsigned long long *d_used = nullptr; unsigned int *d_next = nullptr;
+    int rc;
+    if ((rc = arena_bufs.alloc(&d_arena, p.stride * p.n_arenas))) return rc;
+    if (listed) {
+        d_heap = sd.pa.ex.heap; d_list = sd.pa.list; d_used = sd.pa.ex.heap_used; d_next = sd.next0; d_rest = sd.rest0;
+    } else {
+        if ((rc = heap_bufs.alloc(&d_heap, heap_cap)) || (rc = heap_bufs.alloc(&d_list, n_pass))
+            || (rc = heap_bufs.alloc(&d_used, 1))
+            || (rc = heap_bufs.alloc(&d_next, 4))        // k_align's next read and arena; the reads k_exact_reads leaves
+            || (sd.exact_reads && (rc = heap_bufs.alloc(&d_rest, n_pass))))
+            return rc;
+    }
+    ta->heap[pass] = d_heap;
+    tick("pass: arena/heap alloc");
+    if (!listed && ((rc = h2d(d_list, ps->list.data(), (size_t)n_pass * 4, st)) || (rc = dev_zero(d_used, 8, st))
+                    || (rc = dev_zero(d_next, 16, st))))
+        return rc;
+    // the read-dependent part of the gate (exact_read_strand); max_len keeps what k_align's own exit required
+    ExactArgs ea;
+    std::memset(&ea, 0, sizeof(ea));
+    if (sd.exact_reads) {
+        exact_args(b, c.dcfg, k, p.caps, lq, sd.summary, sd.hdr, &ea);
+        ea.list = d_list; ea.n_list = n_pass; ea.n_list_dev = listed ? sd.pa.n_list : nullptr;
+        ea.rest = d_rest; ea.n_rest = d_next + 1;
+        ea.heap = d_heap; ea.heap_cap = heap_cap; ea.heap_used = d_used;
+    }
+    const bool run_exact = sd.exact_reads && ea.max_len >= k;
+    AlignArgs a;
+    a.ix = index->view; a.cfg = c.dcfg; a.caps = p.caps; a.lay.carve(p.caps); a.slay = p.slay;
+    a.use_fast = std::getenv("MGB_TEST_NOFAST") ? 0 : 1; a.phase_out = nullptr;
+#if defined(MGB_PHASE_TIMERS) && !defined(MGB_HOST_EMU)
+    unsigned long long *d_phase = nullptr;
+    if ((rc = heap_bufs.alloc(&d_phase, 8)) || (rc = dev_zero(d_phase, 64, st))) return rc;
+    a.phase_out = d_phase;
+#endif
+    const SubkArgs &sk = sd.sk;
+    a.qf = b.qf; a.qr = b.qr; a.cf = b.cf; a.cr = b.cr; a.offsets = b.offsets; a.koff = b.koff;
+    a.nodes_f = b.nodes_f; a.nodes_r = b.nodes_r;
+    a.sub_first_f = sd.subk ? sk.first_f : nullptr; a.sub_last_f = sk.last_f; a.sub_len_f = sd.subk ? sk.len_f : nullptr;
+    a.sub_first_r = sk.first_r; a.sub_last_r = sk.last_r;
+    a.sub_len_r = sd.subk && c.dcfg.forward_and_reverse_complement ? sk.len_r : nullptr;
+    a.read_list = d_list; a.n_list = n_pass; a.n_list_dev = nullptr;
+    a.arena = d_arena; a.arena_stride = p.stride; a.n_arenas = p.n_arenas;
+    a.hdr = sd.hdr; a.heap = d_heap; a.heap_cap = heap_cap; a.heap_used = d_used; a.next = d_next;
+    record(st, 3);
+    // reads k_align gets (after run_exact: known on the host once the pass is done, or at once when read back)
+    uint32_t n_align = a.n_list;
+    bool align_dev = false;         // k_align reads the length of its list from the device
+    if (run_exact) {
+        // k_align takes only the reads left over. On pass 0 it reads their count from the device and the host
+        // launches the grid it sized for the whole list without waiting; retry passes read the count back
+        // and size the grid by it. MGB_DEBUG reads it back on pass 0 too, for its lines.
+        if ((rc = launch_exact_reads(index, ea, st))) return rc;
+        align_dev = pass == 0;
+        uint32_t n_rest[2] = { 0, 0 };          // and after k_prepare_exact, the length of its list
+        if ((!align_dev || tick.on) && ((rc = d2h(n_rest, d_next + 1, listed ? 8 : 4, st)) || (rc = sync(st)))) return rc;
+        if (listed && tick.on) debug_exact_counts(c, res->lo, b, koff, seqs, offsets, sd, ea, n_rest, st);
+        a.read_list = d_rest;
+        if (align_dev) a.n_list_dev = d_next + 1;      // (a.n_list, the whole list's length, bounds it)
+        else a.n_list = n_rest[0];
+        n_align = n_rest[0];
+        res->stats.kernel_launches += 1;
+    }
+    if ((rc = launch_align(index, a, p, n_align, tick.on, st))) return rc;
+    record(st, 4);
+    unsigned long long used = 0;
+    if ((rc = d2h(&used, d_used, 8, st))) return rc;
+    if (align_dev && !tick.on && (rc = d2h(&n_align, d_next + 1, 4, st))) return rc;
+    if ((rc = sync(st))) return rc;
+    ps->align_ms += elapsed_ms(st, 3, 4);
+    record(st, 3);
+    tick("pass: h2d+seed+align kernels");
+    if (n_align) res->stats.kernel_launches += 1;       // (a k_align over an empty list aligns nothing)
+#if defined(MGB_PHASE_TIMERS) && !defined(MGB_HOST_EMU)
+    unsigned long long ph[8];
+    cudaMemcpy(ph, a.phase_out, 64, cudaMemcpyDeviceToHost);
+    std::fprintf(stderr, "[phase cycles/read] setup %.0f seeds %.0f fwd %.0f backtrack %.0f align_total %.0f; columns/read: register path %.1f, general path %.1f (reads %u)\n",
+                 (double)ph[0] / n_align, (double)ph[1] / n_align, (double)ph[2] / n_align,
+                 (double)ph[3] / n_align, (double)ph[4] / n_align, (double)ph[5] / n_align,
+                 (double)ph[6] / n_align, n_align);
+#endif
+    if (used > heap_cap) used = heap_cap;
+    if (text) used = 0;                        // the records stay on the device
+    else {
+        HostBuf heap_host = hostbuf_acquire((size_t)used + 16);
+        tick("pass: host buffer");
+        if (!heap_host.p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
+        res->heaps.push_back(heap_host);
+        res->heap_bytes.push_back(used);
+        if (used && (rc = d2h(heap_host.p, d_heap, used, st))) return rc;
+    }
+    if ((rc = d2h(hdr_host, sd.hdr, (size_t)n_reads * sizeof(ReadHdr), st)) || (rc = sync(st))) return rc;
+    record(st, 4);
+    if ((rc = sync(st))) return rc;
+    ps->d2h_ms += elapsed_ms(st, 3, 4);
+    res->stats.d2h_bytes += used + (size_t)n_reads * sizeof(ReadHdr);
+    tick("pass: d2h");
+    // classify this pass; alignments are materialised in read order after the last pass
+    std::vector<uint32_t> retry;
+    const uint32_t heap_id = text ? (uint32_t)pass : (uint32_t)res->heaps.size() - 1;
+    if (ps->list.size() != n_pass) ps->all_reads(n_reads);
+    for (uint32_t r : ps->list) {
+        const ReadHdr &h = hdr_host[r];
+        if (h.status == MGB_READ_OVERFLOW) { MGB_EMU_HIT(EMU_READ_OVERFLOW); retry.push_back(r); continue; }
+        res->stats.num_seeds += h.stats.num_seeds; res->stats.num_extensions += h.stats.num_extensions;
+        res->stats.num_explored_nodes += h.stats.num_explored_nodes; res->stats.dp_cells += h.stats.dp_cells;
+        res->stats.dp_columns += h.stats.dp_columns;
+        res->count[r] = h.n_aln;
+        res->first[r] = h.heap_off;          // byte offset for now, patched by materialise
+        ps->read_heap[r] = heap_id;
+    }
+    res->stats.num_reads_retried += retry.size();
+    ps->list.swap(retry);
+    ps->n_pass = (uint32_t)ps->list.size();
+    tick("pass: classify");
+    return 0;
+}
+
+// record route: mgb_alignment_t records in read order, from the heaps the passes downloaded
+static void materialise(const Call &c, const std::vector<uint32_t> &read_heap, Piece *res) {
+    const uint32_t n_reads = res->n_reads;
+    std::vector<uint64_t> byte_off(res->first, res->first + n_reads);
+    for (uint32_t r = 0; r < n_reads; ++r) { res->src_off[r] = byte_off[r]; res->src_heap[r] = read_heap[r]; }
+    uint64_t pos = 0;
+    for (uint32_t r = 0; r < n_reads; ++r) { res->first[r] = pos; pos += res->count[r]; }
+    res->n_alns = pos;
+    #pragma omp parallel for schedule(static) num_threads(host_team()) if (n_reads > 20000)
+    for (int64_t r = 0; r < (int64_t)n_reads; ++r)
+        unpack_records(res->heaps[read_heap[r]].p + byte_off[r], res->count[r], c.dcfg.result_nodes != 0,
+                       res->lo + (uint32_t)r, res->alns + res->first[r]);
+}
+
+static int align_range(const Call &c, uint32_t lo, uint32_t n_reads, Piece *res) {
+    const mgb_index_t *index = c.index;
+    Ticks tick { std::getenv("MGB_DEBUG") != nullptr, lo, n_reads };
     std::memset(&res->stats, 0, sizeof(res->stats));
     res->lo = lo; res->n_reads = n_reads;
+    const bool text = c.text_format != 0;
     // offsets relative to the first character of the piece
     // (device-resident reads: the piece starts at the 16-byte word that holds its first character, as the kernels'
     // word reads assume)
-    std::vector<uint64_t> offs_local;
-    const uint64_t *offsets = all_offsets + lo;
-    const uint64_t base = res->dev_input ? all_offsets[lo] & ~15ull : all_offsets[lo];
-    const char *seqs = all_seqs ? all_seqs + base : nullptr;
-    if (all_offsets[lo]) {
-        offs_local.resize((size_t)n_reads + 1);
-        for (uint32_t r = 0; r <= n_reads; ++r) offs_local[r] = all_offsets[lo + r] - base;
-        offsets = offs_local.data();
-    }
-    const bool text = res->text_format != 0;
-    std::vector<uint64_t> name_offs_local;
-    const uint64_t *name_offs = text ? res->name_offsets + lo : nullptr;
-    const char *names = text && res->names ? res->names + res->name_offsets[lo] : nullptr;
-    if (text && res->name_offsets[lo]) {
-        name_offs_local.resize((size_t)n_reads + 1);
-        for (uint32_t r = 0; r <= n_reads; ++r) name_offs_local[r] = res->name_offsets[lo + r] - res->name_offsets[lo];
-        name_offs = name_offs_local.data();
-    }
+    std::vector<uint64_t> offs_local, name_offs_local;
+    const uint64_t base = c.dev_input ? c.offsets[lo] & ~15ull : c.offsets[lo];
+    const uint64_t *offsets = rebase_offsets(c.offsets, lo, n_reads, base, &offs_local);
+    const char *seqs = c.seqs ? c.seqs + base : nullptr;
+    const uint64_t *name_offs = text ? rebase_offsets(c.name_offsets, lo, n_reads, c.name_offsets[lo], &name_offs_local) : nullptr;
+    const char *names = text && c.names ? c.names + c.name_offsets[lo] : nullptr;
 
-    Stream st;
-    struct WsGuard { const mgb_index_t *ix; Workspace *w; ~WsGuard() { ix->ws_release(w); } } wsg{ index, index->ws_acquire() };
-#if !defined(MGB_HOST_EMU)
-    CUDA_TRY(cudaSetDevice(index->device));
-    if ((rc = wsg.w->ready())) return rc;
-    st.s = wsg.w->stream;
-    cudaEvent_t *ev = wsg.w->ev;
-#endif
+    CallWorkspace cw(index);
+    Stream &st = cw.st;
+    int rc = cw.ready();
+    if (rc) return rc;
     HostBuf hdr_buf = hostbuf_acquire(((size_t)n_reads + 1) * sizeof(ReadHdr));
     if (!hdr_buf.p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
-    ReadHdr *hdr_host = (ReadHdr*)hdr_buf.p;
     struct HdrGuard { HostBuf b; ~HdrGuard() { hostbuf_release(b); } } hdr_guard{ hdr_buf };
-    std::vector<uint32_t> read_heap(n_reads, 0);   // which pass produced the read's alignments
-    {
-        DevBufs bufs(st, wsg.w, 0);
-        Batch b; std::vector<uint64_t> koff;
-        const bool both = dcfg.forward_and_reverse_complement;
-        const bool map_nodes = dcfg.max_seed_length >= index->view.k;
-#if !defined(MGB_HOST_EMU)
-        cudaEventRecord(ev[0], st.s);
-#endif
-        tick("setup");
-        rc = upload_batch(index, seqs, offsets, n_reads, both, st, bufs, &b, &koff, &res->stats, res->dev_input);
-        // text route: the headers go up with the reads (workspace slots from 96 on: above every pass's heap, below)
-        DevBufs text_bufs(st, wsg.w, 96);
-        TextArgs ta;
-        std::memset(&ta, 0, sizeof(ta));
-        if (!rc && text) {
-            const uint64_t name_bytes = name_offs[n_reads];
-            char *d_names = res->dev_input ? const_cast<char*>(names) : nullptr; uint64_t *d_name_off = nullptr;
-            if (!rc && !res->dev_input) rc = text_bufs.alloc(&d_names, name_bytes + 64);
-            if (!rc) rc = text_bufs.alloc(&d_name_off, (size_t)n_reads + 1);
-            if (!rc && name_bytes && !res->dev_input) rc = h2d(d_names, names, name_bytes, st);
-            if (!rc) rc = h2d(d_name_off, name_offs, ((size_t)n_reads + 1) * 8, st);
-            res->stats.h2d_bytes += (res->dev_input ? 0 : name_bytes) + ((size_t)n_reads + 1) * 8;
-            ta.seqs = b.seqs; ta.offsets = b.offsets; ta.names = d_names; ta.name_off = d_name_off;
-            ta.n_reads = n_reads; ta.k = index->view.k; ta.json = res->text_format == MGB_TEXT_JSON;
-            ta.result_nodes = dcfg.result_nodes; ta.min_path_score = res->min_path_score;
-        }
-        // per pass: its heap, read list and counters (DevBufs from workspace slot 33 on). The record route downloads the
-        // heap after the pass and reuses the slots; the text route keeps every pass's heap on the device until the text is
-        // rendered (slots 40 + 8 pass).
-        std::deque<DevBufs> pass_keep;
-        tick("upload_batch (host part)");
-        // whole-read exact answers ahead of k_align (kernels.cuh ExactArgs): the configuration part of the gate. The
-        // seeding kernel of graphs with the k-mer hash index summarises what it stored per read; without it the node
-        // arrays are read instead.
-        const uint32_t k = index->view.k;
-        const bool exact_reads = dcfg.exact_shortcut && both && index->view.mode == 0 && dcfg.min_seed_length == k
-                                 && dcfg.max_seed_length == k && !dcfg.seed_complexity_filter && dcfg.min_exact_match <= 1.0;
-        uint8_t *summary = nullptr;
-        if (!rc && exact_reads && index->view.kh_slots) rc = bufs.alloc(&summary, (size_t)n_reads + 1);
-        if (!rc) rc = dev_zero(b.nodes_f, (b.total_kmers + 1) * 8, st);
-        if (!rc && both) rc = dev_zero(b.nodes_r, (b.total_kmers + 1) * 8, st);
-        ReadHdr *d_hdr = nullptr;
-        if (!rc) rc = bufs.alloc(&d_hdr, (size_t)n_reads + 1);
-#if defined(MGB_PROBE_NO_WRITES)
-        if (!rc) rc = dev_zero(d_hdr, ((size_t)n_reads + 1) * sizeof(ReadHdr), st);     // k_prepare_exact stores none
-#endif
-        // query length k_align stages on chip (0: none; MGB_TEST_LQ: test knob that forces the unstaged path)
-        const int lq = b.L_max + 1 <= 512 ? (int)((b.L_max + 1 + 15) & ~15u) : 0;
-        int lq_v = lq;
-        if (const char *e = std::getenv("MGB_TEST_LQ")) lq_v = std::atoi(e);
-        // output heap of a pass over n reads: generous first guess, doubled on retry passes (MGB_TEST_HEAP0: test knob,
-        // pass 0's capacity in bytes)
-        auto heap_cap_of = [&](uint64_t n, uint32_t scale) {
-            const uint64_t per_read = sizeof(OutAln) + 9ull * (b.L_max + 64 + index->view.k) + 4ull * 64;
-            uint64_t cap = n * per_read * dcfg.num_alternative_paths * scale + 4096;
-            if (const char *e = std::getenv("MGB_TEST_HEAP0")) if (scale == 1) cap = std::min<uint64_t>(cap, std::atoll(e));
-            return cap;
-        };
-        // longest read with a whole-read exact answer: k_align's own exit needed both strands staged on chip
-        // (L + 1 <= lq) and room for L characters and L - k + 1 nodes in an alignment slot
-        auto exact_max_len = [&](const Caps &caps) -> uint32_t {
-            const uint64_t max_len = std::min<uint64_t>({ lq_v > 0 ? (uint64_t)lq_v - 1 : 0, caps.aln_seq,
-                                                         (uint64_t)caps.aln_nodes + k - 1 });
-            return caps.aln_cigar >= 1 ? (uint32_t)max_len : 0;
-        };
-        auto exact_args = [&](const Caps &caps, ExactArgs *ea) {
-            std::memset(ea, 0, sizeof(*ea));
-            ea->k = k;
-            ea->end_bonus = dcfg.left_end_bonus + dcfg.right_end_bonus;
-            ea->min_score = std::max({ 0, (int)dcfg.min_cell_score, (int)dcfg.min_path_score });
-            ea->max_len = exact_max_len(caps);
-            ea->result_nodes = dcfg.result_nodes;
-            std::memcpy(ea->diag, dcfg.diag, sizeof(ea->diag));
-            ea->qf = b.qf; ea->qr = b.qr; ea->offsets = b.offsets; ea->koff = b.koff;
-            ea->nodes_f = b.nodes_f; ea->nodes_r = b.nodes_r; ea->summary = summary;
-            ea->hdr = d_hdr;
-        };
-        // Whole-read exact answers from the raw reads, in place of k_prepare (kernels.cuh PrepExactArgs), on graphs with
-        // the k-mer hash index and the path layout: the reads left over are prepared, seeded and go on as before. Pass 0's
-        // heap, its counters and the list exist before the kernel runs; pass 0 below takes them over.
-        // MGB_TEST_NO_PREPARE_EXACT: test knob, the route off.
-        PrepExactArgs pa;
-        std::memset(&pa, 0, sizeof(pa));
-        unsigned int *next0 = nullptr;      // k_align's next read, the reads k_exact_reads leaves, the length of pa.list,
-                                            // k_align's next arena
-        uint32_t *rest0 = nullptr;
-        const bool prep_exact = !rc && exact_reads && index->view.kh_slots && index->view.pl_n
-                                && exact_max_len(choose_caps(b.L_max, dcfg, k, 1)) >= k
-                                && !std::getenv("MGB_TEST_NO_PREPARE_EXACT");
-        if (prep_exact) {
-            pa.ix = index->view;
-            pa.prep = PrepArgs { b.seqs, b.offsets, b.n_reads, b.qf, b.qr, b.cf, b.cr, {0} };
-            std::memcpy(pa.prep.code_of, index->at.code_of, sizeof(pa.prep.code_of));
-            exact_args(choose_caps(b.L_max, dcfg, k, 1), &pa.ex);
-            pa.stage_bytes = prep_stage_bytes(b.L_max);
-            pa.ex.heap_cap = heap_cap_of(n_reads, 1);
-            if (!rc) rc = bufs.alloc(&pa.ex.heap, pa.ex.heap_cap);
-            if (!rc) rc = bufs.alloc(&pa.ex.heap_used, 1);
-            if (!rc) rc = bufs.alloc(&next0, 4);
-            if (!rc) rc = bufs.alloc(&pa.list, (size_t)n_reads + 1);
-            if (!rc) rc = bufs.alloc(&rest0, (size_t)n_reads + 1);
-            if (!rc) rc = dev_zero(pa.ex.heap_used, 8, st);
-            if (!rc) rc = dev_zero(next0, 16, st);
-            pa.n_list = next0 + 2;
-#if defined(MGB_PREP_TIMERS) && !defined(MGB_HOST_EMU)
-            if (!rc) rc = bufs.alloc(&pa.phase_out, PREP_N_PHASES);
-            if (!rc) rc = dev_zero(pa.phase_out, 8 * PREP_N_PHASES, st);
-#endif
-        }
-#if !defined(MGB_HOST_EMU)
-        cudaEventRecord(ev[1], st.s);
-#endif
-        if (!rc) rc = prep_exact ? launch_prepare_exact(index, pa, st) : launch_prepare(index, b, st, index->num_sms);
-        res->stats.kernel_launches += 1;
-        if (!rc && map_nodes)
-            rc = launch_seed(index, b, both ? 2 : 1, st, bufs, summary, &res->stats.kernel_launches,
-                             prep_exact ? pa.list : nullptr, prep_exact ? pa.n_list : nullptr);
-        // sub-k seeding (min_seed_length < k): the independent index_range lookups run GPU-wide first
-        SubkArgs sk;
-        std::memset(&sk, 0, sizeof(sk));
-        const bool subk = !rc && map_nodes && dcfg.min_seed_length < index->view.k && b.total_chars
-                          && !std::getenv("MGB_TEST_NOSUBK");
-        if (subk) {
-            sk.ix = index->view; sk.cf = b.cf; sk.cr = b.cr; sk.offsets = b.offsets; sk.koff = b.koff;
-            sk.nodes_f = b.nodes_f; sk.nodes_r = b.nodes_r; sk.n_reads = n_reads; sk.n_strands = both ? 2 : 1;
-            sk.min_seed_length = dcfg.min_seed_length;
-            sk.max_len = dcfg.max_seed_length < index->view.k - 1 ? dcfg.max_seed_length : index->view.k - 1;
-            const size_t nc = b.total_chars + 64;
-            if (!rc) rc = bufs.alloc(&sk.first_f, nc);
-            if (!rc) rc = bufs.alloc(&sk.last_f, nc);
-            if (!rc) rc = bufs.alloc(&sk.len_f, nc);
-            if (!rc && both) rc = bufs.alloc(&sk.first_r, nc);
-            if (!rc && both) rc = bufs.alloc(&sk.last_r, nc);
-            if (!rc && both) rc = bufs.alloc(&sk.len_r, nc);
-            const uint32_t chunks = (b.L_max + kSubkChunk - 1) / kSubkChunk;
-#if defined(MGB_HOST_EMU)
-            for (uint32_t r = 0; r < n_reads && !rc; ++r)
-                for (uint32_t s2 = 0; s2 < sk.n_strands; ++s2)
-                    for (uint32_t c = 0; c < chunks; ++c) subk_item(sk, r, s2, c);
-#else
-            if (!rc) {
-                // one warp per 32 query positions of a strand, 4 warps per block
-                const uint64_t items = (uint64_t)n_reads * sk.n_strands * ((chunks * kSubkChunk + 31) / 32);
-                const uint64_t blocks = std::min<uint64_t>((items + 3) / 4, (uint64_t)index->num_sms * 16);
-                CUDA_TRY(index->view.wide ? kern_any::launch_subk((unsigned)blocks, st.s, sk, chunks)
-                                          : kern_dna::launch_subk((unsigned)blocks, st.s, sk, chunks));
-            }
-#endif
-            res->stats.kernel_launches += 1;
-        }
-#if !defined(MGB_HOST_EMU)
-        cudaEventRecord(ev[2], st.s);
-#endif
+    DevBufs bufs(st, cw.w, kBatchSlots), text_bufs(st, cw.w, kTextSlots);
+    Batch b; std::vector<uint64_t> koff;
+    record(st, 0);
+    tick("setup");
+    if ((rc = upload_batch(index, seqs, offsets, n_reads, c.dcfg.forward_and_reverse_complement, st, bufs, &b, &koff,
+                           &res->stats, c.dev_input)))
+        return rc;
+    TextArgs ta;
+    std::memset(&ta, 0, sizeof(ta));
+    if (text && (rc = upload_headers(c, b, names, name_offs, st, text_bufs, &ta, &res->stats))) return rc;
+    tick("upload_batch (host part)");
+    // query length k_align stages on chip (0: none; MGB_TEST_LQ: test knob that forces the unstaged path)
+    int lq = b.L_max + 1 <= 512 ? (int)((b.L_max + 1 + 15) & ~15u) : 0;
+    if (const char *e = std::getenv("MGB_TEST_LQ")) lq = std::atoi(e);
+    Seeded sd;
+    if ((rc = prepare_and_seed(c, b, lq, st, bufs, &sd, &res->stats))) return rc;
 
-        // align passes: all reads with scale 1, overflowed reads again with larger arenas
-        // The pass's reads. Pass 0 after k_prepare_exact takes its list from the device and needs the host's copy of all
-        // n_reads only once it is done: filling it first would delay the launches behind it.
-        std::vector<uint32_t> list;
-        auto all_reads = [&] { list.resize(n_reads); for (uint32_t r = 0; r < n_reads; ++r) list[r] = r; };
-        if (!prep_exact) all_reads();
-        uint32_t n_pass = n_reads;
-        uint32_t scale = 1;
-        float align_ms = 0, d2h_ms = 0; (void)align_ms; (void)d2h_ms;
-        for (int pass = 0; !rc && n_pass; ++pass, scale *= 4) {
-            if (pass == 6) { rc = fail(MGB_ERR_OVERFLOW, "a read exceeded the largest per-read work arena"); break; }
-            // the arena fits the longest read of the pass: on a retry pass the reads that overflowed, not the batch
-            uint32_t L_pass = b.L_max;
-            if (pass > 0) {
-                L_pass = 0;
-                for (uint32_t r : list) L_pass = std::max<uint32_t>(L_pass, (uint32_t)(offsets[r + 1] - offsets[r]));
-            }
-            Caps caps = choose_caps(L_pass, dcfg, index->view.k, scale);
-            size_t stride = arena_bytes(caps);
-            // on-chip working set per warp: the column buffers hold the widest column the x-drop band
-            // allows (choose_caps' estimate; at least 64 cells, the register path of the extender needs 40) of
-            // reads up to 248 bp; wider columns spill to the arena scratch
-            uint64_t band_est = (uint64_t)b.L_max + 9;
-            if (dcfg.gap_ext < 0 && dcfg.xdrop < (1 << 20))
-                band_est = std::min<uint64_t>(band_est, 2ull * (dcfg.xdrop / (-dcfg.gap_ext)) + 16 + 8);
-            const int bmax = band_est <= 256 ? std::max(64, (int)((band_est + 31) & ~31ull)) : 256;
-            int hcap = 16;
-            // test knobs: force the spill paths (arena scratch, queue migration)
-            int bmax_v = bmax;
-            if (const char *e = std::getenv("MGB_TEST_BMAX")) bmax_v = std::atoi(e);
-            if (const char *e = std::getenv("MGB_TEST_HCAP")) hcap = std::atoi(e);
-            SmemLayout slay;
-            const size_t smem_per_warp = slay.carve(bmax_v, lq_v, hcap, (int)dcfg.num_alternative_paths, !index->view.wide);
-            DevBufs pass_bufs(st, wsg.w, 32);          // slot 32: the arena
-            DevBufs &heap_bufs = pass_keep.emplace_back(st, wsg.w, text ? 40 + 8 * (size_t)pass : 33);
-#if defined(MGB_HOST_EMU)
-            const uint32_t n_arenas = 1;
-#else
-            int blocks_per_sm = 0;
-            const size_t smem_block = smem_per_warp * kern_dna::kWarpsPerBlock;
-            {
-                // driver queries serialise against running work: ask once per shared-memory size
-                static std::mutex occ_mu;
-                static std::map<std::pair<int, size_t>, int> occ_cache;
-                std::lock_guard<std::mutex> lk(occ_mu);
-                const int variant = index->view.wide ? 1 : index->view.mode != 0 ? 2 : 0;    // which k_align
-                auto key = std::make_pair(index->device * 4 + variant, smem_block);
-                auto it = occ_cache.find(key);
-                if (it == occ_cache.end()) {
-                    // the shared memory limit is a high-water mark per device and kernel: keep the largest
-                    size_t mx = smem_block;
-                    for (auto &kv : occ_cache) if (kv.first.first == key.first) mx = std::max(mx, kv.first.second);
-                    CUDA_TRY(variant == 1 ? kern_any::align_occupancy(mx, smem_block, &blocks_per_sm)
-                           : variant == 2 ? kern_canon::align_occupancy(mx, smem_block, &blocks_per_sm)
-                                          : kern_dna::align_occupancy(mx, smem_block, &blocks_per_sm));
-                    occ_cache[key] = blocks_per_sm;
-                } else blocks_per_sm = it->second;
-            }
-            if (blocks_per_sm < 1) blocks_per_sm = 1;
-            const uint64_t wpb = kern_dna::kWarpsPerBlock;        // warps (reads in flight) per block
-            uint64_t n_warps64 = (uint64_t)index->num_sms * blocks_per_sm * wpb;
-            if (n_warps64 > ((uint64_t)n_pass + wpb - 1) / wpb * wpb) n_warps64 = ((uint64_t)n_pass + wpb - 1) / wpb * wpb;
-            n_warps64 = kern_dna::read_path_grid(n_warps64 / wpb) * wpb;    // (MGB_TEST_MAX_BLOCKS)
-            // one arena per warp that can take a read, and as many as fit in 60 % of the free memory (at least one)
-            uint64_t n_arenas64 = std::min<uint64_t>(n_warps64, n_pass);
-            if (stride * n_arenas64 > pass_bufs.capacity_of_next()) {
-                size_t free_b = 0, total_b = 0;
-                cudaMemGetInfo(&free_b, &total_b);
-                const uint64_t mem_arenas = (uint64_t)(free_b * 0.6 + pass_bufs.capacity_of_next()) / (stride ? stride : 1);
-                n_arenas64 = std::max<uint64_t>(1, std::min(n_arenas64, mem_arenas));
-                n_warps64 = std::min(n_warps64, (n_arenas64 + wpb - 1) / wpb * wpb);
-            }
-            uint32_t n_warps = (uint32_t)n_warps64, n_arenas = (uint32_t)n_arenas64;
-#endif
-            // pass 0 after k_prepare_exact: its heap, counters and list of reads left over are in place already
-            const bool listed = pass == 0 && prep_exact;
-            const uint64_t heap_cap = listed ? pa.ex.heap_cap : heap_cap_of(n_pass, scale);
-            char *d_arena = nullptr, *d_heap = nullptr; uint32_t *d_list = nullptr, *d_rest = nullptr;
-            unsigned long long *d_used = nullptr; unsigned int *d_next = nullptr;
-            if ((rc = pass_bufs.alloc(&d_arena, stride * n_arenas))) break;
-            if (listed) {
-                d_heap = pa.ex.heap; d_list = pa.list; d_used = pa.ex.heap_used; d_next = next0; d_rest = rest0;
-            } else {
-                if ((rc = heap_bufs.alloc(&d_heap, heap_cap))) break;
-                if ((rc = heap_bufs.alloc(&d_list, n_pass))) break;
-                if ((rc = heap_bufs.alloc(&d_used, 1))) break;
-                if ((rc = heap_bufs.alloc(&d_next, 4))) break;    // k_align's next read and arena; the reads k_exact_reads leaves
-                if (exact_reads && (rc = heap_bufs.alloc(&d_rest, n_pass))) break;
-            }
-            ta.heap[pass] = d_heap;
-            tick("pass: arena/heap alloc");
-            if (!listed) {
-                if ((rc = h2d(d_list, list.data(), (size_t)n_pass * 4, st))) break;
-                if ((rc = dev_zero(d_used, 8, st))) break;
-                if ((rc = dev_zero(d_next, 16, st))) break;
-            }
-            // the read-dependent part of the gate (exact_read_strand); max_len keeps what k_align's own exit required
-            ExactArgs ea;
-            std::memset(&ea, 0, sizeof(ea));
-            if (exact_reads) {
-                exact_args(caps, &ea);
-                ea.list = d_list; ea.n_list = n_pass; ea.n_list_dev = listed ? pa.n_list : nullptr;
-                ea.rest = d_rest; ea.n_rest = d_next + 1;
-                ea.heap = d_heap; ea.heap_cap = heap_cap; ea.heap_used = d_used;
-            }
-            const bool run_exact = exact_reads && ea.max_len >= k;
-            AlignArgs a;
-            a.ix = index->view; a.cfg = dcfg; a.caps = caps; a.lay.carve(caps); a.slay = slay;
-            a.use_fast = std::getenv("MGB_TEST_NOFAST") ? 0 : 1;
-            a.phase_out = nullptr;
-#if defined(MGB_PHASE_TIMERS) && !defined(MGB_HOST_EMU)
-            unsigned long long *d_phase = nullptr;
-            if ((rc = heap_bufs.alloc(&d_phase, 8))) break;
-            if ((rc = dev_zero(d_phase, 64, st))) break;
-            a.phase_out = d_phase;
-#endif
-            a.qf = b.qf; a.qr = b.qr; a.cf = b.cf; a.cr = b.cr; a.offsets = b.offsets; a.koff = b.koff;
-            a.nodes_f = b.nodes_f; a.nodes_r = b.nodes_r;
-            a.sub_first_f = subk ? sk.first_f : nullptr; a.sub_last_f = sk.last_f; a.sub_len_f = subk ? sk.len_f : nullptr;
-            a.sub_first_r = sk.first_r; a.sub_last_r = sk.last_r; a.sub_len_r = subk && both ? sk.len_r : nullptr;
-            a.read_list = d_list; a.n_list = n_pass; a.n_list_dev = nullptr;
-            a.arena = d_arena; a.arena_stride = stride; a.n_arenas = n_arenas;
-            a.hdr = d_hdr; a.heap = d_heap; a.heap_cap = heap_cap; a.heap_used = d_used; a.next = d_next;
-            unsigned long long used = 0;
-#if !defined(MGB_HOST_EMU)
-            cudaEventRecord(ev[3], st.s);
-#endif
-            // reads k_align gets (after run_exact: known on the host once the pass is done, or at once when read back)
-            uint32_t n_align = a.n_list;
-            bool align_dev = false;         // k_align reads the length of its list from the device
-            if (run_exact) {
-                // k_align takes only the reads left over. On pass 0 it reads their count from the device and the host
-                // launches the grid it sized for the whole list without waiting; retry passes read the count back
-                // and size the grid by it. MGB_DEBUG reads it back on pass 0 too, for its lines.
-                if ((rc = launch_exact_reads(index, ea, st))) break;
-#if !defined(MGB_HOST_EMU)
-                align_dev = pass == 0;
-#endif
-                uint32_t n_rest[2] = { 0, 0 };          // and after k_prepare_exact, the length of its list
-                if (!align_dev || dbg_time) {
-                    if ((rc = d2h(n_rest, d_next + 1, listed ? 8 : 4, st))) break;
-#if !defined(MGB_HOST_EMU)
-                    CUDA_TRY(cudaStreamSynchronize(st.s));
-#endif
-                }
-                if (listed && dbg_time) {
-                    std::fprintf(stderr, "[mgb] reads %u+%u k_prepare_exact answered %u, left over %u\n", lo, n_reads,
-                                 n_reads - n_rest[1], n_rest[1]);
-                    std::fprintf(stderr, "[mgb] reads %u+%u k_exact_reads answered %u, left to k_align %u\n", lo, n_reads,
-                                 n_rest[1] - n_rest[0], n_rest[0]);
-                    if (n_rest[0] <= 8 && !res->dev_input)
-                        debug_left_over(index->view, pa, ea, seqs, offsets, koff, b, summary, d_rest, n_rest[0], lo,
-                                        n_reads, st);
-                }
-#if defined(MGB_PREP_TIMERS) && !defined(MGB_HOST_EMU)
-                if (listed && dbg_time) {
-                    unsigned long long ph[PREP_N_PHASES];
-                    CUDA_TRY(cudaMemcpy(ph, pa.phase_out, sizeof(ph), cudaMemcpyDeviceToHost));
-                    const double nr = n_reads ? (double)n_reads : 1.0;
-                    std::fprintf(stderr, "[mgb] k_prepare_exact cycles/read: stage %.0f keys %.0f lookup %.0f stop_rc %.0f "
-                                 "text %.0f alloc %.0f write %.0f left %.0f\n", ph[PREP_STAGE] / nr, ph[PREP_KEYS] / nr,
-                                 ph[PREP_LOOKUP] / nr, ph[PREP_STOPRC] / nr, ph[PREP_TEXT] / nr, ph[PREP_ALLOC] / nr,
-                                 ph[PREP_WRITE] / nr, ph[PREP_LEFT] / nr);
-                }
-#endif
-                a.read_list = d_rest;
-                if (align_dev) a.n_list_dev = d_next + 1;      // (a.n_list, the whole list's length, bounds it)
-                else a.n_list = n_rest[0];
-                n_align = n_rest[0];
-                res->stats.kernel_launches += 1;
-            }
-#if defined(MGB_HOST_EMU)
-            if (a.n_list) init_arena(a, d_arena);
-            std::vector<char> smem_emu(smem_per_warp + 64);
-            const WarpMem mem_emu { d_arena, &a.lay };
-            const WarpSmem sm_emu { smem_emu.data(), &a.slay };
-            for (uint32_t t = 0; t < a.n_list; ++t) align_read(a, a.read_list[t], mem_emu, sm_emu);
-            used = *d_used;
-#else
-            const uint32_t grid = (uint32_t)(std::min<uint64_t>(n_warps, ((uint64_t)a.n_list + wpb - 1) / wpb * wpb) / wpb);
-            if (dbg_time) {         // every pass; per_round: warps launched with an arena, each aligning one read at a time
-                char launched[128] = "";          // (one fprintf: pieces on two host threads print at once)
-                if (a.n_list) std::snprintf(launched, sizeof(launched), "; launch k_align grid=%u block=%d per_round=%llu items=%u",
-                                            grid, kern_dna::kAlignThreads,
-                                            (unsigned long long)std::min<uint64_t>((uint64_t)grid * wpb, n_arenas), n_align);
-                std::fprintf(stderr, "[mgb] k_align grid: %u warps (%llu resident), arena %zu bytes per warp, %u arenas%s\n",
-                             n_warps, (unsigned long long)index->num_sms * blocks_per_sm * wpb, stride, n_arenas, launched);
-            }
-            if (a.n_list) {
-                CUDA_TRY(index->view.wide ? kern_any::launch_align(grid, smem_block, st.s, a)
-                       : index->view.mode != 0 ? kern_canon::launch_align(grid, smem_block, st.s, a)
-                                               : kern_dna::launch_align(grid, smem_block, st.s, a));
-            }
-            cudaEventRecord(ev[4], st.s);
-            if ((rc = d2h(&used, d_used, 8, st))) break;
-            if (align_dev && !dbg_time && (rc = d2h(&n_align, d_next + 1, 4, st))) break;
-            CUDA_TRY(cudaStreamSynchronize(st.s));
-            float ms = 0; cudaEventElapsedTime(&ms, ev[3], ev[4]); align_ms += ms;
-            cudaEventRecord(ev[3], st.s);
-#endif
-            tick("pass: h2d+seed+align kernels");
-            if (n_align) res->stats.kernel_launches += 1;       // (a k_align over an empty list aligns nothing)
-#if defined(MGB_PHASE_TIMERS) && !defined(MGB_HOST_EMU)
-            {
-                unsigned long long ph[8];
-                cudaMemcpy(ph, a.phase_out, 64, cudaMemcpyDeviceToHost);
-                std::fprintf(stderr, "[phase cycles/read] setup %.0f seeds %.0f fwd %.0f backtrack %.0f align_total %.0f; columns/read: register path %.1f, general path %.1f (reads %u)\n",
-                             (double)ph[0] / n_align, (double)ph[1] / n_align, (double)ph[2] / n_align,
-                             (double)ph[3] / n_align, (double)ph[4] / n_align, (double)ph[5] / n_align,
-                             (double)ph[6] / n_align, n_align);
-            }
-#endif
-            if (used > heap_cap) used = heap_cap;
-            if (text) {
-                used = 0;                              // the records stay on the device
-            } else {
-                HostBuf heap_host = hostbuf_acquire((size_t)used + 16);
-                tick("pass: host buffer");
-                if (!heap_host.p) { rc = fail(MGB_ERR_CUDA, "host buffer allocation failed"); break; }
-                res->heaps.push_back(heap_host);
-                res->heap_bytes.push_back(used);
-                if (used && (rc = d2h(heap_host.p, d_heap, used, st))) break;
-            }
-            if ((rc = d2h(hdr_host, d_hdr, (size_t)n_reads * sizeof(ReadHdr), st))) break;
-#if !defined(MGB_HOST_EMU)
-            CUDA_TRY(cudaStreamSynchronize(st.s));
-            cudaEventRecord(ev[4], st.s);
-            CUDA_TRY(cudaStreamSynchronize(st.s));
-            { float ms = 0; cudaEventElapsedTime(&ms, ev[3], ev[4]); d2h_ms += ms; }
-#endif
-            res->stats.d2h_bytes += used + (size_t)n_reads * sizeof(ReadHdr);
-            tick("pass: d2h");
-            // classify this pass; alignments are materialised in read order after the last pass
-            std::vector<uint32_t> retry;
-            const uint32_t heap_id = text ? (uint32_t)pass : (uint32_t)res->heaps.size() - 1;
-            if (list.size() != n_pass) all_reads();
-            for (uint32_t r : list) {
-                const ReadHdr &h = hdr_host[r];
-                if (h.status == MGB_READ_OVERFLOW) { MGB_EMU_HIT(EMU_READ_OVERFLOW); retry.push_back(r); continue; }
-                res->stats.num_seeds += h.stats.num_seeds;
-                res->stats.num_extensions += h.stats.num_extensions;
-                res->stats.num_explored_nodes += h.stats.num_explored_nodes;
-                res->stats.dp_cells += h.stats.dp_cells;
-                res->stats.dp_columns += h.stats.dp_columns;
-                res->count[r] = h.n_aln;
-                res->first[r] = h.heap_off;          // byte offset for now, patched below
-                read_heap[r] = heap_id;
-            }
-            res->stats.num_reads_retried += retry.size();
-            list.swap(retry);
-            n_pass = (uint32_t)list.size();
-            tick("pass: classify");
+    // align passes: all reads with scale 1, overflowed reads again with larger arenas. Pass 0 after k_prepare_exact
+    // takes its list from the device and needs the host's copy of all n_reads only once it is done: filling it first
+    // would delay the launches behind it.
+    PassState ps;
+    ps.read_heap.assign(n_reads, 0);
+    ps.n_pass = n_reads;
+    if (!sd.prep_exact) ps.all_reads(n_reads);
+    std::deque<DevBufs> heap_keep;       // the text route keeps every pass's heap until the text is rendered
+    for (int pass = 0; ps.n_pass; ++pass) {
+        const uint32_t scale = 1u << (2 * pass);
+        if (pass == kMaxPasses) return fail(MGB_ERR_OVERFLOW, "a read exceeded the largest per-read work arena");
+        // the arena fits the longest read of the pass: on a retry pass the reads that overflowed, not the batch
+        uint32_t L_pass = b.L_max;
+        if (pass > 0) {
+            L_pass = 0;
+            for (uint32_t r : ps.list) L_pass = std::max<uint32_t>(L_pass, (uint32_t)(offsets[r + 1] - offsets[r]));
         }
-        // text route: every read's pass goes up (its heap offset is in d_hdr already), then the text comes down
-        if (!rc && text && n_reads) {
-            uint8_t *d_pass = nullptr;
-            std::vector<uint8_t> pass_of(read_heap.begin(), read_heap.end());
-            if (!rc) rc = text_bufs.alloc(&d_pass, n_reads);
-            if (!rc) rc = h2d(d_pass, pass_of.data(), n_reads, st);
-            res->stats.h2d_bytes += n_reads;
-            ta.hdr = d_hdr; ta.pass = d_pass;
-            if (!rc) rc = render_text(index, ta, text_bufs, st, &res->text, &res->text_bytes, &res->stats);
-            tick("text");
-        }
-#if !defined(MGB_HOST_EMU)
-        if (!rc) {
-            float ms = 0;
-            cudaEventElapsedTime(&ms, ev[0], ev[1]); res->stats.h2d_ms = ms;
-            cudaEventElapsedTime(&ms, ev[1], ev[2]); res->stats.seed_kernel_ms = ms;
-            res->stats.align_kernel_ms = align_ms; res->stats.d2h_ms = d2h_ms;
-        }
-#endif
+        DevBufs arena_bufs(st, cw.w, kArenaSlots);
+        DevBufs &heap_bufs = heap_keep.emplace_back(st, cw.w, text ? text_heap_slots(pass) : kPassHeapSlots);
+        PassPlan plan;
+        if ((rc = pass_plan(c, b, L_pass, scale, lq, ps.n_pass, arena_bufs, &plan))
+            || (rc = run_pass(c, b, sd, plan, pass, scale, lq, seqs, offsets, koff, arena_bufs, heap_bufs,
+                              (ReadHdr*)hdr_buf.p, st, tick, &ps, &ta, res)))
+            return rc;
     }
-#if !defined(MGB_HOST_EMU)
-    cudaStreamSynchronize(st.s);
-#endif
-    if (rc) return rc;
+    if (text && n_reads) {      // every read's pass goes up (its heap offset is in sd.hdr already), then the text comes down
+        uint8_t *d_pass = nullptr;
+        const std::vector<uint8_t> pass_of(ps.read_heap.begin(), ps.read_heap.end());
+        rc = text_bufs.alloc(&d_pass, n_reads);
+        if (!rc) rc = h2d(d_pass, pass_of.data(), n_reads, st);
+        res->stats.h2d_bytes += n_reads;
+        ta.hdr = sd.hdr; ta.pass = d_pass;
+        if (rc || (rc = render_text(index, ta, text_bufs, st, &res->text, &res->text_bytes, &res->stats))) return rc;
+        tick("text");
+    }
+    res->stats.h2d_ms = elapsed_ms(st, 0, 1);
+    res->stats.seed_kernel_ms = elapsed_ms(st, 1, 2);
+    res->stats.align_kernel_ms = ps.align_ms; res->stats.d2h_ms = ps.d2h_ms;
     tick("free device buffers");
     if (text) {                                   // counts only: the text route has no records on the host
         uint64_t pos = 0;
@@ -1921,32 +2007,7 @@ static int align_range(const mgb_index_t *index, const DevConfig &dcfg, const ch
         res->n_alns = pos;
         return MGB_OK;
     }
-    // materialise mgb_alignment_t records in read order
-    {
-        std::vector<uint64_t> byte_off(res->first, res->first + n_reads);
-        for (uint32_t r = 0; r < n_reads; ++r) { res->src_off[r] = byte_off[r]; res->src_heap[r] = read_heap[r]; }
-        uint64_t pos = 0;
-        for (uint32_t r = 0; r < n_reads; ++r) { res->first[r] = pos; pos += res->count[r]; }
-        res->n_alns = pos;
-        #pragma omp parallel for schedule(static) num_threads(host_team()) if (n_reads > 20000)
-        for (int64_t r = 0; r < (int64_t)n_reads; ++r) {
-            const char *p = res->heaps[read_heap[r]].p + byte_off[r];
-            for (uint32_t i = 0; i < res->count[r]; ++i) {
-                const OutAln *o = (const OutAln*)p;
-                mgb_alignment_t al;
-                std::memset(&al, 0, sizeof(al));
-                al.read_index = lo + (uint32_t)r; al.orientation = (uint8_t)o->orientation; al.score = o->score;
-                al.offset = o->offset; al.query_begin = o->query_begin; al.query_len = o->query_len;
-                al.num_nodes = o->n_nodes; al.sequence_len = o->seq_len; al.num_cigar_ops = o->n_cigar;
-                p += sizeof(OutAln);
-                if (dcfg.result_nodes) al.nodes = nullptr;
-                else { al.nodes = (const uint64_t*)p; p += 8ull * o->n_nodes; }
-                al.cigar = (const uint32_t*)p; p += (4ull * o->n_cigar + 7) & ~7ull;
-                al.sequence = p; p += ((uint64_t)o->seq_len + 7) & ~7ull;
-                res->alns[res->first[r] + i] = al;
-            }
-        }
-    }
+    materialise(c, ps.read_heap, res);
     tick("materialise");
     return MGB_OK;
 }
@@ -2039,35 +2100,27 @@ static int align_batch(const mgb_index_t *index, const mgb_config_t *config, con
             pieces[i].src_off = res->src_off.data() + piece_lo(i);
             pieces[i].src_heap = res->src_heap.data() + piece_lo(i);
         }
-        pieces[i].text_format = text_format;
-        pieces[i].min_path_score = config->min_path_score;
-        pieces[i].names = names; pieces[i].name_offsets = name_offsets;
-        pieces[i].dev_input = dev_input;
     }
-    if (n_pieces == 1) {
-        rc = align_range(index, dcfg, seqs, offsets, 0, n_reads, &pieces[0]);
-        if (rc) return rc;
-    } else {
-        std::atomic<uint32_t> next{0};
-        std::atomic<bool> failed{false};
-        auto lane = [&]() {
-            for (uint32_t i; !failed.load() && (i = next.fetch_add(1)) < n_pieces; ) {
-                Piece &pc = pieces[i];
-                pc.rc = align_range(index, dcfg, seqs, offsets, piece_lo(i), piece_lo(i + 1) - piece_lo(i), &pc);
-                if (pc.rc) { pc.err = g_err; failed.store(true); }
-            }
-        };
-        // two host threads keep two pieces in flight (MGB_TEST_LANES: measurement knob)
-        uint32_t n_lanes = 2;
-        if (const char *e = std::getenv("MGB_TEST_LANES")) n_lanes = std::max(1, std::atoi(e));
-        n_lanes = std::min(n_lanes, n_pieces);
-        std::vector<std::thread> others;
-        for (uint32_t t = 1; t < n_lanes; ++t) others.emplace_back(lane);
-        lane();
-        for (std::thread &t : others) t.join();
-        for (Piece &pc : pieces)
-            if (pc.rc) return fail(pc.rc, pc.err);
-    }
+    const Call call { index, dcfg, seqs, offsets, names, name_offsets, text_format, config->min_path_score, dev_input };
+    std::atomic<uint32_t> next{0};
+    std::atomic<bool> failed{false};
+    auto lane = [&]() {
+        for (uint32_t i; !failed.load() && (i = next.fetch_add(1)) < n_pieces; ) {
+            Piece &pc = pieces[i];
+            pc.rc = align_range(call, piece_lo(i), piece_lo(i + 1) - piece_lo(i), &pc);
+            if (pc.rc) { pc.err = g_err; failed.store(true); }
+        }
+    };
+    // two host threads keep two pieces in flight (MGB_TEST_LANES: measurement knob)
+    uint32_t n_lanes = 2;
+    if (const char *e = std::getenv("MGB_TEST_LANES")) n_lanes = std::max(1, std::atoi(e));
+    n_lanes = std::min(n_lanes, n_pieces);
+    std::vector<std::thread> others;
+    for (uint32_t t = 1; t < n_lanes; ++t) others.emplace_back(lane);
+    lane();
+    for (std::thread &t : others) t.join();
+    for (Piece &pc : pieces)
+        if (pc.rc) return fail(pc.rc, pc.err);
     if (dbg_time) std::fprintf(stderr, "[mgb] %u pieces done at %.2f ms\n", n_pieces, since());
 
     // close the gaps between the regions (none if every read produced num_alt alignments)
@@ -2091,12 +2144,7 @@ static int align_batch(const mgb_index_t *index, const mgb_config_t *config, con
         for (HostBuf b : pc.heaps) res->heaps.push_back(b);
         for (uint64_t b : pc.heap_bytes) res->heap_bytes.push_back(b);
         pc.heaps.clear();
-        mgb_stats_t &t = res->stats; const mgb_stats_t &u = pc.stats;
-        t.num_seeds += u.num_seeds; t.num_extensions += u.num_extensions;
-        t.num_explored_nodes += u.num_explored_nodes; t.dp_cells += u.dp_cells; t.dp_columns += u.dp_columns;
-        t.num_reads_retried += u.num_reads_retried; t.seed_kernel_ms += u.seed_kernel_ms;
-        t.align_kernel_ms += u.align_kernel_ms; t.h2d_ms += u.h2d_ms; t.d2h_ms += u.d2h_ms;
-        t.h2d_bytes += u.h2d_bytes; t.d2h_bytes += u.d2h_bytes; t.kernel_launches += u.kernel_launches;
+        add_stats(res->stats, pc.stats);
     }
     res->n_alns = total;
     if (text_format) {
@@ -2110,15 +2158,8 @@ static int align_batch(const mgb_index_t *index, const mgb_config_t *config, con
             if (!res->text.p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
             uint64_t at = 0;
             for (Piece &pc : pieces) {
-                const uint64_t n = pc.text_bytes;
-                const int64_t chunks = (int64_t)((n + (1 << 22) - 1) >> 22);
-                char *dst = res->text.p + at; const char *src = pc.text.p;
-                #pragma omp parallel for schedule(static) num_threads(host_team()) if (chunks > 4)
-                for (int64_t c = 0; c < chunks; ++c) {
-                    const uint64_t o = (uint64_t)c << 22;
-                    std::memcpy(dst + o, src + o, std::min<uint64_t>(1ull << 22, n - o));
-                }
-                at += n;
+                parallel_copy(res->text.p + at, pc.text.p, pc.text_bytes);
+                at += pc.text_bytes;
             }
         }
         res->text_bytes = bytes;
@@ -2167,21 +2208,6 @@ static int fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes
     return MGB_OK;
 }
 
-// a workspace of the index held for the duration of a call (the parsed chunk lives in it)
-struct CallWorkspace {
-    const mgb_index_t *ix; Workspace *w; Stream st;
-    explicit CallWorkspace(const mgb_index_t *i) : ix(i), w(i->ws_acquire()) {}
-    ~CallWorkspace() { ix->ws_release(w); }
-    int ready() {
-#if !defined(MGB_HOST_EMU)
-        CUDA_TRY(cudaSetDevice(ix->device));
-        if (int rc = w->ready()) return rc;
-        st.s = w->stream;
-#endif
-        return MGB_OK;
-    }
-};
-
 int mgb_align_fastx_text(const mgb_index_t *index, const mgb_config_t *config, const char *buf, uint64_t bytes,
                          int at_eof, const char *comment_delim, int flags, int format, uint64_t *consumed, int *ended,
                          mgb_results_t **out) {
@@ -2192,7 +2218,7 @@ int mgb_align_fastx_text(const mgb_index_t *index, const mgb_config_t *config, c
     CallWorkspace cw(index);
     int rc = cw.ready();
     if (rc) return rc;
-    DevBufs bufs(cw.st, cw.w, 0);
+    DevBufs bufs(cw.st, cw.w, kBatchSlots);
     FastxDev dev;
     FastxRecords host;
     mgb_stats_t parse;
@@ -2209,8 +2235,7 @@ int mgb_align_fastx_text(const mgb_index_t *index, const mgb_config_t *config, c
                      : align_batch(index, config, dev.seqs, dev.offsets.data(), dev.names, dev.name_offsets.data(), n,
                                    format, out, true);
     if (rc) return rc;
-    mgb_stats_t &t = (*out)->stats;
-    t.h2d_bytes += parse.h2d_bytes; t.d2h_bytes += parse.d2h_bytes; t.kernel_launches += parse.kernel_launches;
+    add_stats((*out)->stats, parse);
     return MGB_OK;
 }
 
@@ -2232,24 +2257,21 @@ int mgb_fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes, i
     };
     if (!device_route) {
         Stream st;
-        DevBufs none(st, nullptr, 0);
+        DevBufs none(st, nullptr, kBatchSlots);
         fastx_parse(index, buf, bytes, at_eof != 0, comment_delim, fwd_rev, false, st, none, &dev, &host, consumed,
                     ended, &parse);
     } else {
         CallWorkspace cw(index);
         int rc = cw.ready();
         if (rc) return rc;
-        DevBufs bufs(cw.st, cw.w, 0);
+        DevBufs bufs(cw.st, cw.w, kBatchSlots);
         if ((rc = fastx_parse(index, buf, bytes, at_eof != 0, comment_delim, fwd_rev, true, cw.st, bufs, &dev, &host,
                               consumed, ended, &parse)))
             return rc;
         if (!dev.refused) {
             if (!fits(dev.offsets, dev.name_offsets)) return fail(MGB_ERR_OVERFLOW, "output arrays too small");
             if ((rc = d2h(seqs, dev.seqs, dev.offsets.back(), cw.st))) return rc;
-            if ((rc = d2h(names, dev.names, dev.name_offsets.back(), cw.st))) return rc;
-#if !defined(MGB_HOST_EMU)
-            CUDA_TRY(cudaStreamSynchronize(cw.st.s));
-#endif
+            if ((rc = d2h(names, dev.names, dev.name_offsets.back(), cw.st)) || (rc = sync(cw.st))) return rc;
             std::memcpy(offsets, dev.offsets.data(), dev.offsets.size() * 8);
             std::memcpy(name_offsets, dev.name_offsets.data(), dev.name_offsets.size() * 8);
             *n_records = dev.offsets.size() - 1;
@@ -2302,14 +2324,8 @@ int mgb_results_export(const mgb_results_t *r, void *dst, uint64_t capacity) {
     std::memcpy(p, r->heap_bytes.data(), 8 * r->heap_bytes.size()); p += 8 * r->heap_bytes.size();
     p = (char*)dst + (((uint64_t)(p - (char*)dst) + 15) & ~15ull);
     for (size_t i = 0; i < r->heaps.size(); ++i) {
-        const uint64_t n = r->heap_bytes[i];
-        const int64_t chunks = (int64_t)((n + (1 << 22) - 1) >> 22);
-        #pragma omp parallel for schedule(static) num_threads(host_team()) if (chunks > 4)
-        for (int64_t c = 0; c < chunks; ++c) {
-            const uint64_t lo = (uint64_t)c << 22, len = std::min<uint64_t>(1ull << 22, n - lo);
-            std::memcpy(p + lo, r->heaps[i].p + lo, len);
-        }
-        p += (n + 15) & ~15ull;
+        parallel_copy(p, r->heaps[i].p, r->heap_bytes[i]);
+        p += (r->heap_bytes[i] + 15) & ~15ull;
     }
     return MGB_OK;
 }
@@ -2341,12 +2357,7 @@ int mgb_results_import(const void *blob, uint64_t bytes, uint32_t read_index_bas
     {
         uint64_t o = 0;
         for (size_t i = 0; i < h.n_heaps; ++i) { heap_base[i] = o; o += (res->heap_bytes[i] + 15) & ~15ull; }
-        const int64_t chunks = (int64_t)((heaps_total + (1 << 22) - 1) >> 22);
-        #pragma omp parallel for schedule(static) num_threads(host_team()) if (chunks > 4)
-        for (int64_t c = 0; c < chunks; ++c) {
-            const uint64_t lo = (uint64_t)c << 22, len = std::min<uint64_t>(1ull << 22, heaps_total - lo);
-            std::memcpy(hb.p + lo, p + lo, len);
-        }
+        parallel_copy(hb.p, p, heaps_total);
     }
     res->alns_buf = hostbuf_acquire((h.n_alns + 1) * sizeof(mgb_alignment_t));
     if (!res->alns_buf.p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
@@ -2358,20 +2369,8 @@ int mgb_results_import(const void *blob, uint64_t bytes, uint32_t read_index_bas
     #pragma omp parallel for schedule(static) num_threads(host_team()) if (n > 20000)
     for (int64_t r = 0; r < (int64_t)n; ++r) {
         if (!res->count[r]) continue;
-        const char *q = hb.p + heap_base[res->src_heap[r]] + res->src_off[r];
-        for (uint32_t i = 0; i < res->count[r]; ++i) {
-            const OutAln *o = (const OutAln*)q;
-            mgb_alignment_t al;
-            std::memset(&al, 0, sizeof(al));
-            al.read_index = read_index_base + (uint32_t)r; al.orientation = (uint8_t)o->orientation; al.score = o->score;
-            al.offset = o->offset; al.query_begin = o->query_begin; al.query_len = o->query_len;
-            al.num_nodes = o->n_nodes; al.sequence_len = o->seq_len; al.num_cigar_ops = o->n_cigar;
-            q += sizeof(OutAln);
-            if (no_nodes) al.nodes = nullptr; else { al.nodes = (const uint64_t*)q; q += 8ull * o->n_nodes; }
-            al.cigar = (const uint32_t*)q; q += (4ull * o->n_cigar + 7) & ~7ull;
-            al.sequence = q; q += ((uint64_t)o->seq_len + 7) & ~7ull;
-            res->alns[res->first[r] + i] = al;
-        }
+        unpack_records(hb.p + heap_base[res->src_heap[r]] + res->src_off[r], res->count[r], no_nodes,
+                       read_index_base + (uint32_t)r, res->alns + res->first[r]);
     }
     // after the import the records live in heap 0 at the rebased offsets
     for (uint32_t r = 0; r < n; ++r) { res->src_off[r] += heap_base[res->src_heap[r]]; res->src_heap[r] = 0; }
