@@ -1533,10 +1533,11 @@ struct ReadAligner {
     // Open-addressing table keyed by node id; the per-node score vector lives in a
     // segment of the conv cell arena, indexed by absolute query position.
     // --------------------------------------------------------------------------------
-    MGB_HD uint32_t hash_node(uint64_t key) const {
+    // first probe of `key`; mask = hash_size - 1
+    MGB_HD static uint32_t hash_node(uint64_t key, uint32_t mask) {
         uint32_t h = (uint32_t)key * 0x9E3779B1u ^ (uint32_t)(key >> 32) * 0x85EBCA77u;
         h ^= h >> 15;
-        return h & (caps.hash_size - 1);
+        return h & mask;
     }
     MGB_HD void conv_clear(int e) {
         StrandCtx &t = cx[e];
@@ -1549,7 +1550,7 @@ struct ReadAligner {
     // *free_at (optional) = the free slot the probe sequence ended on when the key is absent (-1: none)
     MGB_HD int conv_find(const ConvSlot *slots, uint32_t epoch, uint64_t key, ConvSlot *out,
                          bool use_prefetch = false, int *free_at = nullptr) {
-        uint32_t h = hash_node(key);
+        uint32_t h = hash_node(key, caps.hash_size - 1);
         if (free_at) *free_at = -1;
         for (uint32_t probe = 0; probe < caps.hash_size; ++probe) {
             uint32_t p = (h + probe) & (caps.hash_size - 1);
@@ -1559,34 +1560,24 @@ struct ReadAligner {
         }
         return -1;
     }
-    // new entry covering [start, start + size), cells uninitialised
-    // free_at >= 0: the free slot conv_find just ended on for this key (no second probe)
-    MGB_HD int conv_insert(int e, uint64_t key, int start, int size, ConvSlot *out, int free_at = -1) {
+    // new entry covering [start, start + size) in the free slot conv_find ended on for this key, cells uninitialised.
+    // conv_find ends on no free slot only when every slot is taken, which the load test below rejects first
+    MGB_HD bool conv_insert(int e, uint64_t key, int start, int size, ConvSlot *out, int free_at) {
         StrandCtx &t = cx[e];
-        const uint32_t n_entries = t.conv_n, cells_used = t.conv_cells_used, epoch = t.conv_epoch;
-        ConvSlot *slots = t.conv_slots;
-        if (n_entries >= caps.max_conv_entries || 2 * (n_entries + 1) > caps.hash_size) {
-            overflow = true; return -1;
+        const uint32_t n_entries = t.conv_n, cells_used = t.conv_cells_used;
+        if (n_entries >= caps.max_conv_entries || 2 * (n_entries + 1) > caps.hash_size || free_at < 0) {
+            overflow = true; return false;
         }
         int seg_start = imax(0, start - 8);
         int seg_cap = imin(L + 1, start + size + 8) - seg_start;
-        if (cells_used + seg_cap > caps.max_conv_cells) { overflow = true; return -1; }
-        ConvSlot sl; sl.key = key; sl.epoch = epoch; sl.start = start; sl.size = size;
+        if (cells_used + seg_cap > caps.max_conv_cells) { overflow = true; return false; }
+        ConvSlot sl; sl.key = key; sl.epoch = t.conv_epoch; sl.start = start; sl.size = size;
         sl.seg_start = seg_start; sl.seg_cap = seg_cap; sl.seg_off = cells_used;
         t.conv_cells_used = cells_used + seg_cap;
         t.conv_n = n_entries + 1;
-        if (free_at >= 0) { slots[free_at] = sl; *out = sl; return free_at; }
-        uint32_t h = hash_node(key);
-        for (uint32_t probe = 0; probe < caps.hash_size; ++probe) {
-            uint32_t p = (h + probe) & (caps.hash_size - 1);
-            if (slots[p].epoch != epoch) {
-                slots[p] = sl;
-                *out = sl;
-                return (int)p;
-            }
-        }
-        overflow = true;
-        return -1;
+        t.conv_slots[free_at] = sl;
+        *out = sl;
+        return true;
     }
     // make the stored vector cover [new_start, new_end) (superset of the current range),
     // new cells = ninf. Mirrors vec.insert(begin, n, ninf) / resize(n, ninf).
@@ -1616,6 +1607,21 @@ struct ReadAligner {
         return true;
     }
 
+    // The entry of `key`, made to cover [start, start + size) (extender.cpp:113-141, 165-194): a new entry (cells
+    // uninitialised) or the stored one, grown with ninf cells. Returns what was found: CONV_NEW, CONV_DISJOINT (the range
+    // lies before or after the stored one), CONV_OVERLAP, or CONV_FAILED (table or cells full: overflow is set).
+    enum : int { CONV_FAILED, CONV_NEW, CONV_DISJOINT, CONV_OVERLAP };
+    MGB_HD int conv_entry(int e, uint64_t key, int start, int size, bool use_prefetch, ConvSlot *en) {
+        StrandCtx &t = cx[e];
+        int free_at;
+        const int slot = conv_find(t.conv_slots, t.conv_epoch, key, en, use_prefetch, &free_at);
+        if (slot < 0) return conv_insert(e, key, start, size, en, free_at) ? CONV_NEW : CONV_FAILED;
+        const bool disjoint = start + size <= en->start || start >= en->start + en->size;
+        const int ns = imin(start, en->start), ne = imax(start + size, en->start + en->size);
+        if ((ns != en->start || ne != en->start + en->size) && !conv_grow(e, slot, en, ns, ne)) return CONV_FAILED;
+        return disjoint ? CONV_DISJOINT : CONV_OVERLAP;
+    }
+
     // extender.cpp:100-156; sv = S[s_first .. s_first + size) of the column being committed
     MGB_HD score_t update_seed_filter(int e, uint64_t node, int query_start, const score_t *sv, int size) {
         score_t mx = kNinf;
@@ -1623,30 +1629,15 @@ struct ReadAligner {
         mx = wreduce_max(mx);
         if (node == 0) return mx;
         StrandCtx &t = cx[e];
-        uint64_t key = node + ((!MGB_CANONICAL(cfg) && t.rc) ? ix.n : 0);
-        score_t *cells = t.conv_cells;
         ConvSlot en;
-        int free_at;
-        int slot = conv_find(t.conv_slots, t.conv_epoch, key, &en, false, &free_at);
-        if (slot < 0) {
-            slot = conv_insert(e, key, query_start, size, &en, free_at);
-            if (slot < 0) return kNinf;
-            score_t *c = cells + en.seg_off;
-            for (int j = wlane(); j < size; j += kWarp) c[query_start + j - en.seg_start] = sv[j];
+        const int got = conv_entry(e, node + ((!MGB_CANONICAL(cfg) && t.rc) ? ix.n : 0), query_start, size, false, &en);
+        if (got == CONV_FAILED) return kNinf;
+        score_t *v = t.conv_cells + en.seg_off + (query_start - en.seg_start);
+        if (got != CONV_OVERLAP) {                       // new, or before / after the stored range: stored as is
+            for (int j = wlane(); j < size; j += kWarp) v[j] = sv[j];
             wsync();
             return mx;
         }
-        const bool disjoint = query_start + size <= en.start || query_start >= en.start + en.size;
-        int ns = imin(query_start, en.start), ne = imax(query_start + size, en.start + en.size);
-        if (ns != en.start || ne != en.start + en.size)
-            if (!conv_grow(e, slot, &en, ns, ne)) return kNinf;
-        if (disjoint) {                                  // before / after the stored range: stored as is
-            score_t *c = cells + en.seg_off;
-            for (int j = wlane(); j < size; j += kWarp) c[query_start + j - en.seg_start] = sv[j];
-            wsync();
-            return mx;
-        }
-        score_t *v = cells + en.seg_off + (query_start - en.seg_start);
         score_t max_changed = kNinf;
         for (int j = wlane(); j < size; j += kWarp) {
             score_t sj = sv[j];
@@ -1662,10 +1653,11 @@ struct ReadAligner {
         return max_changed;
     }
 
-    // update_seed_filter (extender.cpp:100-156) for a column of the register path: lane l holds S[l * kCPL + c] in
-    // S[c]; the passed range is cells [s_first, size)
-    MGB_HD score_t update_seed_filter_regs(int e, uint64_t node, int query_start, const score_t (&S)[kCPL],
-                                           int s_first, int size) {
+    // The cells [s_first, size) of a register-path column (lane l holds cell l * kCPL + c in S[c]) written into a
+    // convergence entry whose cells v0 points to, indexed by cell: stored as they are (a new entry, or a range before or
+    // after the stored one; returns their maximum), or merged with the stored cells (:143-153; returns the largest cell
+    // that changed, ninf if none).
+    MGB_HD static score_t conv_store_regs(score_t *v0, const score_t (&S)[kCPL], int s_first, int size) {
         const int j0 = wlane() * kCPL;
         score_t mx = kNinf;
 #if MGB_DEVICE_CODE
@@ -1673,76 +1665,65 @@ struct ReadAligner {
 #endif
         for (int c = 0; c < kCPL; ++c) {
             const int j = j0 + c;
-            if (j >= s_first && j < size) mx = imax(mx, S[c]);
+            if (j >= s_first && j < size) { v0[j] = S[c]; mx = imax(mx, S[c]); }
         }
         mx = wreduce_max(mx);
-        if (node == 0) return mx;
-        StrandCtx &t = cx[e];
-        const uint64_t key = node + ((!MGB_CANONICAL(cfg) && t.rc) ? ix.n : 0);
-        ConvSlot en;
-        int free_at;
-        int slot = conv_find(t.conv_slots, t.conv_epoch, key, &en, true, &free_at);
-        const int n_pass = size - s_first;
-        if (slot < 0) {
-            slot = conv_insert(e, key, query_start, n_pass, &en, free_at);
-            if (slot < 0) return kNinf;
-        } else {
-            // the node was met before in this extension (seed columns share the seed's node; cycles; re-convergent
-            // branches). Disjoint from the stored range (before / after it): the values are stored as they are
-            // (:118-131); one conv_grow call site serves all three cases
-            const bool disjoint = query_start + n_pass <= en.start || query_start >= en.start + en.size;
-            const int ns = imin(query_start, en.start), ne = imax(query_start + n_pass, en.start + en.size);
-            if (ns != en.start || ne != en.start + en.size)
-                if (!conv_grow(e, slot, &en, ns, ne)) return kNinf;
-            if (!disjoint) {
-                score_t *v0 = t.conv_cells + en.seg_off + (query_start - s_first - en.seg_start);   // indexed by cell
-                score_t max_changed = kNinf;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-                for (int c = 0; c < kCPL; ++c) {
-                    const int j = j0 + c;
-                    if (j >= s_first && j < size) {
-                        score_t vj = v0[j];
-                        if ((double)S[c] > (double)vj * cfg.rel_score_cutoff) {
-                            vj = imax(vj, S[c]);
-                            v0[j] = vj;
-                            max_changed = imax(max_changed, vj);
-                        }
-                    }
-                }
-                max_changed = wreduce_max(max_changed);
-                wsync();
-                return max_changed;
-            }
-        }
-        score_t *c0 = t.conv_cells + en.seg_off + (query_start - s_first - en.seg_start);           // indexed by cell
+        wsync();
+        return mx;
+    }
+    MGB_HD static score_t conv_merge_regs(score_t *v0, const score_t (&S)[kCPL], int s_first, int size,
+                                          double rel_score_cutoff) {
+        const int j0 = wlane() * kCPL;
+        score_t max_changed = kNinf;
 #if MGB_DEVICE_CODE
 #pragma unroll
 #endif
         for (int c = 0; c < kCPL; ++c) {
             const int j = j0 + c;
-            if (j >= s_first && j < size) c0[j] = S[c];
+            if (j >= s_first && j < size) {
+                score_t vj = v0[j];
+                if ((double)S[c] > (double)vj * rel_score_cutoff) {
+                    vj = imax(vj, S[c]);
+                    v0[j] = vj;
+                    max_changed = imax(max_changed, vj);
+                }
+            }
         }
+        max_changed = wreduce_max(max_changed);
         wsync();
-        return mx;
+        return max_changed;
+    }
+
+    // update_seed_filter (extender.cpp:100-156) for a column of the register path: the passed range is cells
+    // [s_first, size)
+    MGB_HD score_t update_seed_filter_regs(int e, uint64_t node, int query_start, const score_t (&S)[kCPL],
+                                           int s_first, int size) {
+        if (node == 0) {
+            const int j0 = wlane() * kCPL;
+            score_t mx = kNinf;
+#if MGB_DEVICE_CODE
+#pragma unroll
+#endif
+            for (int c = 0; c < kCPL; ++c)
+                if (j0 + c >= s_first && j0 + c < size) mx = imax(mx, S[c]);
+            return wreduce_max(mx);
+        }
+        StrandCtx &t = cx[e];
+        ConvSlot en;
+        const int got = conv_entry(e, node + ((!MGB_CANONICAL(cfg) && t.rc) ? ix.n : 0), query_start, size - s_first,
+                                   true, &en);
+        if (got == CONV_FAILED) return kNinf;
+        score_t *v0 = t.conv_cells + en.seg_off + (query_start - s_first - en.seg_start);   // indexed by cell
+        return got == CONV_OVERLAP ? conv_merge_regs(v0, S, s_first, size, cfg.rel_score_cutoff)
+                                   : conv_store_regs(v0, S, s_first, size);
     }
 
     // extender.cpp:158-207 (every cell of [query_start, query_end) ends up at -ninf)
     MGB_HD void filter_nodes(int e, uint64_t node, int query_start, int query_end) {
         const score_t mscore = -kNinf;
-        int size = query_end - query_start;
         StrandCtx &t = cx[e];
         ConvSlot en;
-        int slot = conv_find(t.conv_slots, t.conv_epoch, node, &en);
-        if (slot < 0) {
-            slot = conv_insert(e, node, query_start, size, &en);
-            if (slot < 0) return;
-        } else {
-            int ns = imin(query_start, en.start), ne = imax(query_end, en.start + en.size);
-            if (ns != en.start || ne != en.start + en.size)
-                if (!conv_grow(e, slot, &en, ns, ne)) return;
-        }
+        if (conv_entry(e, node, query_start, query_end - query_start, false, &en) == CONV_FAILED) return;
         score_t *c = t.conv_cells + en.seg_off;
         for (int p = query_start + wlane(); p < query_end; p += kWarp) c[p - en.seg_start] = mscore;
         wsync();
@@ -1827,6 +1808,45 @@ struct ReadAligner {
         while ((uint32_t)size_final > cap) cap *= 2;
         if ((uint32_t)size_final + 5 > cap) cap = size_final + 5;
         return cap;
+    }
+    // std::vector<DPTColumn>::capacity() once the table holds n columns (table_cap: the capacity before)
+    MGB_HD static uint32_t table_capacity(uint32_t table_cap, uint32_t n) {
+        return n > table_cap ? (table_cap ? 2 * table_cap : 1) : table_cap;
+    }
+    // what a column adds to table_size_bytes (extender.cpp:466-469, 705-711): the DPTColumns the table grew by from
+    // cap_before to cap, and the capacity of the column's S, E and F
+    MGB_HD static uint64_t column_bytes(uint32_t cap_before, uint32_t cap, int size0, int size) {
+        return 136ull * (cap - cap_before) + 3ull * vec_capacity(size0, size) * 4;
+    }
+    // the end of a child column's step (:681-719): false when the column is dropped (pop(table.size() - 1)); otherwise
+    // its bytes are counted, and the x-drop cutoff and best_score follow its maximum
+    MGB_HD static bool accept_column(bool in_seed, score_t max_val, bool has_extension, uint32_t cap_before, uint32_t cap,
+                                     int size0, int size, score_t xdrop, score_t &cutoff, score_t &best_score,
+                                     uint64_t &table_size_bytes) {
+        if (!in_seed && (max_val < cutoff || !has_extension)) return false;
+        table_size_bytes += column_bytes(cap_before, cap, size0, size);
+        if ((int64_t)max_val - cutoff > xdrop) cutoff = max_val - xdrop;
+        best_score = imax(best_score, max_val);
+        return true;
+    }
+    MGB_HD static ColMeta make_col(uint64_t node, uint32_t parent, uint8_t c, int offset, int max_pos, int trim,
+                                   score_t score, uint8_t fmt, int size, uint32_t cells_off) {
+        ColMeta col;
+        col.node = node; col.parent = parent; col.c = c;
+        col.offset = offset; col.max_pos = max_pos; col.trim = trim; col.score = score;
+        col.is_tip = 0; col.started = 0; col.fmt = fmt; col.pad0 = col.pad1 = 0;
+        col.size = size; col.cells_off = cells_off;
+        return col;
+    }
+    // global_xdrop (:525-546), before a column is expanded whose best cell (par_max) is below best_score: the budget
+    // that ends the extension, the table's columns per window character or its bytes; BUDGET_NONE if neither
+    enum : int { BUDGET_NONE, BUDGET_NODES, BUDGET_RAM };
+    MGB_HD static int budget_stop(const DevConfig &cfg, score_t par_max, score_t best_score, uint32_t n_cols, int wlen,
+                                  uint64_t table_size_bytes) {
+        if (par_max >= best_score) return BUDGET_NONE;
+        if ((double)n_cols / wlen >= cfg.max_nodes_per_seq_char) return BUDGET_NODES;
+        if ((double)table_size_bytes / 1000000 > cfg.max_ram_per_alignment) return BUDGET_RAM;
+        return BUDGET_NONE;
     }
 
     // Working buffer of the column being computed: S | E | F with stride `cap`
@@ -2048,6 +2068,67 @@ struct ReadAligner {
         return size;
     }
 
+    // per-column scan (:643-669) of a register column of `size` cells whose cell j is row begin + j: the smallest
+    // finite and the largest score, max_pos (the row of the largest score nearest to the diagonal diag_i, the lowest
+    // such row on ties) and has_extension (in the seed, or a cell reaches ext_cut with the suffix sum psb[j] added).
+    // One reduction over the key (|off-diagonal| << 5) | j finds max_pos; the key fits while L < 2^25.
+    struct ColScan { score_t min, max; int max_pos; bool has_extension; };
+    MGB_HD static ColScan reg_scan(const RegCol &r, int size, int begin, int diag_i, bool in_seed, const int32_t *psb,
+                                   score_t ext_cut) {
+        const int j0 = wlane() * kCPL;
+        score_t mn = 0x7fffffff, bs = INT32_MIN;
+#if MGB_DEVICE_CODE
+#pragma unroll
+#endif
+        for (int c = 0; c < kCPL; ++c) {
+            const bool cell = j0 + c < size;
+            const score_t v = r.S[c];
+            if (cell && v != kNinf) mn = imin(mn, v);
+            if (cell) bs = imax(bs, v);
+        }
+        ColScan sc;
+        sc.min = wreduce_min(mn);
+        sc.max = wreduce_max(bs);
+        int bkey = 0x7fffffff; bool he = false;
+#if MGB_DEVICE_CODE
+#pragma unroll
+#endif
+        for (int c = 0; c < kCPL; ++c) {
+            const int j = j0 + c;
+            const bool cell = j < size;
+            if (cell && r.S[c] == sc.max) bkey = imin(bkey, (iabs(j + begin - diag_i) << 5) | j);
+            if (!in_seed && cell && wadd(r.S[c], psb[j]) >= ext_cut) he = true;
+        }
+        sc.max_pos = (wreduce_min(bkey) & 31) + begin;
+        sc.has_extension = in_seed || wballot(he) != 0;
+        return sc;
+    }
+    // commit of a register column in the compact format, in whole 32-byte sectors: S and the flag bytes to the DP table
+    // at the first multiple of 8 cells from cells_used, S and F to the on-chip child buffer child_S (F at
+    // child_S + 2 * bmax). Returns the cells' offset; cells_used moves past them and the space reserved for F.
+    MGB_HD static uint32_t commit_compact(const RegCol &r, int size, score_t *cells, uint32_t &cells_used, score_t *child_S,
+                                          int bmax) {
+        const int j0 = wlane() * kCPL;
+        const int capr = capr_of(size);
+        const uint32_t off = (cells_used + 7u) & ~7u;
+        cells_used = off + 2 * capr + 8;
+        score_t *dst = cells + off;
+        store_cells(dst, j0, r.S, capr);
+        store_flags(reinterpret_cast<uint8_t*>(dst + capr), j0, r.fl);
+        store_cells(child_S, j0, r.S, 32); store_cells(child_S + 2 * bmax, j0, r.F, 32);
+        return off;
+    }
+    // band of a register column under cutoff: bit j set for the cells j < size with S >= cutoff
+    MGB_HD static uint32_t reg_band(const RegCol &r, int size, score_t cutoff) {
+        const int j0 = wlane() * kCPL;
+        uint32_t bits = 0;
+#if MGB_DEVICE_CODE
+#pragma unroll
+#endif
+        for (int c = 0; c < kCPL; ++c) if (j0 + c < size && r.S[c] >= cutoff) bits |= 1u << c;
+        return kCPL == 32 ? bits : wreduce_or(bits << (j0 & 31));
+    }
+
     // --------------------------------------------------------------------------------
     // DefaultColumnExtender::extend (extender.cpp:412-772) + backtrack (:800-1034)
     //   e      extender (query strand) index, seed in slot `seed_slot`
@@ -2070,8 +2151,9 @@ struct ReadAligner {
         int res0 = -1, res1 = -1;                         // columns resident in sm.buf(0) / sm.buf(1)
         ColMeta last_col = ColMeta(); uint32_t last_idx = 0xffffffffu;  // newest committed column (register copy)
         bool last_band_valid = false; uint32_t last_band_mask = 0; score_t last_band_cutoff = 0;
-        const bool reg_path = use_fast && sm.bmax() >= 40 && (sm.bmax() & 3) == 0;
-        const bool chain_ok = !MGB_WIDE(ix) && !MGB_PRIMARY(ix) && sm.lay->has_prof && L + 1 <= sm.lq() && L < (1 << 25);
+        // (L < 2^25: reg_scan's key holds a cell's distance to the diagonal and its row in one int)
+        const bool reg_path = use_fast && sm.bmax() >= 40 && (sm.bmax() & 3) == 0 && L < (1 << 25);
+        const bool chain_ok = !MGB_WIDE(ix) && !MGB_PRIMARY(ix) && sm.lay->has_prof && L + 1 <= sm.lq();
         uint32_t cells_limit = 0;
         score_t min_cell_score = 0, best_score = 0;
         int heap_n = 0, nn_n = 0;
@@ -2144,16 +2226,12 @@ struct ReadAligner {
                 wsync();
                 int size = extend_ins_end(sc, 1, wlen + 1, cutoff);
                 if (!overflow) {
-                    ColMeta root;
-                    root.node = seed_node0; root.parent = 0xffffffffu; root.c = 0;
-                    root.offset = seed_off_m1; root.max_pos = 0; root.trim = 0; root.score = 0;
-                    root.is_tip = 0; root.started = 0; root.fmt = FMT_FULL; root.pad0 = root.pad1 = 0; root.size = size;
-                    root.cells_off = commit_column(sc, size);
+                    m.cols()[n_cols++] = make_col(seed_node0, 0xffffffffu, 0, seed_off_m1, 0, 0, 0, FMT_FULL, size,
+                                                  commit_column(sc, size));
                     if (sc.on_chip) res0 = 0;
-                    m.cols()[n_cols++] = root;
-                    if (n_cols > cx[e].table_cap) cx[e].table_cap = cx[e].table_cap ? 2 * cx[e].table_cap : 1;
+                    cx[e].table_cap = table_capacity(cx[e].table_cap, n_cols);
                     stats.dp_cells += size; ++stats.dp_columns;
-                    table_size_bytes = 136ull * cx[e].table_cap + 3ull * vec_capacity(1, size) * 4;
+                    table_size_bytes = column_bytes(0, cx[e].table_cap, 1, size);   // the table's whole capacity
                     wsync();
                 }
             }
@@ -2236,18 +2314,10 @@ struct ReadAligner {
                 }
                 cb = pb >= 0 ? 1 - pb : 0;                // buffer for the children
 
-                if (parS[par.max_pos - par.trim] < best_score) {
-                    double node_counter = (double)n_cols;
-                    if (node_counter / wlen >= cfg.max_nodes_per_seq_char) {
-                        MGB_EMU_HIT(EMU_NODES_STOP_GENERAL);
-                        heap_n = 0; nn_n = 0;            // global_xdrop
-                        continue;
-                    }
-                    if ((double)table_size_bytes / 1000000 > cfg.max_ram_per_alignment) {
-                        MGB_EMU_HIT(EMU_RAM_STOP_GENERAL);
-                        heap_n = 0; nn_n = 0;
-                        continue;
-                    }
+                if (const int b = budget_stop(cfg, parS[par.max_pos - par.trim], best_score, n_cols, wlen, table_size_bytes)) {
+                    MGB_EMU_HIT(b == BUDGET_NODES ? EMU_NODES_STOP_GENERAL : EMU_RAM_STOP_GENERAL);
+                    heap_n = 0; nn_n = 0;
+                    continue;
                 }
                 // band within the xdrop cutoff (:549-560)
                 int prev_end;
@@ -2343,7 +2413,7 @@ struct ReadAligner {
                 {   // requests whose latency overlaps the DP below
                     if (!rc && cnode && !MGB_WIDE(ix) && !MGB_PRIMARY(ix)) { pf_node = cnode; pf_adj = load_adj(ix, cnode); }
                     pf_key = cnode + (rc ? ix.n : 0);
-                    pf_slot_idx = hash_node(pf_key);
+                    pf_slot_idx = hash_node(pf_key, caps.hash_size - 1);
                     pf_slot = cx[e].conv_slots[pf_slot_idx];
                 }
                 RegCol r;
@@ -2353,79 +2423,23 @@ struct ReadAligner {
                                             cfg.ge_shift, r);
                 if (size >= 0) {
                     MGB_COUNT(5);
-                    const int j0 = wlane() * kCPL;
                     const uint32_t cap_before = cx[e].table_cap;
-                    if (n_cols + 1 > cap_before) cx[e].table_cap = cap_before ? 2 * cap_before : 1;
+                    cx[e].table_cap = table_capacity(cap_before, n_cols + 1);
                     stats.dp_cells += size; ++stats.dp_columns;
-                    // per-column scan (:643-669)
-                    const score_t extension_cutoff
-                        = (score_t)((double)best_score * cfg.rel_score_cutoff + (double)partial_sum_offset);
-                    score_t mn = 0x7fffffff, bs = INT32_MIN;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-                    for (int c = 0; c < kCPL; ++c) {
-                        const bool cell = j0 + c < size;
-                        const score_t v = r.S[c];
-                        if (cell && v != kNinf) mn = imin(mn, v);
-                        if (cell) bs = imax(bs, v);
-                    }
-                    min_cell_score = imin(min_cell_score, wreduce_min(mn));
-                    const score_t max_val = wreduce_max(bs);
-                    int bd = 0x7fffffff; bool he = false;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-                    for (int c = 0; c < kCPL; ++c) {
-                        const int j = j0 + c;
-                        const bool cell = j < size;
-                        if (cell && r.S[c] == max_val) bd = imin(bd, iabs(j + begin - diag_i));
-                        if (!in_seed && cell && wadd(r.S[c], cx[s].ps[start + begin + j]) >= extension_cutoff) he = true;
-                    }
-                    const int gd = wreduce_min(bd);
-                    int bj = 0x7fffffff;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-                    for (int c = 0; c < kCPL; ++c) {
-                        const int j = j0 + c;
-                        if (j < size && r.S[c] == max_val && iabs(j + begin - diag_i) == gd) bj = imin(bj, j);
-                    }
-                    const int max_pos = wreduce_min(bj) + begin;
-                    const bool has_extension = in_seed || wballot(he) != 0;
-                    if (!in_seed && (max_val < cutoff || !has_extension))
-                        continue;                        // pop(table.size() - 1)
-                    table_size_bytes += 136ull * (cx[e].table_cap - cap_before)
-                        + 3ull * vec_capacity(size0, size) * 4;
-                    if ((int64_t)max_val - cutoff > xdrop) cutoff = max_val - xdrop;
-                    best_score = imax(best_score, max_val);
+                    const ColScan scan = reg_scan(r, size, begin, diag_i, in_seed, cx[s].ps + start + begin,
+                                                (score_t)((double)best_score * cfg.rel_score_cutoff + (double)partial_sum_offset));
+                    min_cell_score = imin(min_cell_score, scan.min);
+                    if (!accept_column(in_seed, scan.max, scan.has_extension, cap_before, cx[e].table_cap, size0, size, xdrop,
+                                       cutoff, best_score, table_size_bytes))
+                        continue;
                     if (cells_used > cells_limit) { overflow = true; continue; }
-                    // commit: DP table (compact format, whole 32-byte sectors) and the on-chip child buffer
-                    const int capr = capr_of(size);
-                    const uint32_t off = (cells_used + 7u) & ~7u;
-                    cells_used = off + 2 * capr + 8;
-                    score_t *dst = m.cells() + off;
-                    score_t *cb_S = sm.buf(cb);
-                    store_cells(dst, j0, r.S, capr);
-                    store_flags(reinterpret_cast<uint8_t*>(dst + capr), j0, r.fl);
-                    store_cells(cb_S, j0, r.S, 32); store_cells(cb_S + 2 * sm.bmax(), j0, r.F, 32);
-                    ColMeta col;
-                    col.node = cnode; col.parent = i; col.c = ch;
-                    col.offset = next_offset; col.max_pos = max_pos; col.trim = begin; col.score = add;
-                    col.is_tip = 0; col.started = 0; col.fmt = FMT_COMPACT; col.pad0 = col.pad1 = 0;
-                    col.size = size; col.cells_off = off;
+                    const uint32_t off = commit_compact(r, size, m.cells(), cells_used, sm.buf(cb), sm.bmax());
+                    const ColMeta col = make_col(cnode, i, ch, next_offset, scan.max_pos, begin, add, FMT_COMPACT, size, off);
                     const uint32_t idx = n_cols;
                     m.cols()[n_cols++] = col;
                     last_col = col; last_idx = idx;
-                    {   // band of this column under the (updated) cutoff, for when it is expanded
-                        uint32_t bits = 0;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-                        for (int c = 0; c < kCPL; ++c) if (j0 + c < size && r.S[c] >= cutoff) bits |= 1u << c;
-                        last_band_mask = kCPL == 32 ? bits : wreduce_or(bits << (j0 & 31));
-                        last_band_cutoff = cutoff; last_band_valid = true;
-                    }
+                    // band of this column under the (updated) cutoff, for when it is expanded
+                    last_band_mask = reg_band(r, size, cutoff); last_band_cutoff = cutoff; last_band_valid = true;
                     if (cb) res1 = (int)idx; else res0 = (int)idx;
                     wsync();
                     // convergence filter from registers (update_seed_filter)
@@ -2434,8 +2448,8 @@ struct ReadAligner {
                     const score_t converged = update_seed_filter_regs(e, cnode, vec_offset, r.S, s_first, size);
                     if (overflow) continue;
                     if (converged != kNinf) {
-                        HeapItem it; it.score = converged; it.neg_off_diag = -iabs(max_pos - diag_i);
-                        it.idx = idx; it.max_score = max_val;
+                        HeapItem it; it.score = converged; it.neg_off_diag = -iabs(scan.max_pos - diag_i);
+                        it.idx = idx; it.max_score = scan.max;
                         if (nn_n && converged == np[0].score) nn_push(nn_n, it);
                         else if (heap_n == 0 && nn_n == 0 && t == n_out) {
                             // sole candidate: pushing it and popping it in the next round is the
@@ -2445,7 +2459,7 @@ struct ReadAligner {
                             continue;
                         } else heap_push(heap_n, it);
                         // the column waits in the queue: a later expansion reads its F from the table
-                        store_cells(dst + capr + 8, j0, r.F, capr);
+                        store_cells(m.cells() + off + capr_of(size) + 8, wlane() * kCPL, r.F, capr_of(size));
                         m.cols()[idx].fmt = FMT_COMPACT_F; last_col.fmt = FMT_COMPACT_F;
                     }
                     continue;
@@ -2471,7 +2485,7 @@ struct ReadAligner {
             for (int j = wlane(); j < size0 + 5; j += kWarp) { sc.S[j] = kNinf; sc.E[j] = kNinf; sc.F[j] = kNinf; }
             wsync();
             const uint32_t cap_before = cx[e].table_cap;
-            if (n_cols + 1 > cx[e].table_cap) cx[e].table_cap = cx[e].table_cap ? 2 * cx[e].table_cap : 1;
+            cx[e].table_cap = table_capacity(cap_before, n_cols + 1);
 
             update_column(s, parS + shift, parF + shift, sc, size0, n, start + begin, cutoff,
                           code, add, next_offset > 1);
@@ -2503,23 +2517,13 @@ struct ReadAligner {
             }
             const score_t max_val = sc.S[max_pos - begin];
 
-            if (!in_seed && (max_val < cutoff || !has_extension))
-                continue;                        // pop(table.size() - 1)
-
-            table_size_bytes += 136ull * (cx[e].table_cap - cap_before)
-                + 3ull * vec_capacity(size0, size) * 4;
-
-            if ((int64_t)max_val - cutoff > xdrop) cutoff = max_val - xdrop;
-            best_score = imax(best_score, max_val);
-
+            if (!accept_column(in_seed, max_val, has_extension, cap_before, cx[e].table_cap, size0, size, xdrop, cutoff,
+                               best_score, table_size_bytes))
+                continue;
             if ((uint64_t)cells_used + 3ull * (size + 5) + 3ull * (wlen + 16) > 3ull * caps.max_cells) {
                 overflow = true; continue;
             }
-            ColMeta col;
-            col.node = cnode; col.parent = i; col.c = ch;
-            col.offset = next_offset; col.max_pos = max_pos; col.trim = begin; col.score = add;
-            col.is_tip = 0; col.started = 0; col.fmt = FMT_FULL; col.pad0 = col.pad1 = 0; col.size = size;
-            col.cells_off = commit_column(sc, size);
+            const ColMeta col = make_col(cnode, i, ch, next_offset, max_pos, begin, add, FMT_FULL, size, commit_column(sc, size));
             const uint32_t idx = n_cols;
             m.cols()[n_cols++] = col;
             last_col = col; last_idx = idx; last_band_valid = false;
@@ -2589,7 +2593,6 @@ struct ReadAligner {
         score_t *buf0 = sm.buf(0);
         const int bmax = sm.bmax();
         const int Lq = L;
-        const int j0 = wlane() * kCPL;
 
         uint32_t ci = io.ci; uint64_t c_node = io.c_node;
         int c_offset = io.c_offset, c_trim = io.c_trim, c_pb = io.c_pb;
@@ -2606,13 +2609,8 @@ struct ReadAligner {
         bool ovf = false;
 
         while (!stop) {                                    // every exit sets stop
-            if (c_maxval < best_score) {
-                if ((double)ncols / wlen >= cfg.max_nodes_per_seq_char) {                           // global_xdrop
-                    MGB_EMU_HIT(EMU_NODES_STOP_CHAIN); stop = 1; break;
-                }
-                if ((double)table_bytes / 1000000 > cfg.max_ram_per_alignment) {
-                    MGB_EMU_HIT(EMU_RAM_STOP_CHAIN); stop = 1; break;
-                }
+            if (const int b = budget_stop(cfg, c_maxval, best_score, ncols, wlen, table_bytes)) {
+                MGB_EMU_HIT(b == BUDGET_NODES ? EMU_NODES_STOP_CHAIN : EMU_RAM_STOP_CHAIN); stop = 1; break;
             }
             if (!c_bm) { stop = 1; break; }                    // no band: no children
             const int begin = ffs32(c_bm) - 1 + c_trim;
@@ -2657,8 +2655,7 @@ struct ReadAligner {
             // requests whose latency overlaps the DP below: the child's adjacency record, its convergence slot
             if (!rc) { pfn = cnode; pfa = adj[cnode]; }
             const uint64_t key = cnode + (rc ? n_edges : 0);
-            uint32_t hp = ((uint32_t)key * 0x9E3779B1u) ^ ((uint32_t)(key >> 32) * 0x85EBCA77u);
-            hp = (hp ^ (hp >> 15)) & hash_mask;
+            uint32_t hp = hash_node(key, hash_mask);
             ConvSlot sl = cslots[hp];
 
             const score_t *pS = buf0 + (size_t)c_pb * 3 * bmax + (begin - c_trim);
@@ -2670,33 +2667,9 @@ struct ReadAligner {
                                         pS, pS + 2 * bmax, n, size0, wlen + 1 - begin, 0, noff > 1, cutoff, go, ge,
                                         ge_shift, r);
             if (size < 0) { stop = 2; break; }
-            // per-column scan (:643-669)
             const int diag_i = noff - seed_off_m1;
-            score_t mn = 0x7fffffff, bs = INT32_MIN;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-            for (int c = 0; c < kCPL; ++c) {
-                const bool cell = j0 + c < size;
-                const score_t v = r.S[c];
-                if (cell && v != kNinf) mn = imin(mn, v);
-                if (cell) bs = imax(bs, v);
-            }
-            const score_t col_min = wreduce_min(mn);
-            const score_t max_val = wreduce_max(bs);
-            int bkey = 0x7fffffff; bool he = false;            // (distance to the diagonal, row) of the best cell
-            score_t ext_cut = 0;
-            if (!in_seed) ext_cut = (score_t)((double)best_score * rsc + pso);
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-            for (int c = 0; c < kCPL; ++c) {
-                const int j = j0 + c;
-                const bool cell = j < size;
-                if (cell && r.S[c] == max_val) bkey = imin(bkey, (iabs(j + begin - diag_i) << 5) | j);
-                if (!in_seed && cell && wadd(r.S[c], ps[start + begin + j]) >= ext_cut) he = true;
-            }
-            const int max_pos = (wreduce_min(bkey) & 31) + begin;
+            const ColScan scan = reg_scan(r, size, begin, diag_i, in_seed, ps + start + begin,
+                                          in_seed ? 0 : (score_t)((double)best_score * rsc + pso));
             // ---- convergence filter, first half (update_seed_filter, :100-156): find the node's entry. Cases
             // that move data around are left to the general code before anything has been written
             const int s_first = begin ? 0 : 1;
@@ -2727,37 +2700,18 @@ struct ReadAligner {
             }
 
             const uint32_t cap_before = t_cap;
-            if (ncols + 1 > t_cap) t_cap = t_cap ? 2 * t_cap : 1;
+            t_cap = table_capacity(t_cap, ncols + 1);
             made_cells += size; ++made;
-            min_cell_score = imin(min_cell_score, col_min);
-            if (!in_seed && (max_val < cutoff || !wballot(he))) { stop = 1; break; }   // pop(table.size() - 1)
-
-            table_bytes += 136ull * (t_cap - cap_before) + 3ull * vec_capacity(size0, size) * 4;
-            if ((int64_t)max_val - cutoff > xdrop) cutoff = max_val - xdrop;
-            best_score = imax(best_score, max_val);
+            min_cell_score = imin(min_cell_score, scan.min);
+            if (!accept_column(in_seed, scan.max, scan.has_extension, cap_before, t_cap, size0, size, xdrop, cutoff,
+                               best_score, table_bytes)) {
+                stop = 1; break;
+            }
             if (cused > cells_limit) { ovf = true; stop = 1; break; }
-            // ---- commit: DP table (compact format, whole 32-byte sectors) and the on-chip child buffer
-            const int capr = capr_of(size);
-            const uint32_t off = (cused + 7u) & ~7u;
-            cused = off + 2 * capr + 8;
-            score_t *dst = cells + off;
-            score_t *cb_S = buf0 + (size_t)(1 - c_pb) * 3 * bmax;
-            store_cells(dst, j0, r.S, capr);
-            store_flags(reinterpret_cast<uint8_t*>(dst + capr), j0, r.fl);
-            store_cells(cb_S, j0, r.S, 32); store_cells(cb_S + 2 * bmax, j0, r.F, 32);
-            ColMeta col;
-            col.node = cnode; col.parent = ci; col.c = ch;
-            col.offset = noff; col.max_pos = max_pos; col.trim = begin; col.score = 0;
-            col.is_tip = 0; col.started = 0; col.fmt = FMT_COMPACT; col.pad0 = col.pad1 = 0;
-            col.size = size; col.cells_off = off;
+            const uint32_t off = commit_compact(r, size, cells, cused, buf0 + (size_t)(1 - c_pb) * 3 * bmax, bmax);
             const uint32_t idx = ncols;
-            cols[ncols++] = col;
-            uint32_t bits = 0;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-            for (int c = 0; c < kCPL; ++c) if (j0 + c < size && r.S[c] >= cutoff) bits |= 1u << c;
-            const uint32_t bm_new = kCPL == 32 ? bits : wreduce_or(bits << (j0 & 31));
+            cols[ncols++] = make_col(cnode, ci, ch, noff, scan.max_pos, begin, 0, FMT_COMPACT, size, off);
+            const uint32_t bm_new = reg_band(r, size, cutoff);
 
             // ---- convergence filter, second half
             score_t converged;
@@ -2765,15 +2719,7 @@ struct ReadAligner {
             if (!hit) {
                 conv_used += sl.seg_cap; ++conv_n;
                 cslots[hp] = sl;
-                score_t mx = kNinf;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-                for (int c = 0; c < kCPL; ++c) {
-                    const int j = j0 + c;
-                    if (j >= s_first && j < size) { c0[j] = r.S[c]; mx = imax(mx, r.S[c]); }
-                }
-                converged = wreduce_max(mx);
+                converged = conv_store_regs(c0, r.S, s_first, size);
             } else {
                 const int old_end = sl.start + sl.size;
                 if (new_end > old_end) {                       // vec.resize(n, ninf)
@@ -2783,29 +2729,13 @@ struct ReadAligner {
                     cslots[hp] = sl;
                     wsync();
                 }
-                score_t max_changed = kNinf;
-#if MGB_DEVICE_CODE
-#pragma unroll
-#endif
-                for (int c = 0; c < kCPL; ++c) {
-                    const int j = j0 + c;
-                    if (j >= s_first && j < size) {
-                        score_t vj = c0[j];
-                        if ((double)r.S[c] > (double)vj * rsc) {
-                            vj = imax(vj, r.S[c]);
-                            c0[j] = vj;
-                            max_changed = imax(max_changed, vj);
-                        }
-                    }
-                }
-                converged = wreduce_max(max_changed);
+                converged = conv_merge_regs(c0, r.S, s_first, size, rsc);
             }
-            wsync();
             // the new column becomes the parent
             ci = idx; c_node = cnode; c_offset = noff; c_trim = begin; c_bm = bm_new; c_pb = 1 - c_pb;
-            c_maxval = max_val;
-            cur_it.score = converged; cur_it.neg_off_diag = -iabs(max_pos - diag_i); cur_it.idx = idx;
-            cur_it.max_score = max_val;
+            c_maxval = scan.max;
+            cur_it.score = converged; cur_it.neg_off_diag = -iabs(scan.max_pos - diag_i); cur_it.idx = idx;
+            cur_it.max_score = scan.max;
             if (converged == kNinf) { stop = 1; break; }
         }
         tc.table_cap = t_cap; tc.conv_n = conv_n; tc.conv_cells_used = conv_used;
