@@ -154,6 +154,14 @@ int mgb_index_create(const uint8_t *W, const uint8_t *last, uint64_t n_plus_1,
  * Set the mode once, right after mgb_index_create and before the index is shared between threads. */
 int mgb_index_set_mode(mgb_index_t *index, int mode);
 void mgb_index_destroy(mgb_index_t *index);
+/* A copy of src on `device` (src's own device allowed), made device to device: no host build, no build kernels.
+ * The graph mode and the tables mgb_index_set_mode built come along. The replica is independent of src: either may
+ * be destroyed first, and both may be used from several threads at once. Table for table, the replica is what
+ * mgb_index_create would build on `device` at that moment: the k-mer hash index, the path layout and its two leaner
+ * copies (DESIGN.md §4) follow the build's free-memory rules and knobs on that device, so a replica may leave out a
+ * table its source holds, never the reverse; results do not depend on these tables. A bad ordinal or a null
+ * argument: MGB_ERR_INVALID_ARGUMENT; a failed allocation or copy: MGB_ERR_CUDA, and nothing stays allocated. */
+int mgb_index_replicate(const mgb_index_t *src, int device, mgb_index_t **out);
 uint64_t mgb_index_num_edges(const mgb_index_t *index);
 uint64_t mgb_index_device_bytes(const mgb_index_t *index);
 uint32_t mgb_index_k(const mgb_index_t *index);
@@ -219,6 +227,20 @@ enum { MGB_FASTX_FWD_AND_REVERSE = 1 };
 int mgb_align_fastx_text(const mgb_index_t *index, const mgb_config_t *config, const char *buf, uint64_t bytes,
                          int at_eof, const char *comment_delim, int flags, int format,
                          uint64_t *consumed, int *ended, mgb_results_t **out);
+/* mgb_align_fastx_text in two steps, so that a caller learns where a chunk's records end long before they are
+ * aligned, and can hand the rest of its buffer on while the device aligns. mgb_fastx_stage parses the complete records
+ * of buf[0, bytes) as mgb_align_fastx_text does (on the device, or on the host for a chunk the device route refuses)
+ * and returns once *consumed and *ended are known. The records stay on index's device (or in host memory for a
+ * refused chunk); buf may be reused as soon as this returns. A staged batch holds one of the index's working-memory
+ * sets until it is aligned or freed. mgb_align_fastx_batch_text aligns and renders a staged batch as
+ * mgb_align_fastx_text would have, result stats included; the batch is consumed, also on error. A batch staged on
+ * another index: MGB_ERR_INVALID_ARGUMENT. mgb_fastx_batch_free frees a batch that will not be aligned (NULL: no-op). */
+typedef struct mgb_fastx_batch mgb_fastx_batch_t;
+int mgb_fastx_stage(const mgb_index_t *index, const char *buf, uint64_t bytes, int at_eof, const char *comment_delim,
+                    int flags, uint64_t *consumed, int *ended, mgb_fastx_batch_t **out);
+int mgb_align_fastx_batch_text(const mgb_index_t *index, const mgb_config_t *config, mgb_fastx_batch_t *batch,
+                               int format, mgb_results_t **out);
+void mgb_fastx_batch_free(mgb_fastx_batch_t *batch);
 /* Diagnostic entry, not needed to align files: the reads and headers mgb_align_fastx_text aligns for the same
  * arguments, without aligning them, so that the device parser can be checked against the host restatement and either
  * parser can be timed on its own. device_route = 1:

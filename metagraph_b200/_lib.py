@@ -87,6 +87,14 @@ def load_library(path=None):
     L.mgb_align_fastx_text.restype = i
     L.mgb_align_fastx_text.argtypes = [vp, ctypes.POINTER(mgb_config_t), vp, u64, i, cp, i, i, ctypes.POINTER(u64),
                                        ctypes.POINTER(i), ctypes.POINTER(vp)]
+    L.mgb_index_replicate.restype = i
+    L.mgb_index_replicate.argtypes = [vp, i, ctypes.POINTER(vp)]
+    L.mgb_fastx_stage.restype = i
+    L.mgb_fastx_stage.argtypes = [vp, vp, u64, i, cp, i, ctypes.POINTER(u64), ctypes.POINTER(i), ctypes.POINTER(vp)]
+    L.mgb_align_fastx_batch_text.restype = i
+    L.mgb_align_fastx_batch_text.argtypes = [vp, ctypes.POINTER(mgb_config_t), vp, i, ctypes.POINTER(vp)]
+    L.mgb_fastx_batch_free.restype = None
+    L.mgb_fastx_batch_free.argtypes = [vp]
     L.mgb_fastx_parse.restype = i
     L.mgb_fastx_parse.argtypes = [vp, vp, u64, i, cp, i, i, vp, u64, vp, vp, u64, vp, u64, ctypes.POINTER(u64),
                                   ctypes.POINTER(u64), ctypes.POINTER(i), ctypes.POINTER(i)]
@@ -139,7 +147,8 @@ REQUIRED_SYMBOLS = [
     "mgb_results_alignments", "mgb_results_stats", "mgb_results_free", "mgb_results_export_bytes",
     "mgb_results_export", "mgb_results_import", "mgb_boss_build", "mgb_boss_free",
     "mgb_boss_mask_dummy", "mgb_set_pipeline_pieces", "mgb_set_host_threads", "mgb_dbg_load", "mgb_dbg_last_error", "mgb_boss_last_error", "mgb_config_check", "mgb_dbg_load_suffix_ranges", "mgb_dbg_free_suffix_ranges", "mgb_index_set_mode",
-    "mgb_align_batch_text", "mgb_results_text", "mgb_align_fastx_text", "mgb_fastx_parse",
+    "mgb_align_batch_text", "mgb_results_text", "mgb_align_fastx_text", "mgb_fastx_parse", "mgb_index_replicate",
+    "mgb_fastx_stage", "mgb_align_fastx_batch_text", "mgb_fastx_batch_free",
 ]
 MGB_TEXT_TSV, MGB_TEXT_JSON = 1, 2
 MGB_FASTX_FWD_AND_REVERSE = 1

@@ -138,6 +138,14 @@ class DBGSuccinctIndex:
             self._L.mgb_index_destroy(self.handle)
             self.handle = None
 
+    def replicate(self, device):
+        """a copy of this index on `device` (mgb_index_replicate: device to device, no rebuild), with its own handle"""
+        h = ctypes.c_void_p()
+        _lib.check(self._L, self._L.mgb_index_replicate(self.handle, int(device), ctypes.byref(h)))
+        rep = DBGSuccinctIndex.__new__(DBGSuccinctIndex)
+        rep._L, rep.k, rep.mode, rep.handle = self._L, self.k, self.mode, h
+        return rep
+
     def __del__(self):
         try:
             self.close()
@@ -504,6 +512,36 @@ class B200Aligner:
             return self.text_of(res), consumed, ended
         finally:
             self.free_raw(res)
+
+    def stage_fastx(self, buf, at_eof=True, comment_delim=None, fwd_and_reverse=False):
+        """mgb_fastx_stage: parses the complete records of one chunk (a uint8 array or bytes) and returns (batch
+        handle, consumed, ended) as soon as the boundary is known; buf may be reused at once. The batch is aligned by
+        align_staged_text or freed by free_staged."""
+        arr = np.frombuffer(buf, np.uint8) if isinstance(buf, (bytes, bytearray, memoryview)) else buf
+        batch, consumed, ended = ctypes.c_void_p(), ctypes.c_uint64(), ctypes.c_int()
+        flags = _lib.MGB_FASTX_FWD_AND_REVERSE if fwd_and_reverse else 0
+        delim = None if comment_delim is None else _as_bytes(comment_delim)
+        _lib.check(self._L, self._L.mgb_fastx_stage(self.graph.handle, arr.ctypes.data, len(arr), int(bool(at_eof)),
+                                                    delim, flags, ctypes.byref(consumed), ctypes.byref(ended),
+                                                    ctypes.byref(batch)))
+        return batch, consumed.value, bool(ended.value)
+
+    def align_staged_text(self, batch, json=False):
+        """mgb_align_fastx_batch_text: the text of a staged batch, as align_fastx_text would have returned it; the
+        batch is consumed, also when this raises"""
+        c = self.config.to_c() if not isinstance(self.config, mgb_config_t) else self.config
+        res = ctypes.c_void_p()
+        fmt = _lib.MGB_TEXT_JSON if json else _lib.MGB_TEXT_TSV
+        _lib.check(self._L, self._L.mgb_align_fastx_batch_text(self.graph.handle, ctypes.byref(c), batch, fmt,
+                                                               ctypes.byref(res)))
+        try:
+            self.last_stats = self.stats_of(res)
+            return self.text_of(res)
+        finally:
+            self.free_raw(res)
+
+    def free_staged(self, batch):
+        self._L.mgb_fastx_batch_free(batch)
 
     def align(self, query):
         return self.align_batch([("", query)])[0]

@@ -1,9 +1,12 @@
 """`python -m metagraph_b200 align -i GRAPH.dbg [options] FILE...`: prints what `metagraph align` prints for the
-FASTA/FASTQ files (plain, .gz or .bgz), aligned on one device (CUDA_VISIBLE_DEVICES picks it).
+FASTA/FASTQ files (plain, .gz or .bgz), aligned on the devices --devices lists (CUDA_VISIBLE_DEVICES numbers them).
 
-The files are read in chunks; each chunk is parsed, aligned and rendered by mgb_align_fastx_text, so only the file's
-bytes go to the device and only the text comes back. A thread reads the next chunk while the device works on the
-current one. Output is in input order, which is one of the orders the reference's thread pool can print.
+The files are read in chunks; each chunk is parsed, aligned and rendered on a device, so only the file's bytes go to
+the device and only the text comes back. A thread reads the next chunk while the devices work. With one worker
+(`--devices 0`, the default) each chunk is one mgb_align_fastx_text call. With several, worker i mod W stages chunk i
+(mgb_fastx_stage: parse, and learn where its records end), hands the rest of the buffer on to the next worker and then
+aligns its batch while the next chunk is staged. Output is in input order either way, the same bytes for any worker
+list, and one of the orders the reference's thread pool can print.
 """
 import argparse
 import gzip
@@ -42,7 +45,10 @@ def _parser():
                    help="also align the reverse complement of each read, as a separate read under the same header")
     p.add_argument("--header-comment-delim", default=None, help="join the FASTA/FASTQ name and comment with this")
     p.add_argument("-p", "--parallel", type=int, default=1,
-                   help="accepted for compatibility; changes no output (one device does the work)")
+                   help="accepted for compatibility; changes no output (--devices sets the workers)")
+    p.add_argument("--devices", default="0", metavar="LIST",
+                   help="comma-separated CUDA ordinals, one worker each (an ordinal listed twice runs two workers on "
+                        "that device's one index), or `all`: every visible device once [0]")
     p.add_argument("--batch-size", type=int, default=100000000,
                    help="accepted for compatibility; changes no output")
     p.add_argument("--align-only-forwards", action="store_true")
@@ -84,6 +90,22 @@ def parse_args(argv):
     if args.align_alternative_alignments == 0:
         raise UsageError("align-alternative-alignments must be > 0")
     return args
+
+
+def devices_of(spec, count):
+    """the worker list of --devices: ordinals below `count`, the number of visible devices"""
+    if spec == "all":
+        if not count:
+            raise UsageError("--devices all: no CUDA device is visible")
+        return list(range(count))
+    try:
+        devices = [int(x) for x in spec.split(",")]
+    except ValueError:
+        raise UsageError("--devices takes comma-separated CUDA ordinals or `all`, not %r" % spec)
+    bad = [d for d in devices if not 0 <= d < count]
+    if bad:
+        raise UsageError("--devices: no CUDA device %d (%d visible)" % (bad[0], count))
+    return devices
 
 
 def config_of(args, k, alphabet):
@@ -177,6 +199,107 @@ def align_file(aligner, path, out, json=False, comment_delim=None, fwd_and_rever
     return written
 
 
+def align_file_workers(aligners, path, out, json=False, comment_delim=None, fwd_and_reverse=False,
+                       chunk_bytes=CHUNK_BYTES):
+    """align_file with one worker thread per aligner; the same bytes go to `out`. Chunk i is staged by worker i mod W,
+    which holds the token (the rest of the last buffer and the grow rule of align_file) while it reads and stages, and
+    hands it on before it aligns. A worker stages chunk i only once fewer than W texts wait ahead of the one to write
+    next. The first error stops every worker and the reader: nothing after the last text in order is written, every
+    staged batch is freed, every thread is joined, and the error is raised here."""
+    W = len(aligners)
+    opener = gzip.open if path.endswith((".gz", ".bgz")) else open
+    cv = threading.Condition()
+    st = dict(turn=0, pending=b"", at_eof=False, want=0, n_chunks=None, next_out=0, error=None, stop=False)
+    texts = {}
+
+    def halted():
+        return st["stop"] or st["error"] is not None
+
+    def failed(e):
+        with cv:
+            if st["error"] is None:
+                st["error"] = e
+            cv.notify_all()
+
+    def worker(w, al, chunks):
+        i = w
+        try:
+            while True:
+                with cv:
+                    cv.wait_for(lambda: halted() or st["n_chunks"] is not None
+                                or (st["turn"] == i and i <= st["next_out"] + W))
+                    if halted() or st["n_chunks"] is not None:
+                        return
+                # this worker holds the token: it alone reads and stages until it hands the token on
+                pending, at_eof, want = st["pending"], st["at_eof"], st["want"]
+                while not at_eof and not halted():
+                    nxt = chunks.next()
+                    at_eof = not nxt
+                    pending = pending + nxt if pending else nxt
+                    if len(pending) >= want:
+                        break
+                if halted():
+                    return
+                if not pending:
+                    with cv:
+                        st["n_chunks"] = i
+                        cv.notify_all()
+                    return
+                batch, consumed, ended = al.stage_fastx(pending, at_eof, comment_delim, fwd_and_reverse)
+                with cv:
+                    if ended or at_eof:
+                        st["n_chunks"] = i + 1
+                    else:
+                        st["want"] = 2 * len(pending) if consumed == 0 else 0
+                        st["pending"], st["at_eof"] = pending[consumed:], at_eof
+                    st["turn"] = i + 1
+                    cv.notify_all()
+                    stop = halted()
+                if stop:
+                    al.free_staged(batch)
+                    return
+                text = al.align_staged_text(batch, json)      # consumes the batch
+                with cv:
+                    texts[i] = text
+                    cv.notify_all()
+                i += W
+        except BaseException as e:
+            failed(e)
+
+    written = 0
+    with opener(path, "rb") as f:
+        chunks = _Chunks(f, chunk_bytes)
+        threads = []
+        try:
+            for w, al in enumerate(aligners):
+                threads.append(threading.Thread(target=worker, args=(w, al, chunks)))
+                threads[-1].start()
+            while True:
+                with cv:
+                    cv.wait_for(lambda: st["error"] is not None or st["next_out"] in texts
+                                or st["n_chunks"] == st["next_out"])
+                    if st["error"] is not None or st["n_chunks"] == st["next_out"]:
+                        break
+                    text = texts.pop(st["next_out"])
+                out.write(text)
+                written += len(text)
+                with cv:
+                    st["next_out"] += 1
+                    cv.notify_all()
+        except BaseException as e:
+            failed(e)
+        finally:
+            with cv:
+                st["stop"] = True
+                cv.notify_all()
+            for t in threads:
+                t.join()
+            chunks.close()
+    if st["error"] is not None:
+        raise st["error"]
+    return written
+
+
 def main(argv=None):
     argv = sys.argv[1:] if argv is None else argv
     if not argv or argv[0] != "align":
@@ -184,24 +307,57 @@ def main(argv=None):
         return 2
     try:
         args = parse_args(argv[1:])
+        from . import _lib
         from .aligner import B200Aligner, BOSSTable, DBGSuccinctIndex
+        devices = devices_of(args.devices, _lib.load_library().mgb_device_count())
         boss = BOSSTable.from_dbg(args.graph)
         alphabet = {0: "dna", 1: "protein"}.get(boss.alphabet, "code %d" % boss.alphabet)
         cfg = config_of(args, boss.k, alphabet)
     except UsageError as e:
         sys.stderr.write("error: %s\n" % e)
         return 1
-    index = DBGSuccinctIndex(boss, device=0)
-    aligner = B200Aligner(index, cfg)
-    for path in args.files:
-        if not os.path.exists(path):
-            sys.stderr.write("ERROR: Cannot read from file %s\n" % path)
-            return 1
-        if args.outfile:
-            with open(args.outfile, "wb") as out:       # reopened and truncated per input (cli/align.cpp:409-411)
-                align_file(aligner, path, out, args.json, args.header_comment_delim, args.fwd_and_reverse)
-        else:
-            align_file(aligner, path, sys.stdout.buffer, args.json, args.header_comment_delim, args.fwd_and_reverse)
-            sys.stdout.buffer.flush()
-    index.close()
+    # the index is built once, on the first listed device, and copied device to device to the others, all at once
+    indexes = {devices[0]: DBGSuccinctIndex(boss, device=devices[0])}
+    try:
+        errors = []
+
+        def replicate(d):
+            try:
+                indexes[d] = indexes[devices[0]].replicate(d)
+            except Exception as e:
+                errors.append(e)
+
+        threads = [threading.Thread(target=replicate, args=(d,)) for d in sorted(set(devices[1:]) - {devices[0]})]
+        for t in threads:
+            t.start()
+        for t in threads:
+            t.join()
+        if errors:
+            raise errors[0]
+        aligners = [B200Aligner(indexes[d], cfg) for d in devices]
+
+        def align(path, out):
+            if len(aligners) == 1:
+                align_file(aligners[0], path, out, args.json, args.header_comment_delim, args.fwd_and_reverse,
+                           CHUNK_BYTES)
+            else:
+                align_file_workers(aligners, path, out, args.json, args.header_comment_delim, args.fwd_and_reverse,
+                                   CHUNK_BYTES)
+
+        for path in args.files:
+            if not os.path.exists(path):
+                sys.stderr.write("ERROR: Cannot read from file %s\n" % path)
+                return 1
+            if args.outfile:
+                with open(args.outfile, "wb") as out:       # reopened and truncated per input (cli/align.cpp:409-411)
+                    align(path, out)
+            else:
+                align(path, sys.stdout.buffer)
+                sys.stdout.buffer.flush()
+    except Exception as e:
+        sys.stderr.write("error: %s\n" % e)
+        return 1
+    finally:
+        for ix in indexes.values():
+            ix.close()
     return 0

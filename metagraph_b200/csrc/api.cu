@@ -284,7 +284,9 @@ struct mgb_index {
     int device = 0;
     uint64_t device_bytes = 0;
     int num_sms = 1;
-    std::vector<void*> bufs;
+    struct DevArray { const void *p; size_t bytes; };
+    std::vector<DevArray> bufs;        // every device array the index owns (the device build)
+    void keep(const void *p, size_t bytes) { bufs.push_back({ p, bytes }); device_bytes += bytes; }
 #if defined(MGB_HOST_EMU)
     std::vector<uint32_t> rc_host;   // PRIMARY graphs: rcs / rcp / palin (mgb_index_set_mode)
 #endif
@@ -310,7 +312,7 @@ struct mgb_index {
 
 mgb_index::~mgb_index() {
 #if !defined(MGB_HOST_EMU)
-    if (!bufs.empty()) { cudaSetDevice(device); for (void *p : bufs) cudaFree(p); }
+    if (!bufs.empty()) { cudaSetDevice(device); for (const DevArray &b : bufs) cudaFree(const_cast<void*>(b.p)); }
 #endif
     for (Workspace *w : ws_free) delete w;
 }
@@ -393,8 +395,8 @@ static int build_layout_words(mgb_index *idx) {
         cudaFree(pl_word); cudaFree(kh_pos);
         return fail(MGB_ERR_CUDA, std::string("layout words: ") + cudaGetErrorString(e));
     }
-    if (pl_word) { idx->bufs.push_back(pl_word); idx->device_bytes += word_bytes; v.pl_word = pl_word; }
-    if (kh_pos) { idx->bufs.push_back(kh_pos); idx->device_bytes += pos_bytes; v.kh_pos = kh_pos; }
+    if (pl_word) { idx->keep(pl_word, word_bytes); v.pl_word = pl_word; }
+    if (kh_pos) { idx->keep(kh_pos, pos_bytes); v.kh_pos = kh_pos; }
     return MGB_OK;
 }
 
@@ -472,14 +474,52 @@ static int build_path_layout(mgb_index *idx, const unsigned long long *kmer) {
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
     if (int rc = check("path layout")) return rc;
     cudaFree(a.jump); cudaFree(ctr);
-    idx->bufs.push_back(a.pred); idx->bufs.push_back(a.node); idx->bufs.push_back(a.text); idx->bufs.push_back(a.rc);
-    idx->bufs.push_back(a.stop);
-    idx->device_bytes += (n + 1) * 4 + bytes;
+    idx->keep(a.pred, (n + 1) * 4); idx->keep(a.node, n_pos * 4); idx->keep(a.text, n_pos / 4); idx->keep(a.rc, n_pos / 8);
+    idx->keep(a.stop, n_pos / 8);
     idx->view.pl_pos = a.pred; idx->view.pl_node = a.node;
     idx->view.pl_text = reinterpret_cast<const unsigned long long*>(a.text);
     idx->view.pl_rc = a.rc; idx->view.pl_stop = a.stop;
     idx->view.pl_n = n_pos;
     return build_layout_words(idx);
+}
+#endif
+
+#if !defined(MGB_HOST_EMU)
+// what an index sets up on the device it lives on (the current device)
+static void device_setup(int device) {
+    {   // Every access of this path to the index and to the per-read arenas is a single 8 .. 64-byte record at a
+        // data-dependent address; L2 may fetch whole 128-byte lines from HBM for them. MGB_L2_FETCH=32 / 64 asks for
+        // smaller fetches (process-wide): fewer bytes, but the access rate, not the bytes, is what HBM limits on this
+        // path, so the default is left alone unless MGB_L2_FETCH is set.
+        size_t gran = 0;
+        if (const char *e = std::getenv("MGB_L2_FETCH")) gran = (size_t)std::atoi(e);
+        if (gran) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, gran);
+        cudaGetLastError();
+    }
+    {   // keep stream-ordered allocations cached between calls
+        cudaMemPool_t pool;
+        if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
+            uint64_t thr = UINT64_MAX;
+            cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
+        }
+    }
+}
+
+// f(field, name, opt) for every pointer of the view: the table's name and, for the tables mgb_index_create builds only
+// when the device memory is there (and no knob leaves them out), which one it is
+enum class Opt { none, hash, path, pl_word, kh_pos };
+template <class F> static void each_table(IndexView &v, F &&f) {
+    f(v.blocks, "blocks", Opt::none); f(v.blk_rank, "blk_rank", Opt::none); f(v.sel_last, "sel_last", Opt::none);
+    for (auto &p : v.sel_W) f(p, "sel_W", Opt::none);
+    f(v.valid, "valid", Opt::none); f(v.sfx, "sfx", Opt::none); f(v.adj, "adj", Opt::none);
+    f(v.radj, "radj", Opt::none);
+    f(v.kh_keys, "kh_keys", Opt::hash); f(v.kh_vals, "kh_vals", Opt::hash);
+    f(v.pl_node, "pl_node", Opt::path); f(v.pl_pos, "pl_pos", Opt::path); f(v.pl_text, "pl_text", Opt::path);
+    f(v.pl_rc, "pl_rc", Opt::path); f(v.pl_stop, "pl_stop", Opt::path);
+    f(v.kh_pos, "kh_pos", Opt::kh_pos); f(v.pl_word, "pl_word", Opt::pl_word);
+    f(v.rcs, "rcs", Opt::none); f(v.rcp, "rcp", Opt::none); f(v.palin, "palin", Opt::none);
+    f(v.wW, "wW", Opt::none); f(v.wl, "wl", Opt::none); f(v.wrank, "wrank", Opt::none); f(v.wsel, "wsel", Opt::none);
+    f(v.wadj, "wadj", Opt::none);
 }
 #endif
 
@@ -579,32 +619,16 @@ int mgb_index_create(const uint8_t *W, const uint8_t *last, uint64_t n_plus_1, c
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
     idx->num_sms = prop.multiProcessorCount;
-    {   // Every access of this path to the index and to the per-read arenas is a single 8 .. 64-byte record at a
-        // data-dependent address; L2 may fetch whole 128-byte lines from HBM for them. MGB_L2_FETCH=32 / 64 asks for
-        // smaller fetches (process-wide): fewer bytes, but the access rate, not the bytes, is what HBM limits on this
-        // path, so the default is left alone unless MGB_L2_FETCH is set.
-        size_t gran = 0;
-        if (const char *e = std::getenv("MGB_L2_FETCH")) gran = (size_t)std::atoi(e);
-        if (gran) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, gran);
-        cudaGetLastError();
-    }
-    {   // keep stream-ordered allocations cached between calls
-        cudaMemPool_t pool;
-        if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
-            uint64_t thr = UINT64_MAX;
-            cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
-        }
-    }
+    device_setup(device);
     IndexView v = h.view();
     auto upload = [&](const std::vector<uint32_t> &src, const uint32_t **dst) -> int {
         if (src.empty()) { *dst = nullptr; return 0; }
         void *p = nullptr;
         cudaError_t e = cudaMalloc(&p, src.size() * 4);
         if (e != cudaSuccess) return fail(MGB_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-        idx->bufs.push_back(p);
+        idx->keep(p, src.size() * 4);
         e = cudaMemcpy(p, src.data(), src.size() * 4, cudaMemcpyHostToDevice);
         if (e != cudaSuccess) return fail(MGB_ERR_CUDA, std::string("cudaMemcpy: ") + cudaGetErrorString(e));
-        idx->device_bytes += src.size() * 4;
         *dst = (const uint32_t*)p;
         return 0;
     };
@@ -631,10 +655,9 @@ int mgb_index_create(const uint8_t *W, const uint8_t *last, uint64_t n_plus_1, c
         void *p = nullptr;
         cudaError_t e = cudaMalloc(&p, h.adj.size() * sizeof(uint2));
         if (e != cudaSuccess) return fail(MGB_ERR_CUDA, std::string("cudaMalloc(adj): ") + cudaGetErrorString(e));
-        idx->bufs.push_back(p);
+        idx->keep(p, h.adj.size() * sizeof(uint2));
         e = cudaMemcpy(p, h.adj.data(), h.adj.size() * sizeof(uint2), cudaMemcpyHostToDevice);
         if (e != cudaSuccess) return fail(MGB_ERR_CUDA, std::string("cudaMemcpy(adj): ") + cudaGetErrorString(e));
-        idx->device_bytes += h.adj.size() * sizeof(uint2);
         v.adj = (const uint2*)p;
     }
     idx->view = v;
@@ -657,11 +680,10 @@ int mgb_index_create(const uint8_t *W, const uint8_t *last, uint64_t n_plus_1, c
             // the previous level is no longer needed (the host-built one is freed with the index)
             if (len > sfx_host + 1) {
                 cudaFree((void*)cur);
-                idx->bufs.erase(std::find(idx->bufs.begin(), idx->bufs.end(), (void*)cur));
+                idx->bufs.erase(std::find_if(idx->bufs.begin(), idx->bufs.end(), [&](const mgb_index::DevArray &b) { return b.p == cur; }));
                 idx->device_bytes -= cur_num * 8;
             }
-            idx->bufs.push_back(nxt);
-            idx->device_bytes += nxt_num * 8;
+            idx->keep(nxt, nxt_num * 8);
             cur = nxt; cur_num = nxt_num;
             idx->view.sfx = nxt; idx->view.sfx_len = len;
         }
@@ -723,12 +745,10 @@ int mgb_index_create(const uint8_t *W, const uint8_t *last, uint64_t n_plus_1, c
             cudaFree(kmer); cudaFree(radj); cudaFree(kh_keys); cudaFree(kh_vals);
             return fail(MGB_ERR_CUDA, std::string("radj / k-mer hash build: ") + cudaGetErrorString(e));
         }
-        idx->bufs.push_back(radj);
-        idx->device_bytes += (n + 1) * sizeof(uint2);
+        idx->keep(radj, (n + 1) * sizeof(uint2));
         idx->view.radj = radj;
         if (kh_keys) {
-            idx->bufs.push_back(kh_keys); idx->bufs.push_back(kh_vals);
-            idx->device_bytes += kh_slots * 12;
+            idx->keep(kh_keys, kh_slots * 8); idx->keep(kh_vals, kh_slots * 4);
             idx->view.kh_keys = kh_keys; idx->view.kh_vals = kh_vals; idx->view.kh_slots = kh_slots;
             rc = build_path_layout(idx.get(), kmer);
         }
@@ -771,8 +791,7 @@ int mgb_index_set_mode(mgb_index_t *index, int mode) {
         e = cudaGetLastError();
         if (e == cudaSuccess) e = cudaDeviceSynchronize();
         if (e != cudaSuccess) { cudaFree(buf); return fail(MGB_ERR_CUDA, std::string("rc tables: ") + cudaGetErrorString(e)); }
-        index->bufs.push_back(buf);
-        index->device_bytes += words * 4;
+        index->keep(buf, words * 4);
 #endif
         index->view.rcs = ra.rcs; index->view.rcp = ra.rcp; index->view.palin = ra.palin;
     }
@@ -781,6 +800,127 @@ int mgb_index_set_mode(mgb_index_t *index, int mode) {
 }
 
 void mgb_index_destroy(mgb_index_t *index) { delete index; }
+
+int mgb_index_replicate(const mgb_index_t *src, int device, mgb_index_t **out) {
+    if (!src || !out) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    std::unique_ptr<mgb_index> idx(new mgb_index());
+    idx->alphabet = src->alphabet;
+    idx->at = src->at;
+#if defined(MGB_HOST_EMU)
+    if (device != 0) return fail(MGB_ERR_INVALID_ARGUMENT, "bad device ordinal");
+    // the emulated index has none of the tables that depend on free memory; its arrays are host vectors
+    idx->host = src->host;
+    idx->radj_host = src->radj_host;
+    idx->rc_host = src->rc_host;
+    idx->device_bytes = src->device_bytes;
+    const IndexView &s = src->view;
+    IndexView v = idx->host.view();
+    v.sfx_len = s.sfx_len;
+    v.mode = s.mode;
+    v.radj = idx->radj_host.data();
+    auto rc_of = [&](const uint32_t *p) { return p ? idx->rc_host.data() + (p - src->rc_host.data()) : nullptr; };
+    v.rcs = rc_of(s.rcs); v.rcp = rc_of(s.rcp); v.palin = rc_of(s.palin);
+    idx->view = v;
+#else
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+        return fail(MGB_ERR_NO_DEVICE, "no CUDA device available (the kernels have no CPU fallback)");
+    if (device < 0 || device >= ndev) return fail(MGB_ERR_INVALID_ARGUMENT, "bad device ordinal");
+    CUDA_TRY(cudaSetDevice(device));
+    idx->device = device;
+    cudaDeviceProp prop;
+    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
+    idx->num_sms = prop.multiProcessorCount;
+    device_setup(device);
+    // the source's arrays the view points into (not the host-built suffix level the deeper ones replaced), and the
+    // table each one holds
+    IndexView v = src->view;
+    struct Copy { const mgb_index::DevArray *from; const char *name; Opt opt; void *to; };
+    std::vector<Copy> copies;
+    const char *stray = nullptr;
+    each_table(v, [&](auto &field, const char *name, Opt opt) {
+        if (!field) return;
+        const char *p = reinterpret_cast<const char*>(field);
+        for (const mgb_index::DevArray &b : src->bufs) {
+            if (p < (const char*)b.p || p >= (const char*)b.p + b.bytes) continue;
+            for (const Copy &c : copies) if (c.from == &b) return;
+            copies.push_back({ &b, name, opt, nullptr });
+            return;
+        }
+        stray = name;
+    });
+    if (stray) return fail(MGB_ERR_INVALID_ARGUMENT, std::string("table ") + stray + " is not an array of the index");
+    struct Undo {                // frees the copies unless they went to the replica
+        std::vector<Copy> &c; cudaStream_t s = nullptr; bool done = false;
+        ~Undo() {
+            if (s) cudaStreamDestroy(s);
+            if (!done) for (Copy &x : c) cudaFree(x.to);
+        }
+    } undo { copies };
+    // allocates the arrays of one table class; the first that fails, else nullptr (and none of the class is kept)
+    auto alloc = [&](Opt opt) -> const Copy* {
+        for (Copy &c : copies) {
+            if (c.opt != opt || cudaMalloc(&c.to, c.from->bytes) == cudaSuccess) continue;
+            cudaGetLastError();
+            for (Copy &d : copies) if (d.opt == opt) { cudaFree(d.to); d.to = nullptr; }
+            return &c;
+        }
+        return nullptr;
+    };
+    if (const Copy *c = alloc(Opt::none)) return fail(MGB_ERR_CUDA, std::string("cudaMalloc(") + c->name + ") failed");
+    // The optional tables follow mgb_index_create's rules on this device, in its order, each checked with the free
+    // memory the build would see there: less the temporaries the build holds at that point (7 bytes per edge for the
+    // radj rounds, 8 for the per-edge k-mers, 12 for the path layout's pred and jump arrays).
+    const double n1 = (double)(v.n + 1);
+    size_t free_b = 0, total_b = 0;
+    auto free_now = [&]() { cudaMemGetInfo(&free_b, &total_b); return (double)free_b; };
+    bool hash = v.kh_slots && !std::getenv("MGB_NO_KMER_HASH")
+                && free_now() - 7 * n1 > 1.2 * (8.0 * n1 + 12.0 * v.kh_slots) + 16e9 && !alloc(Opt::hash);
+    bool path = hash && v.pl_n && !std::getenv("MGB_NO_PATH_INDEX");
+    if (path) {
+        const double f = free_now() - 8 * n1, pl = (double)v.pl_n;
+        path = f >= 1.2 * 16.5 * n1 && f - 8.6 * n1 >= 16e9
+               && f - 12 * n1 >= 1.2 * (pl * 4 + pl / 4 + 2 * (pl / 8)) && !alloc(Opt::path);
+    }
+    if (path) {
+        const char *no = std::getenv("MGB_TEST_NO_LAYOUT_WORDS");
+        const double keep = std::max(16e9, 0.5 * (double)total_b), word_bytes = (double)(v.pl_n / 32 * 16);
+        double left = free_now() - 8 * n1;
+        if (v.pl_word && (!no || !std::strcmp(no, "kh_pos")) && left - word_bytes >= keep && !alloc(Opt::pl_word))
+            left -= word_bytes;
+        if (v.kh_pos && (!no || !std::strcmp(no, "pl_word")) && left - 4.0 * v.kh_slots >= keep) alloc(Opt::kh_pos);
+    }
+    CUDA_TRY(cudaStreamCreateWithFlags(&undo.s, cudaStreamNonBlocking));
+    for (const Copy &c : copies) {
+        if (!c.to) continue;
+        const cudaError_t e = device == src->device
+            ? cudaMemcpyAsync(c.to, c.from->p, c.from->bytes, cudaMemcpyDeviceToDevice, undo.s)
+            : cudaMemcpyPeerAsync(c.to, device, c.from->p, src->device, c.from->bytes, undo.s);
+        if (e != cudaSuccess) return fail(MGB_ERR_CUDA, std::string("copy of ") + c.name + ": " + cudaGetErrorString(e));
+    }
+    // re-point the view; a table left out is absent, as in an index built without it
+    each_table(v, [&](auto &field, const char *, Opt) {
+        using P = std::remove_reference_t<decltype(field)>;
+        const char *p = reinterpret_cast<const char*>(field);
+        for (const Copy &c : copies) {
+            const char *b = (const char*)c.from->p;
+            if (p && p >= b && p < b + c.from->bytes) { field = c.to ? reinterpret_cast<P>((char*)c.to + (p - b)) : nullptr; return; }
+        }
+    });
+    if (!hash) v.kh_slots = 0;
+    if (!path) v.pl_n = 0;
+    if (src->view.kh_slots && !hash)         // y[16:21) is defined only with the hash index
+        kern_dna::k_adj_clear_rc<<<(unsigned)idx->num_sms * 16, 256, 0, undo.s>>>(const_cast<uint2*>(v.adj), v.n);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaStreamSynchronize(undo.s);
+    if (e != cudaSuccess) return fail(MGB_ERR_CUDA, std::string("index replica copy: ") + cudaGetErrorString(e));
+    for (const Copy &c : copies) if (c.to) idx->keep(c.to, c.from->bytes);
+    undo.done = true;
+    idx->view = v;
+#endif
+    *out = idx.release();
+    return MGB_OK;
+}
 
 uint64_t mgb_index_num_edges(const mgb_index_t *index) { return index->view.n; }
 uint64_t mgb_index_device_bytes(const mgb_index_t *index) { return index->device_bytes; }
@@ -2208,35 +2348,71 @@ static int fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes
     return MGB_OK;
 }
 
+} // extern "C"
+
+// A chunk's records between mgb_fastx_stage and mgb_align_fastx_batch_text: the stage's workspace (its "batch" region
+// holds the parsed arrays on the device) and stream, the host restatement's records for a refused chunk, and the
+// parse's own copies and launches, which the result set reports.
+struct mgb_fastx_batch {
+    CallWorkspace cw;
+    DevBufs bufs;
+    FastxDev dev;
+    FastxRecords host;
+    mgb_stats_t parse;
+    explicit mgb_fastx_batch(const mgb_index_t *index) : cw(index), bufs(cw.st, cw.w, kBatchSlots) {
+        std::memset(&parse, 0, sizeof(parse));
+    }
+};
+
+extern "C" {
+
+int mgb_fastx_stage(const mgb_index_t *index, const char *buf, uint64_t bytes, int at_eof, const char *comment_delim,
+                    int flags, uint64_t *consumed, int *ended, mgb_fastx_batch_t **out) {
+    if (!index || !consumed || !ended || !out || (!buf && bytes)) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (flags & ~MGB_FASTX_FWD_AND_REVERSE) return fail(MGB_ERR_INVALID_ARGUMENT, "unknown flags");
+    std::unique_ptr<mgb_fastx_batch> b(new mgb_fastx_batch(index));
+    int rc = b->cw.ready();
+    if (rc) return rc;
+    rc = fastx_parse(index, buf, bytes, at_eof != 0, comment_delim, (flags & MGB_FASTX_FWD_AND_REVERSE) != 0, true,
+                     b->cw.st, b->bufs, &b->dev, &b->host, consumed, ended, &b->parse);
+    if (rc) return rc;
+    const std::vector<uint64_t> &offs = b->dev.refused ? b->host.offsets : b->dev.offsets;
+    if (offs.size() - 1 > 0xffffffffull) return fail(MGB_ERR_OVERFLOW, "more than 2^32 - 1 records in one chunk");
+    *out = b.release();
+    return MGB_OK;
+}
+
+int mgb_align_fastx_batch_text(const mgb_index_t *index, const mgb_config_t *config, mgb_fastx_batch_t *batch,
+                               int format, mgb_results_t **out) {
+    std::unique_ptr<mgb_fastx_batch> b(batch);
+    if (!index || !config || !batch || !out) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (b->cw.ix != index) return fail(MGB_ERR_INVALID_ARGUMENT, "the batch was staged on another index");
+    if (format != MGB_TEXT_TSV && format != MGB_TEXT_JSON)
+        return fail(MGB_ERR_INVALID_ARGUMENT, "format must be MGB_TEXT_TSV or MGB_TEXT_JSON");
+    const FastxDev &dev = b->dev;
+    const FastxRecords &host = b->host;
+    const std::vector<uint64_t> &offs = dev.refused ? host.offsets : dev.offsets;
+    const uint32_t n = (uint32_t)(offs.size() - 1);
+    const int rc = dev.refused ? align_batch(index, config, host.seqs.data(), host.offsets.data(), host.names.data(),
+                                             host.name_offsets.data(), n, format, out)
+                               : align_batch(index, config, dev.seqs, dev.offsets.data(), dev.names,
+                                             dev.name_offsets.data(), n, format, out, true);
+    if (rc) return rc;
+    add_stats((*out)->stats, b->parse);
+    return MGB_OK;
+}
+
+void mgb_fastx_batch_free(mgb_fastx_batch_t *batch) { delete batch; }
+
 int mgb_align_fastx_text(const mgb_index_t *index, const mgb_config_t *config, const char *buf, uint64_t bytes,
                          int at_eof, const char *comment_delim, int flags, int format, uint64_t *consumed, int *ended,
                          mgb_results_t **out) {
     if (!index || !config || !consumed || !ended || !out || (!buf && bytes)) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
     if (format != MGB_TEXT_TSV && format != MGB_TEXT_JSON)
         return fail(MGB_ERR_INVALID_ARGUMENT, "format must be MGB_TEXT_TSV or MGB_TEXT_JSON");
-    if (flags & ~MGB_FASTX_FWD_AND_REVERSE) return fail(MGB_ERR_INVALID_ARGUMENT, "unknown flags");
-    CallWorkspace cw(index);
-    int rc = cw.ready();
-    if (rc) return rc;
-    DevBufs bufs(cw.st, cw.w, kBatchSlots);
-    FastxDev dev;
-    FastxRecords host;
-    mgb_stats_t parse;
-    std::memset(&parse, 0, sizeof(parse));
-    const bool fwd_rev = flags & MGB_FASTX_FWD_AND_REVERSE;
-    rc = fastx_parse(index, buf, bytes, at_eof != 0, comment_delim, fwd_rev, true, cw.st, bufs, &dev, &host, consumed,
-                     ended, &parse);
-    if (rc) return rc;
-    const std::vector<uint64_t> &offs = dev.refused ? host.offsets : dev.offsets;
-    if (offs.size() - 1 > 0xffffffffull) return fail(MGB_ERR_OVERFLOW, "more than 2^32 - 1 records in one chunk");
-    const uint32_t n = (uint32_t)(offs.size() - 1);
-    rc = dev.refused ? align_batch(index, config, host.seqs.data(), host.offsets.data(), host.names.data(),
-                                   host.name_offsets.data(), n, format, out)
-                     : align_batch(index, config, dev.seqs, dev.offsets.data(), dev.names, dev.name_offsets.data(), n,
-                                   format, out, true);
-    if (rc) return rc;
-    add_stats((*out)->stats, parse);
-    return MGB_OK;
+    mgb_fastx_batch_t *batch = nullptr;
+    const int rc = mgb_fastx_stage(index, buf, bytes, at_eof, comment_delim, flags, consumed, ended, &batch);
+    return rc ? rc : mgb_align_fastx_batch_text(index, config, batch, format, out);
 }
 
 int mgb_fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes, int at_eof, const char *comment_delim,

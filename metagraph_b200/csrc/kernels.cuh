@@ -1721,6 +1721,13 @@ __global__ void __launch_bounds__(256) k_adj_rc(IndexView ix, uint2 *adj, const 
         if (bits) adj[e].y = a.y | bits;
     }
 }
+// Clears y[16:21) of every forward adjacency record: a replica that leaves out the hash index (mgb_index_replicate)
+// holds the records mgb_index_create builds without it.
+__global__ void __launch_bounds__(256) k_adj_clear_rc(uint2 *adj, uint64_t n) {
+    uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint64_t nt = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t e = 1 + t; e <= n; e += nt) adj[e].y &= ~(0x1Fu << 16);
+}
 
 // Path layout (IndexView::pl_*), built once the hash index is complete. Its nodes are the DBG nodes the seeding walk
 // stores (in_graph, a k-mer without '$'). A node whose target has exactly one such child links to it; a child that several
