@@ -241,6 +241,27 @@ int mgb_fastx_stage(const mgb_index_t *index, const char *buf, uint64_t bytes, i
 int mgb_align_fastx_batch_text(const mgb_index_t *index, const mgb_config_t *config, mgb_fastx_batch_t *batch,
                                int format, mgb_results_t **out);
 void mgb_fastx_batch_free(mgb_fastx_batch_t *batch);
+/* mgb_fastx_stage for BGZF input (the block gzip of htslib's bgzip: gzip members of at most 64 KiB of text whose header
+ * carries the member's size). Stages the text `head` (carried over from the previous chunk, host memory) followed by
+ * the text of the complete BGZF blocks at the start of cbuf, inflated on index's device, until their text reaches
+ * max_text. Returns as mgb_fastx_stage does, *consumed and *ended over head + inflated text. *c_consumed: compressed
+ * bytes of the blocks taken. *c_refused = 1: the member at *c_consumed is not served by the device route (not a BGZF
+ * block, its inflate, CRC32 or ISIZE check failed, or it is cut off by the end of the input, c_eof); blocks after it
+ * are not taken. The records are parsed with at_eof = c_eof && *c_consumed == cbytes && !*c_refused. The text after
+ * *consumed stays with the batch (mgb_fastx_batch_tail). The batch is aligned by mgb_align_fastx_batch_text; its
+ * h2d_bytes count the compressed bytes uploaded. */
+int mgb_fastx_stage_bgzf(const mgb_index_t *index, const char *head, uint64_t head_bytes, const uint8_t *cbuf,
+                         uint64_t cbytes, int c_eof, uint64_t max_text, const char *comment_delim, int flags,
+                         uint64_t *c_consumed, int *c_refused, uint64_t *consumed, int *ended,
+                         mgb_fastx_batch_t **out);
+/* text[consumed, end) of a batch staged by mgb_fastx_stage_bgzf, owned by the batch (valid until it is aligned or
+ * freed); empty for a batch of mgb_fastx_stage */
+int mgb_fastx_batch_tail(const mgb_fastx_batch_t *batch, const char **tail, uint64_t *bytes);
+/* Diagnostic entry, as mgb_fastx_parse is: the complete BGZF blocks of cbuf inflated on index's device and downloaded
+ * into out (MGB_ERR_OVERFLOW if they do not fit). *n_blocks: blocks inflated; *c_consumed and *refused as in
+ * mgb_fastx_stage_bgzf. */
+int mgb_bgzf_inflate(const mgb_index_t *index, const uint8_t *cbuf, uint64_t cbytes, int c_eof, char *out,
+                     uint64_t out_cap, uint64_t *out_bytes, uint64_t *c_consumed, uint64_t *n_blocks, int *refused);
 /* Diagnostic entry, not needed to align files: the reads and headers mgb_align_fastx_text aligns for the same
  * arguments, without aligning them, so that the device parser can be checked against the host restatement and either
  * parser can be timed on its own. device_route = 1:

@@ -95,6 +95,14 @@ def load_library(path=None):
     L.mgb_align_fastx_batch_text.argtypes = [vp, ctypes.POINTER(mgb_config_t), vp, i, ctypes.POINTER(vp)]
     L.mgb_fastx_batch_free.restype = None
     L.mgb_fastx_batch_free.argtypes = [vp]
+    L.mgb_fastx_stage_bgzf.restype = i
+    L.mgb_fastx_stage_bgzf.argtypes = [vp, vp, u64, vp, u64, i, u64, cp, i, ctypes.POINTER(u64), ctypes.POINTER(i),
+                                       ctypes.POINTER(u64), ctypes.POINTER(i), ctypes.POINTER(vp)]
+    L.mgb_fastx_batch_tail.restype = i
+    L.mgb_fastx_batch_tail.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(u64)]
+    L.mgb_bgzf_inflate.restype = i
+    L.mgb_bgzf_inflate.argtypes = [vp, vp, u64, i, vp, u64, ctypes.POINTER(u64), ctypes.POINTER(u64),
+                                   ctypes.POINTER(u64), ctypes.POINTER(i)]
     L.mgb_fastx_parse.restype = i
     L.mgb_fastx_parse.argtypes = [vp, vp, u64, i, cp, i, i, vp, u64, vp, vp, u64, vp, u64, ctypes.POINTER(u64),
                                   ctypes.POINTER(u64), ctypes.POINTER(i), ctypes.POINTER(i)]
@@ -148,7 +156,8 @@ REQUIRED_SYMBOLS = [
     "mgb_results_export", "mgb_results_import", "mgb_boss_build", "mgb_boss_free",
     "mgb_boss_mask_dummy", "mgb_set_pipeline_pieces", "mgb_set_host_threads", "mgb_dbg_load", "mgb_dbg_last_error", "mgb_boss_last_error", "mgb_config_check", "mgb_dbg_load_suffix_ranges", "mgb_dbg_free_suffix_ranges", "mgb_index_set_mode",
     "mgb_align_batch_text", "mgb_results_text", "mgb_align_fastx_text", "mgb_fastx_parse", "mgb_index_replicate",
-    "mgb_fastx_stage", "mgb_align_fastx_batch_text", "mgb_fastx_batch_free",
+    "mgb_fastx_stage", "mgb_align_fastx_batch_text", "mgb_fastx_batch_free", "mgb_fastx_stage_bgzf",
+    "mgb_fastx_batch_tail", "mgb_bgzf_inflate",
 ]
 MGB_TEXT_TSV, MGB_TEXT_JSON = 1, 2
 MGB_FASTX_FWD_AND_REVERSE = 1

@@ -543,12 +543,52 @@ class B200Aligner:
     def free_staged(self, batch):
         self._L.mgb_fastx_batch_free(batch)
 
+    def stage_fastx_bgzf(self, head, cbuf, c_eof, max_text, comment_delim=None, fwd_and_reverse=False):
+        """mgb_fastx_stage_bgzf: stages the text `head` followed by the text of the complete BGZF blocks at the start of
+        cbuf (bytes), inflated on the device until their text reaches max_text. Returns (batch, c_consumed, c_refused,
+        consumed, ended, tail): compressed bytes taken, whether the member after them is left to the host, the text
+        consumed and ended as stage_fastx returns them, and the text after the last complete record, as bytes."""
+        hbuf = _as_bytes(head)
+        cb = np.frombuffer(cbuf, np.uint8) if isinstance(cbuf, (bytes, bytearray, memoryview)) else cbuf
+        batch, c_consumed, c_refused = ctypes.c_void_p(), ctypes.c_uint64(), ctypes.c_int()
+        consumed, ended = ctypes.c_uint64(), ctypes.c_int()
+        flags = _lib.MGB_FASTX_FWD_AND_REVERSE if fwd_and_reverse else 0
+        delim = None if comment_delim is None else _as_bytes(comment_delim)
+        _lib.check(self._L, self._L.mgb_fastx_stage_bgzf(
+            self.graph.handle, hbuf, len(hbuf), cb.ctypes.data, len(cb), int(bool(c_eof)), int(max_text), delim, flags,
+            ctypes.byref(c_consumed), ctypes.byref(c_refused), ctypes.byref(consumed), ctypes.byref(ended),
+            ctypes.byref(batch)))
+        p, n = ctypes.c_void_p(), ctypes.c_uint64()
+        try:
+            _lib.check(self._L, self._L.mgb_fastx_batch_tail(batch, ctypes.byref(p), ctypes.byref(n)))
+            tail = bytes((ctypes.c_char * n.value).from_address(p.value)) if n.value else b""
+        except BaseException:
+            self.free_staged(batch)
+            raise
+        return batch, c_consumed.value, bool(c_refused.value), consumed.value, bool(ended.value), tail
+
     def align(self, query):
         return self.align_batch([("", query)])[0]
 
 
 def _as_bytes(x):
     return x.encode("latin1") if isinstance(x, str) else bytes(x)
+
+
+def bgzf_inflate(index, cbuf, c_eof=True):
+    """mgb_bgzf_inflate: the text of the complete BGZF blocks at the start of cbuf (bytes), inflated on index's device.
+    Returns (text, c_consumed, n_blocks, refused)."""
+    from . import bgzf
+    L = index._L
+    cbuf = bytes(cbuf)
+    cb = np.frombuffer(cbuf, np.uint8) if cbuf else np.zeros(1, np.uint8)
+    cap = bgzf.text_of(cbuf)[0] + 1
+    out = np.zeros(cap, np.uint8)
+    n, c_consumed, n_blocks, refused = ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_int()
+    _lib.check(L, L.mgb_bgzf_inflate(index.handle, cb.ctypes.data, len(cbuf), int(bool(c_eof)), out.ctypes.data, cap,
+                                     ctypes.byref(n), ctypes.byref(c_consumed), ctypes.byref(n_blocks),
+                                     ctypes.byref(refused)))
+    return out[:n.value].tobytes(), c_consumed.value, n_blocks.value, bool(refused.value)
 
 
 def parse_fastx(buf, at_eof=True, comment_delim=None, fwd_and_reverse=False, index=None, lib=None):

@@ -7,6 +7,11 @@ the device and only the text comes back. A thread reads the next chunk while the
 (mgb_fastx_stage: parse, and learn where its records end), hands the rest of the buffer on to the next worker and then
 aligns its batch while the next chunk is staged. Output is in input order either way, the same bytes for any worker
 list, and one of the orders the reference's thread pool can print.
+
+A .gz/.bgz file whose first member is a BGZF block (htslib's bgzip) goes up compressed: each stage inflates its
+blocks on the device (mgb_fastx_stage_bgzf) into the text it parses. From the first member the device route does not
+serve on, the rest of the file is read by Python's gzip and takes the text route, so every file that is BGZF only in
+part gives the bytes, or the error, it gives on the gzip route.
 """
 import argparse
 import gzip
@@ -15,6 +20,7 @@ import queue
 import sys
 import threading
 
+from . import bgzf
 from .config import SIZE_MAX, cli_defaults, dna_scoring_matrix
 
 CHUNK_BYTES = 64 << 20
@@ -169,6 +175,8 @@ class _Chunks:
 
 def align_file(aligner, path, out, json=False, comment_delim=None, fwd_and_reverse=False, chunk_bytes=CHUNK_BYTES):
     """aligns one file and writes its text to `out`, chunk by chunk; returns the number of bytes written"""
+    if path.endswith((".gz", ".bgz")) and bgzf.is_bgzf(path):
+        return align_file_workers([aligner], path, out, json, comment_delim, fwd_and_reverse, chunk_bytes)
     opener = gzip.open if path.endswith((".gz", ".bgz")) else open
     written = 0
     with opener(path, "rb") as f:
@@ -199,6 +207,95 @@ def align_file(aligner, path, out, json=False, comment_delim=None, fwd_and_rever
     return written
 
 
+class _Token:
+    """What passes from one stage to the next, held by one worker at a time: the text not yet consumed (`pending`) and
+    the grow rule's `want`; on the BGZF route also the compressed bytes read but not yet staged (`cpend`, which
+    starts at file offset `c_at`)."""
+
+    def __init__(self, path, chunk_bytes):
+        self.path, self.size = path, chunk_bytes
+        self.pending, self.at_eof, self.want = b"", False, 0
+        self.raw = path.endswith((".gz", ".bgz")) and bgzf.is_bgzf(path)
+        self.cpend, self.c_at = b"", 0
+        self.files = [open(path, "rb") if self.raw else (gzip.open if path.endswith((".gz", ".bgz")) else open)(path, "rb")]
+        self.chunks = _Chunks(self.files[0], chunk_bytes)
+
+    def _read(self):
+        nxt = self.chunks.next()
+        self.at_eof = not nxt
+        return nxt
+
+    def stage(self, al, halted, comment_delim, fwd_and_reverse):
+        """reads and stages the next chunk: (batch, last), batch None when there is nothing left to stage; last: no
+        stage follows this one"""
+        if self.raw:
+            return self._stage_bgzf(al, halted, comment_delim, fwd_and_reverse)
+        pending, want = self.pending, self.want
+        while not self.at_eof and not halted():
+            nxt = self._read()
+            pending = pending + nxt if pending else nxt
+            if len(pending) >= want:
+                break
+        if halted() or not pending:
+            return None, True
+        batch, consumed, ended = al.stage_fastx(pending, self.at_eof, comment_delim, fwd_and_reverse)
+        if ended or self.at_eof:
+            return batch, True
+        self.want = 2 * len(pending) if consumed == 0 else 0
+        self.pending = pending[consumed:]
+        return batch, False
+
+    def _stage_bgzf(self, al, halted, comment_delim, fwd_and_reverse):
+        # at most chunk_bytes of text from blocks (or, after a stage with no complete record, as much text as that
+        # stage held, so the next one holds twice as much), plus one block, plus the tail
+        max_text = max(self.size, self.want)
+        while not self.at_eof and not halted():
+            text, other = bgzf.text_of(self.cpend, max_text)
+            if text >= max_text or other:
+                break
+            nxt = self._read()
+            self.cpend = self.cpend + nxt if self.cpend else nxt
+        if halted():
+            return None, True
+        batch, c_used, c_refused, consumed, ended, tail = al.stage_fastx_bgzf(
+            self.pending, self.cpend, self.at_eof, max_text, comment_delim, fwd_and_reverse)
+        self.cpend, self.c_at = self.cpend[c_used:], self.c_at + c_used
+        if ended:
+            return batch, True
+        if c_refused:
+            self._hand_over(tail)
+            return batch, False
+        if self.at_eof and not self.cpend:
+            return batch, True
+        self.want = len(tail) if consumed == 0 else 0
+        self.pending = tail
+        return batch, False
+
+    def _hand_over(self, tail):
+        """the rest of the file, from the member at c_at on, through Python's gzip onto the text route; zero bytes
+        after a member are skipped as gzip skips them"""
+        self.chunks.close()
+        f = open(self.path, "rb")
+        self.files.append(f)
+        f.seek(self.c_at)
+        while True:
+            b = f.read(1 << 16)
+            z = len(b) - len(b.lstrip(b"\0"))
+            if z < len(b) or not b:
+                f.seek(self.c_at + z)
+                break
+            self.c_at += len(b)
+        gz = gzip.GzipFile(fileobj=f, mode="rb")
+        self.files.append(gz)
+        self.chunks = _Chunks(gz, self.size)
+        self.raw, self.pending, self.at_eof, self.want, self.cpend = False, tail, False, 0, b""
+
+    def close(self):
+        self.chunks.close()
+        for f in reversed(self.files):
+            f.close()
+
+
 def align_file_workers(aligners, path, out, json=False, comment_delim=None, fwd_and_reverse=False,
                        chunk_bytes=CHUNK_BYTES):
     """align_file with one worker thread per aligner; the same bytes go to `out`. Chunk i is staged by worker i mod W,
@@ -207,9 +304,8 @@ def align_file_workers(aligners, path, out, json=False, comment_delim=None, fwd_
     next. The first error stops every worker and the reader: nothing after the last text in order is written, every
     staged batch is freed, every thread is joined, and the error is raised here."""
     W = len(aligners)
-    opener = gzip.open if path.endswith((".gz", ".bgz")) else open
     cv = threading.Condition()
-    st = dict(turn=0, pending=b"", at_eof=False, want=0, n_chunks=None, next_out=0, error=None, stop=False)
+    st = dict(turn=0, n_chunks=None, next_out=0, error=None, stop=False)
     texts = {}
 
     def halted():
@@ -221,7 +317,7 @@ def align_file_workers(aligners, path, out, json=False, comment_delim=None, fwd_
                 st["error"] = e
             cv.notify_all()
 
-    def worker(w, al, chunks):
+    def worker(w, al, token):
         i = w
         try:
             while True:
@@ -231,27 +327,17 @@ def align_file_workers(aligners, path, out, json=False, comment_delim=None, fwd_
                     if halted() or st["n_chunks"] is not None:
                         return
                 # this worker holds the token: it alone reads and stages until it hands the token on
-                pending, at_eof, want = st["pending"], st["at_eof"], st["want"]
-                while not at_eof and not halted():
-                    nxt = chunks.next()
-                    at_eof = not nxt
-                    pending = pending + nxt if pending else nxt
-                    if len(pending) >= want:
-                        break
-                if halted():
+                batch, last = token.stage(al, halted, comment_delim, fwd_and_reverse)
+                if halted() and batch is None:
                     return
-                if not pending:
+                if batch is None:
                     with cv:
                         st["n_chunks"] = i
                         cv.notify_all()
                     return
-                batch, consumed, ended = al.stage_fastx(pending, at_eof, comment_delim, fwd_and_reverse)
                 with cv:
-                    if ended or at_eof:
+                    if last:
                         st["n_chunks"] = i + 1
-                    else:
-                        st["want"] = 2 * len(pending) if consumed == 0 else 0
-                        st["pending"], st["at_eof"] = pending[consumed:], at_eof
                     st["turn"] = i + 1
                     cv.notify_all()
                     stop = halted()
@@ -267,34 +353,33 @@ def align_file_workers(aligners, path, out, json=False, comment_delim=None, fwd_
             failed(e)
 
     written = 0
-    with opener(path, "rb") as f:
-        chunks = _Chunks(f, chunk_bytes)
-        threads = []
-        try:
-            for w, al in enumerate(aligners):
-                threads.append(threading.Thread(target=worker, args=(w, al, chunks)))
-                threads[-1].start()
-            while True:
-                with cv:
-                    cv.wait_for(lambda: st["error"] is not None or st["next_out"] in texts
-                                or st["n_chunks"] == st["next_out"])
-                    if st["error"] is not None or st["n_chunks"] == st["next_out"]:
-                        break
-                    text = texts.pop(st["next_out"])
-                out.write(text)
-                written += len(text)
-                with cv:
-                    st["next_out"] += 1
-                    cv.notify_all()
-        except BaseException as e:
-            failed(e)
-        finally:
+    token = _Token(path, chunk_bytes)
+    threads = []
+    try:
+        for w, al in enumerate(aligners):
+            threads.append(threading.Thread(target=worker, args=(w, al, token)))
+            threads[-1].start()
+        while True:
             with cv:
-                st["stop"] = True
+                cv.wait_for(lambda: st["error"] is not None or st["next_out"] in texts
+                            or st["n_chunks"] == st["next_out"])
+                if st["error"] is not None or st["n_chunks"] == st["next_out"]:
+                    break
+                text = texts.pop(st["next_out"])
+            out.write(text)
+            written += len(text)
+            with cv:
+                st["next_out"] += 1
                 cv.notify_all()
-            for t in threads:
-                t.join()
-            chunks.close()
+    except BaseException as e:
+        failed(e)
+    finally:
+        with cv:
+            st["stop"] = True
+            cv.notify_all()
+        for t in threads:
+            t.join()
+        token.close()
     if st["error"] is not None:
         raise st["error"]
     return written

@@ -57,6 +57,7 @@ static void parallel_copy(char *dst, const char *src, uint64_t n) {
 #include "kernels.cuh"
 #include "format_core.cuh"
 #include "fastx_core.cuh"
+#include "bgzf_core.cuh"
 #include "fastx_host.hpp"
 #include "host_common.hpp"
 #include "index_build.hpp"
@@ -1304,30 +1305,35 @@ int scan_u64(uint64_t *off, uint32_t n, Stream &st, DevBufs &bufs) {
     return 0;
 }
 
-int fastx_parse_dev(const mgb_index_t *index, const char *buf, uint64_t bytes, bool at_eof, const char *delim,
-                    bool fwd_rev, Stream &st, DevBufs &bufs, FastxDev *out, mgb_stats_t *stats) {
-    if (bytes >= 0xffffffffull || (delim && std::strlen(delim) > kFastxMaxDelim)) { out->refused = true; return 0; }
+// the chunk's text in device memory: fastx_text_bytes(bytes) bytes, the chunk at the front
+inline uint64_t fastx_text_bytes(uint64_t bytes) { return (bytes + kFastxTile - 1) / kFastxTile * kFastxTile + 16; }
+
+// whether the device route takes a chunk of this size and delimiter at all
+inline bool fastx_dev_takes(uint64_t bytes, const char *delim) {
+    return bytes < 0xffffffffull && (!delim || std::strlen(delim) <= kFastxMaxDelim);
+}
+
+// the records of the chunk d_buf[0, bytes) (device memory of fastx_text_bytes(bytes) bytes, last: its last byte)
+int fastx_parse_text(const mgb_index_t *index, const uint8_t *d_buf, uint64_t bytes, uint8_t last, bool at_eof,
+                     const char *delim, bool fwd_rev, Stream &st, DevBufs &bufs, FastxDev *out, mgb_stats_t *stats) {
+    if (!fastx_dev_takes(bytes, delim)) { out->refused = true; return 0; }
     int rc;
     FastxArgs a;
     std::memset(&a, 0, sizeof(a));
     a.n = (uint32_t)bytes; a.at_eof = at_eof; a.fwd_rev = fwd_rev;
     a.n_tiles = (uint32_t)((bytes + kFastxTile - 1) / kFastxTile);
     if (delim) { a.has_delim = 1; a.dlen = (uint32_t)std::strlen(delim); std::memcpy(a.delim, delim, a.dlen); }
-    uint8_t *d_buf = nullptr;
-    if ((rc = bufs.alloc(&d_buf, (size_t)a.n_tiles * kFastxTile + 16))) return rc;
     if ((rc = bufs.alloc(&a.tile_nl, (size_t)a.n_tiles + 1))) return rc;
     if ((rc = bufs.alloc(&a.sum, 1))) return rc;
-    if (bytes && (rc = h2d(d_buf, buf, bytes, st))) return rc;
     if ((rc = dev_zero(a.sum, sizeof(FastxSummary), st))) return rc;
     a.buf = d_buf;
-    stats->h2d_bytes += bytes;
     [[maybe_unused]] const unsigned tiles_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(a.n_tiles, (uint64_t)index->num_sms * 8));
     // line ends
     uint64_t n_nl = 0;
 #if defined(MGB_HOST_EMU)
     for (uint32_t t = 0; t < a.n_tiles; ++t) {
         uint64_t c = 0;
-        for (uint32_t i = t * kFastxTile; i < a.n && i < (t + 1) * kFastxTile; ++i) c += buf[i] == '\n';
+        for (uint32_t i = t * kFastxTile; i < a.n && i < (t + 1) * kFastxTile; ++i) c += a.buf[i] == '\n';
         a.tile_nl[t] = c;
     }
 #else
@@ -1339,7 +1345,7 @@ int fastx_parse_dev(const mgb_index_t *index, const char *buf, uint64_t bytes, b
     if ((rc = scan_u64(a.tile_nl, a.n_tiles, st, bufs))) return rc;
     if ((rc = d2h(&n_nl, a.tile_nl + a.n_tiles, 8, st)) || (rc = sync(st))) return rc;
     a.n_nl = (uint32_t)n_nl;
-    a.n_lines = a.n_nl + (bytes && buf[bytes - 1] != '\n' ? 1 : 0);
+    a.n_lines = a.n_nl + (bytes && last != '\n' ? 1 : 0);
     if ((rc = bufs.alloc(&a.nl, (size_t)a.n_nl + 1))) return rc;
     [[maybe_unused]] const unsigned lines_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)a.n_lines + 255) / 256,
                                                                                    (uint64_t)index->num_sms * 8));
@@ -1348,7 +1354,7 @@ int fastx_parse_dev(const mgb_index_t *index, const char *buf, uint64_t bytes, b
 #if defined(MGB_HOST_EMU)
     {
         uint64_t o = 0;
-        for (uint32_t i = 0; i < a.n; ++i) if (buf[i] == '\n') a.nl[o++] = i;
+        for (uint32_t i = 0; i < a.n; ++i) if (a.buf[i] == '\n') a.nl[o++] = i;
         a.nl[a.n_nl] = a.n;
         for (uint32_t i = 0; i < a.n_lines; ++i) {
             bool hdr;
@@ -1420,6 +1426,124 @@ int fastx_parse_dev(const mgb_index_t *index, const char *buf, uint64_t bytes, b
     if ((rc = d2h(out->offsets.data(), a.offsets, (n_out + 1) * 8, st))) return rc;
     if ((rc = d2h(out->name_offsets.data(), a.name_offsets, (n_out + 1) * 8, st)) || (rc = sync(st))) return rc;
     stats->d2h_bytes += 16 * (n_out + 1);
+    return 0;
+}
+
+// the chunk buf[0, bytes) (host memory) uploaded and parsed
+int fastx_parse_dev(const mgb_index_t *index, const char *buf, uint64_t bytes, bool at_eof, const char *delim,
+                    bool fwd_rev, Stream &st, DevBufs &bufs, FastxDev *out, mgb_stats_t *stats) {
+    if (!fastx_dev_takes(bytes, delim)) { out->refused = true; return 0; }
+    uint8_t *d_buf = nullptr;
+    int rc;
+    if ((rc = bufs.alloc(&d_buf, fastx_text_bytes(bytes)))) return rc;
+    if (bytes && (rc = h2d(d_buf, buf, bytes, st))) return rc;
+    stats->h2d_bytes += bytes;
+    return fastx_parse_text(index, d_buf, bytes, bytes ? (uint8_t)buf[bytes - 1] : 0, at_eof, delim, fwd_rev, st, bufs,
+                            out, stats);
+}
+
+// ---------------------------------------------------------------------------------------
+// BGZF input (mgb_fastx_stage_bgzf, mgb_bgzf_inflate): the blocks of a compressed buffer listed on the host from their
+// headers, and inflated on the device (bgzf_core.cuh) into the text the parser reads
+// ---------------------------------------------------------------------------------------
+inline uint32_t rd16(const uint8_t *p) { return p[0] | (uint32_t)p[1] << 8; }
+inline uint32_t rd32(const uint8_t *p) { return rd16(p) | rd16(p + 2) << 16; }
+
+struct BgzfWalk {
+    std::vector<BgzfBlock> blocks;
+    uint64_t c_end = 0;      // compressed bytes of the blocks
+    uint64_t text = 0;       // their text (the sum of ISIZE)
+    bool refused = false;    // the member at c_end is not a BGZF block (or is cut off by the end of the input)
+    std::vector<uint64_t> member;      // where each block's member starts
+};
+
+// The complete BGZF blocks at the start of c[0, n), until their text reaches max_text. A member is a BGZF block when its
+// header is ID1 ID2 CM FLG = 31 139 8 4 (FEXTRA only), its extra field holds a BC subfield of SLEN 2 (BSIZE; other
+// subfields are skipped) and ISIZE <= 64 KiB. One header per block is read.
+void bgzf_walk(const uint8_t *c, uint64_t n, bool c_eof, uint64_t max_text, BgzfWalk *w) {
+    uint64_t at = 0;
+    while (w->text < max_text && at < n) {
+        const uint8_t *h = c + at;
+        const uint64_t left = n - at;
+        if (left < 12) { w->refused = c_eof; break; }
+        if (h[0] != 31 || h[1] != 139 || h[2] != 8 || h[3] != 4) { w->refused = true; break; }
+        const uint32_t xlen = rd16(h + 10);
+        if (left < 12 + (uint64_t)xlen) { w->refused = c_eof; break; }
+        int64_t bsize = -1;
+        uint32_t p = 0;
+        while (p + 4 <= xlen) {
+            const uint32_t slen = rd16(h + 12 + p + 2);
+            if (slen > xlen - p - 4) break;
+            if (h[12 + p] == 'B' && h[12 + p + 1] == 'C' && slen == 2) bsize = rd16(h + 12 + p + 4);
+            p += 4 + slen;
+        }
+        const uint64_t size = (uint64_t)bsize + 1;
+        if (p != xlen || bsize < 0 || size < 12 + (uint64_t)xlen + 8) { w->refused = true; break; }
+        if (left < size) { w->refused = c_eof; break; }
+        const uint32_t isize = rd32(h + size - 4);
+        if (isize > kBgzfMaxText) { w->refused = true; break; }
+        BgzfBlock b;
+        b.c_off = at + 12 + xlen; b.t_off = w->text;
+        b.c_len = (uint32_t)(size - 12 - xlen - 8); b.crc = rd32(h + size - 8); b.isize = isize; b.pad = 0;
+        w->blocks.push_back(b);
+        w->member.push_back(at);
+        w->text += isize;
+        at += size;
+    }
+    w->c_end = at;
+}
+
+// The blocks of w inflated on the device after head[0, head_bytes): *d_text (device memory of
+// fastx_text_bytes(*text_bytes) bytes) holds the head and the text of the blocks before the first one the device
+// refuses; *n_ok: those blocks. The last byte of the text is in *last.
+int bgzf_inflate_dev(const mgb_index_t *index, const uint8_t *cbuf, BgzfWalk &w, const char *head, uint64_t head_bytes,
+                     Stream &st, DevBufs &bufs, uint8_t **d_text, uint64_t *text_bytes, uint64_t *n_ok, uint8_t *last,
+                     mgb_stats_t *stats) {
+    (void)index;
+    const uint64_t n = w.blocks.size();
+    if (n > 0xffffffffull) return fail(MGB_ERR_OVERFLOW, "more than 2^32 - 1 BGZF blocks in one call");
+    int rc;
+    BgzfArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.n_blocks = (uint32_t)n;
+    if ((rc = bufs.alloc(d_text, fastx_text_bytes(head_bytes + w.text)))) return rc;
+    if (head_bytes && (rc = h2d(*d_text, head, head_bytes, st))) return rc;
+    stats->h2d_bytes += head_bytes;
+    std::vector<uint32_t> status(n, 0);
+    if (n) {
+        uint8_t *d_c = nullptr;
+        BgzfBlock *d_blocks = nullptr;
+        if ((rc = bufs.alloc(&d_c, w.c_end)) || (rc = bufs.alloc(&d_blocks, n)) || (rc = bufs.alloc(&a.status, n)))
+            return rc;
+        if ((rc = h2d(d_c, cbuf, w.c_end, st)) || (rc = h2d(d_blocks, w.blocks.data(), n * sizeof(BgzfBlock), st)))
+            return rc;
+        stats->h2d_bytes += w.c_end + n * sizeof(BgzfBlock);
+        a.cbuf = d_c; a.blocks = d_blocks; a.text = *d_text + head_bytes;
+#if defined(MGB_HOST_EMU)
+        BgzfShared sh;
+        bgzf_crc_table(sh);
+        for (uint32_t b = 0; b < a.n_blocks; ++b) bgzf_inflate_block(a, b, sh);
+#else
+        const unsigned grid = (unsigned)std::min<uint64_t>((n + kBgzfWarps - 1) / kBgzfWarps, (uint64_t)index->num_sms * 16);
+        k_bgzf_inflate<<<grid, 32 * kBgzfWarps, 0, st.s>>>(a);
+        CUDA_TRY(cudaGetLastError());
+#endif
+        stats->kernel_launches += 1;
+        if ((rc = d2h(status.data(), a.status, n * 4, st)) || (rc = sync(st))) return rc;
+        stats->d2h_bytes += n * 4;
+    }
+    uint64_t ok = 0;
+    while (ok < n && status[ok] == kBgzfOk) ++ok;
+    if (ok < n) { w.c_end = w.member[ok]; w.refused = true; }
+    *n_ok = ok;
+    *text_bytes = head_bytes + (ok < n ? w.blocks[ok].t_off : w.text);
+    *last = 0;
+    if (*text_bytes > head_bytes) {
+        if ((rc = d2h(last, *d_text + *text_bytes - 1, 1, st)) || (rc = sync(st))) return rc;
+        stats->d2h_bytes += 1;
+    } else if (head_bytes) {
+        *last = (uint8_t)head[head_bytes - 1];
+    }
     return 0;
 }
 
@@ -2352,13 +2476,16 @@ static int fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes
 
 // A chunk's records between mgb_fastx_stage and mgb_align_fastx_batch_text: the stage's workspace (its "batch" region
 // holds the parsed arrays on the device) and stream, the host restatement's records for a refused chunk, and the
-// parse's own copies and launches, which the result set reports.
+// parse's own copies and launches, which the result set reports. A BGZF stage also keeps the text the host holds: the
+// whole text when the host restatement parsed it, else text[consumed, end); the tail starts at tail_at.
 struct mgb_fastx_batch {
     CallWorkspace cw;
     DevBufs bufs;
     FastxDev dev;
     FastxRecords host;
     mgb_stats_t parse;
+    std::vector<char> text;
+    uint64_t tail_at = 0;
     explicit mgb_fastx_batch(const mgb_index_t *index) : cw(index), bufs(cw.st, cw.w, kBatchSlots) {
         std::memset(&parse, 0, sizeof(parse));
     }
@@ -2403,6 +2530,83 @@ int mgb_align_fastx_batch_text(const mgb_index_t *index, const mgb_config_t *con
 }
 
 void mgb_fastx_batch_free(mgb_fastx_batch_t *batch) { delete batch; }
+
+int mgb_fastx_stage_bgzf(const mgb_index_t *index, const char *head, uint64_t head_bytes, const uint8_t *cbuf,
+                         uint64_t cbytes, int c_eof, uint64_t max_text, const char *comment_delim, int flags,
+                         uint64_t *c_consumed, int *c_refused, uint64_t *consumed, int *ended,
+                         mgb_fastx_batch_t **out) {
+    if (!index || !c_consumed || !c_refused || !consumed || !ended || !out || (!head && head_bytes) || (!cbuf && cbytes))
+        return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (flags & ~MGB_FASTX_FWD_AND_REVERSE) return fail(MGB_ERR_INVALID_ARGUMENT, "unknown flags");
+    const bool fwd_rev = (flags & MGB_FASTX_FWD_AND_REVERSE) != 0;
+    std::unique_ptr<mgb_fastx_batch> b(new mgb_fastx_batch(index));
+    int rc = b->cw.ready();
+    if (rc) return rc;
+    Stream &st = b->cw.st;
+    BgzfWalk w;
+    bgzf_walk(cbuf, cbytes, c_eof != 0, max_text, &w);
+    uint8_t *d_text = nullptr, last = 0;
+    uint64_t text_bytes = 0, n_ok = 0;
+    if ((rc = bgzf_inflate_dev(index, cbuf, w, head, head_bytes, st, b->bufs, &d_text, &text_bytes, &n_ok, &last,
+                               &b->parse)))
+        return rc;
+    const bool at_eof = c_eof && w.c_end == cbytes && !w.refused;
+    *consumed = 0; *ended = 0;
+    if ((rc = fastx_parse_text(index, d_text, text_bytes, last, at_eof, comment_delim, fwd_rev, st, b->bufs, &b->dev,
+                               &b->parse)))
+        return rc;
+    if (b->dev.refused) {            // the host restatement parses the inflated text
+        b->text.resize(text_bytes);
+        if ((text_bytes && (rc = d2h(b->text.data(), d_text, text_bytes, st))) || (rc = sync(st))) return rc;
+        b->parse.d2h_bytes += text_bytes;
+        fastx_parse_host(b->text.data(), text_bytes, at_eof, comment_delim, fwd_rev, &b->host, consumed, ended);
+        b->tail_at = *consumed;
+    } else {
+        *consumed = b->dev.consumed;
+        b->text.resize(text_bytes - *consumed);
+        if ((b->text.size() && (rc = d2h(b->text.data(), d_text + *consumed, b->text.size(), st))) || (rc = sync(st)))
+            return rc;
+        b->parse.d2h_bytes += b->text.size();
+    }
+    const std::vector<uint64_t> &offs = b->dev.refused ? b->host.offsets : b->dev.offsets;
+    if (offs.size() - 1 > 0xffffffffull) return fail(MGB_ERR_OVERFLOW, "more than 2^32 - 1 records in one chunk");
+    *c_consumed = w.c_end;
+    *c_refused = w.refused ? 1 : 0;
+    *out = b.release();
+    return MGB_OK;
+}
+
+int mgb_fastx_batch_tail(const mgb_fastx_batch_t *batch, const char **tail, uint64_t *bytes) {
+    if (!batch || !tail || !bytes) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    *tail = batch->text.data() + batch->tail_at;
+    *bytes = batch->text.size() - batch->tail_at;
+    return MGB_OK;
+}
+
+int mgb_bgzf_inflate(const mgb_index_t *index, const uint8_t *cbuf, uint64_t cbytes, int c_eof, char *out,
+                     uint64_t out_cap, uint64_t *out_bytes, uint64_t *c_consumed, uint64_t *n_blocks, int *refused) {
+    if (!index || (!cbuf && cbytes) || (!out && out_cap) || !out_bytes || !c_consumed || !n_blocks || !refused)
+        return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    CallWorkspace cw(index);
+    int rc = cw.ready();
+    if (rc) return rc;
+    DevBufs bufs(cw.st, cw.w, kBatchSlots);
+    mgb_stats_t stats;
+    std::memset(&stats, 0, sizeof(stats));
+    BgzfWalk w;
+    bgzf_walk(cbuf, cbytes, c_eof != 0, UINT64_MAX, &w);
+    uint8_t *d_text = nullptr, last = 0;
+    uint64_t text_bytes = 0, n_ok = 0;
+    if ((rc = bgzf_inflate_dev(index, cbuf, w, nullptr, 0, cw.st, bufs, &d_text, &text_bytes, &n_ok, &last, &stats)))
+        return rc;
+    if (text_bytes > out_cap) return fail(MGB_ERR_OVERFLOW, "output buffer too small");
+    if ((text_bytes && (rc = d2h(out, d_text, text_bytes, cw.st))) || (rc = sync(cw.st))) return rc;
+    *out_bytes = text_bytes;
+    *c_consumed = w.c_end;
+    *n_blocks = n_ok;
+    *refused = w.refused ? 1 : 0;
+    return MGB_OK;
+}
 
 int mgb_align_fastx_text(const mgb_index_t *index, const mgb_config_t *config, const char *buf, uint64_t bytes,
                          int at_eof, const char *comment_delim, int flags, int format, uint64_t *consumed, int *ended,
