@@ -254,7 +254,7 @@ int mgb_fastx_stage_bgzf(const mgb_index_t *index, const char *head, uint64_t he
                          uint64_t cbytes, int c_eof, uint64_t max_text, const char *comment_delim, int flags,
                          uint64_t *c_consumed, int *c_refused, uint64_t *consumed, int *ended,
                          mgb_fastx_batch_t **out);
-/* text[consumed, end) of a batch staged by mgb_fastx_stage_bgzf, owned by the batch (valid until it is aligned or
+/* text[consumed, end) of a batch staged by mgb_fastx_stage_bgzf or mgb_fastx_stage_gzip, owned by the batch (valid until it is aligned or
  * freed); empty for a batch of mgb_fastx_stage */
 int mgb_fastx_batch_tail(const mgb_fastx_batch_t *batch, const char **tail, uint64_t *bytes);
 /* Diagnostic entry, as mgb_fastx_parse is: the complete BGZF blocks of cbuf inflated on index's device and downloaded
@@ -262,6 +262,37 @@ int mgb_fastx_batch_tail(const mgb_fastx_batch_t *batch, const char **tail, uint
  * mgb_fastx_stage_bgzf. */
 int mgb_bgzf_inflate(const mgb_index_t *index, const uint8_t *cbuf, uint64_t cbytes, int c_eof, char *out,
                      uint64_t out_cap, uint64_t *out_bytes, uint64_t *c_consumed, uint64_t *n_blocks, int *refused);
+/* Plain gzip input (RFC 1952 members, as gzip and pigz write them). A stream holds, in host memory, where the next
+ * stage starts and the state of the member it is in: the bit position, the member's last 32 KiB of text and its running
+ * CRC32 and length. Any device may stage the next part of a stream. mgb_gzip_stream_state: *in_member = 1 while the
+ * stream is inside a member, and *member_text = that member's text staged so far (0 between members). */
+typedef struct mgb_gzip_stream mgb_gzip_stream_t;
+int mgb_gzip_stream_create(mgb_gzip_stream_t **out);
+void mgb_gzip_stream_free(mgb_gzip_stream_t *stream);
+int mgb_gzip_stream_state(const mgb_gzip_stream_t *stream, int *in_member, uint64_t *member_text);
+/* mgb_fastx_stage_bgzf for plain gzip input. cbuf holds the stream's next bytes (its first byte partly decoded when
+ * the stream is inside a member). Stages `head` followed by the text of the stream, inflated on index's device, up to
+ * the last DEFLATE block boundary it confirmed once the text reaches max_text, or up to the member's end, where the
+ * CRC32 and ISIZE are checked. A stage never runs past a member's end; the next member's header is read by the next
+ * call. *c_consumed: whole bytes of cbuf taken (the stream keeps the bit offset into the next one). *c_refused = 1: the
+ * stream at this point is left to the caller, and nothing of it was staged in this call (the stream is unchanged): the
+ * member header is not one this route serves (not gzip, not DEFLATE, reserved flags), the bytes after a member are
+ * not a member, the stream is invalid, a trailer does not match, the input ends inside a member (c_eof), or a member's
+ * first stage could not be split (stored or fixed-Huffman blocks only). *c_consumed = 0 without a refusal: the call
+ * needs more compressed bytes to make progress. Records are parsed with at_eof = c_eof, every byte taken and the
+ * stream between members. */
+int mgb_fastx_stage_gzip(const mgb_index_t *index, mgb_gzip_stream_t *stream, const char *head, uint64_t head_bytes,
+                         const uint8_t *cbuf, uint64_t cbytes, int c_eof, uint64_t max_text, const char *comment_delim,
+                         int flags, uint64_t *c_consumed, int *c_refused, uint64_t *consumed, int *ended,
+                         mgb_fastx_batch_t **out);
+/* Diagnostic entry: the gzip members of cbuf inflated on index's device, stage after stage, until the input ends or a
+ * stage refuses (*refused, *c_consumed as in mgb_fastx_stage_gzip). sub_bytes: compressed bytes per sub-range (0: the
+ * default). cands (n_cands bit offsets in cbuf, or NULL): the candidate block starts, in place of the finder's. counts:
+ * sub-ranges, candidates found at or before the end of the text they staged, and candidates confirmed, over all
+ * stages. *out_bytes: the text's length, also when it does not fit out_cap (MGB_ERR_OVERFLOW). */
+int mgb_gzip_inflate(const mgb_index_t *index, const uint8_t *cbuf, uint64_t cbytes, int c_eof, uint64_t sub_bytes,
+                     const uint64_t *cands, uint64_t n_cands, char *out, uint64_t out_cap, uint64_t *out_bytes,
+                     uint64_t *c_consumed, int *refused, uint64_t *counts);
 /* Diagnostic entry, not needed to align files: the reads and headers mgb_align_fastx_text aligns for the same
  * arguments, without aligning them, so that the device parser can be checked against the host restatement and either
  * parser can be timed on its own. device_route = 1:

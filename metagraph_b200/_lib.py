@@ -103,6 +103,18 @@ def load_library(path=None):
     L.mgb_bgzf_inflate.restype = i
     L.mgb_bgzf_inflate.argtypes = [vp, vp, u64, i, vp, u64, ctypes.POINTER(u64), ctypes.POINTER(u64),
                                    ctypes.POINTER(u64), ctypes.POINTER(i)]
+    L.mgb_gzip_stream_create.restype = i
+    L.mgb_gzip_stream_create.argtypes = [ctypes.POINTER(vp)]
+    L.mgb_gzip_stream_free.restype = None
+    L.mgb_gzip_stream_free.argtypes = [vp]
+    L.mgb_gzip_stream_state.restype = i
+    L.mgb_gzip_stream_state.argtypes = [vp, ctypes.POINTER(i), ctypes.POINTER(u64)]
+    L.mgb_fastx_stage_gzip.restype = i
+    L.mgb_fastx_stage_gzip.argtypes = [vp, vp, vp, u64, vp, u64, i, u64, cp, i, ctypes.POINTER(u64), ctypes.POINTER(i),
+                                       ctypes.POINTER(u64), ctypes.POINTER(i), ctypes.POINTER(vp)]
+    L.mgb_gzip_inflate.restype = i
+    L.mgb_gzip_inflate.argtypes = [vp, vp, u64, i, u64, vp, u64, vp, u64, ctypes.POINTER(u64), ctypes.POINTER(u64),
+                                   ctypes.POINTER(i), vp]
     L.mgb_fastx_parse.restype = i
     L.mgb_fastx_parse.argtypes = [vp, vp, u64, i, cp, i, i, vp, u64, vp, vp, u64, vp, u64, ctypes.POINTER(u64),
                                   ctypes.POINTER(u64), ctypes.POINTER(i), ctypes.POINTER(i)]
@@ -157,7 +169,8 @@ REQUIRED_SYMBOLS = [
     "mgb_boss_mask_dummy", "mgb_set_pipeline_pieces", "mgb_set_host_threads", "mgb_dbg_load", "mgb_dbg_last_error", "mgb_boss_last_error", "mgb_config_check", "mgb_dbg_load_suffix_ranges", "mgb_dbg_free_suffix_ranges", "mgb_index_set_mode",
     "mgb_align_batch_text", "mgb_results_text", "mgb_align_fastx_text", "mgb_fastx_parse", "mgb_index_replicate",
     "mgb_fastx_stage", "mgb_align_fastx_batch_text", "mgb_fastx_batch_free", "mgb_fastx_stage_bgzf",
-    "mgb_fastx_batch_tail", "mgb_bgzf_inflate",
+    "mgb_fastx_batch_tail", "mgb_bgzf_inflate", "mgb_gzip_stream_create", "mgb_gzip_stream_free",
+    "mgb_gzip_stream_state", "mgb_fastx_stage_gzip", "mgb_gzip_inflate",
 ]
 MGB_TEXT_TSV, MGB_TEXT_JSON = 1, 2
 MGB_FASTX_FWD_AND_REVERSE = 1

@@ -567,8 +567,52 @@ class B200Aligner:
             raise
         return batch, c_consumed.value, bool(c_refused.value), consumed.value, bool(ended.value), tail
 
+    def stage_fastx_gzip(self, stream, head, cbuf, c_eof, max_text, comment_delim=None, fwd_and_reverse=False):
+        """mgb_fastx_stage_gzip: stages the text `head` followed by the text of the plain gzip stream `stream` (a
+        GzipStream) whose next bytes are cbuf, inflated on the device up to a confirmed block boundary once the text
+        reaches max_text, or to the member's end. Returns what stage_fastx_bgzf returns; c_refused: nothing of the
+        stream was staged and the stream is where it was."""
+        hbuf = _as_bytes(head)
+        cb = np.frombuffer(cbuf, np.uint8) if isinstance(cbuf, (bytes, bytearray, memoryview)) else cbuf
+        batch, c_consumed, c_refused = ctypes.c_void_p(), ctypes.c_uint64(), ctypes.c_int()
+        consumed, ended = ctypes.c_uint64(), ctypes.c_int()
+        flags = _lib.MGB_FASTX_FWD_AND_REVERSE if fwd_and_reverse else 0
+        delim = None if comment_delim is None else _as_bytes(comment_delim)
+        _lib.check(self._L, self._L.mgb_fastx_stage_gzip(
+            self.graph.handle, stream.handle, hbuf, len(hbuf), cb.ctypes.data, len(cb), int(bool(c_eof)),
+            int(max_text), delim, flags, ctypes.byref(c_consumed), ctypes.byref(c_refused), ctypes.byref(consumed),
+            ctypes.byref(ended), ctypes.byref(batch)))
+        p, n = ctypes.c_void_p(), ctypes.c_uint64()
+        try:
+            _lib.check(self._L, self._L.mgb_fastx_batch_tail(batch, ctypes.byref(p), ctypes.byref(n)))
+            tail = bytes((ctypes.c_char * n.value).from_address(p.value)) if n.value else b""
+        except BaseException:
+            self.free_staged(batch)
+            raise
+        return batch, c_consumed.value, bool(c_refused.value), consumed.value, bool(ended.value), tail
+
     def align(self, query):
         return self.align_batch([("", query)])[0]
+
+
+class GzipStream:
+    """mgb_gzip_stream_t: where a plain gzip stream's next stage starts, kept in host memory between stages"""
+
+    def __init__(self, L):
+        self._L = L                 # the library the stages run in
+        self.handle = ctypes.c_void_p()
+        _lib.check(self._L, self._L.mgb_gzip_stream_create(ctypes.byref(self.handle)))
+
+    def state(self):
+        """(inside a member, text of that member staged so far)"""
+        m, t = ctypes.c_int(), ctypes.c_uint64()
+        _lib.check(self._L, self._L.mgb_gzip_stream_state(self.handle, ctypes.byref(m), ctypes.byref(t)))
+        return bool(m.value), t.value
+
+    def close(self):
+        if self.handle:
+            self._L.mgb_gzip_stream_free(self.handle)
+            self.handle = ctypes.c_void_p()
 
 
 def _as_bytes(x):
@@ -589,6 +633,30 @@ def bgzf_inflate(index, cbuf, c_eof=True):
                                      ctypes.byref(n), ctypes.byref(c_consumed), ctypes.byref(n_blocks),
                                      ctypes.byref(refused)))
     return out[:n.value].tobytes(), c_consumed.value, n_blocks.value, bool(refused.value)
+
+
+def gzip_inflate(index, cbuf, c_eof=True, sub_bytes=0, cands=None):
+    """mgb_gzip_inflate: the gzip members of cbuf (bytes) inflated on index's device, with sub-ranges of sub_bytes
+    compressed bytes (0: the default) and, when given, the candidate block starts `cands` (bit offsets in cbuf) in
+    place of the finder's. Returns (text, c_consumed, refused, (sub-ranges, candidates found, candidates confirmed))."""
+    L = index._L
+    cbuf = bytes(cbuf)
+    cb = np.frombuffer(cbuf, np.uint8) if cbuf else np.zeros(1, np.uint8)
+    cd = np.asarray(cands if cands is not None else [0], np.uint64)
+    counts = np.zeros(3, np.uint64)
+    n, c_consumed, refused = ctypes.c_uint64(), ctypes.c_uint64(), ctypes.c_int()
+    cap = 4 * len(cbuf) + 1024
+    while True:
+        out = np.zeros(cap, np.uint8)
+        rc = L.mgb_gzip_inflate(index.handle, cb.ctypes.data, len(cbuf), int(bool(c_eof)), int(sub_bytes),
+                                cd.ctypes.data if cands is not None else None, len(cands) if cands is not None else 0,
+                                out.ctypes.data, cap, ctypes.byref(n), ctypes.byref(c_consumed), ctypes.byref(refused),
+                                counts.ctypes.data)
+        if rc == -5 and n.value > cap:          # MGB_ERR_OVERFLOW: again with room for the whole text
+            cap = n.value
+            continue
+        _lib.check(L, rc)
+        return out[:n.value].tobytes(), c_consumed.value, bool(refused.value), tuple(int(x) for x in counts)
 
 
 def parse_fastx(buf, at_eof=True, comment_delim=None, fwd_and_reverse=False, index=None, lib=None):

@@ -12,6 +12,11 @@ A .gz/.bgz file whose first member is a BGZF block (htslib's bgzip) goes up comp
 blocks on the device (mgb_fastx_stage_bgzf) into the text it parses. From the first member the device route does not
 serve on, the rest of the file is read by Python's gzip and takes the text route, so every file that is BGZF only in
 part gives the bytes, or the error, it gives on the gzip route.
+
+Any other .gz/.bgz file (plain gzip, as gzip and pigz write it) goes up compressed too: each stage inflates part of
+a member on the device (mgb_fastx_stage_gzip), decoding the DEFLATE stream from many points at once. Where the device
+route refuses, the file is reopened at the current member's start with Python's gzip, the text of that member already
+staged is skipped, and the rest takes the text route: the same bytes, or the same error, as Python's gzip.
 """
 import argparse
 import gzip
@@ -173,11 +178,20 @@ class _Chunks:
         self.t.join()
 
 
+def route_of(path):
+    """how a file is read: "plain" (the text as it is), "bgzf" (BGZF blocks inflated on the device), "gzip" (plain
+    gzip inflated on the device) or "host" (Python's gzip, the route both device routes hand a file over to)"""
+    if not path.endswith((".gz", ".bgz")):
+        return "plain"
+    return "bgzf" if bgzf.is_bgzf(path) else "gzip"
+
+
 def align_file(aligner, path, out, json=False, comment_delim=None, fwd_and_reverse=False, chunk_bytes=CHUNK_BYTES):
     """aligns one file and writes its text to `out`, chunk by chunk; returns the number of bytes written"""
-    if path.endswith((".gz", ".bgz")) and bgzf.is_bgzf(path):
+    route = route_of(path)
+    if route in ("bgzf", "gzip"):
         return align_file_workers([aligner], path, out, json, comment_delim, fwd_and_reverse, chunk_bytes)
-    opener = gzip.open if path.endswith((".gz", ".bgz")) else open
+    opener = gzip.open if route == "host" else open
     written = 0
     with opener(path, "rb") as f:
         chunks = _Chunks(f, chunk_bytes)
@@ -209,15 +223,18 @@ def align_file(aligner, path, out, json=False, comment_delim=None, fwd_and_rever
 
 class _Token:
     """What passes from one stage to the next, held by one worker at a time: the text not yet consumed (`pending`) and
-    the grow rule's `want`; on the BGZF route also the compressed bytes read but not yet staged (`cpend`, which
-    starts at file offset `c_at`)."""
+    the grow rule's `want`; on the device routes also the compressed bytes read but not yet staged (`cpend`, which
+    starts at file offset `c_at`), and on the gzip route the stream's state and the compressed bytes a stage is
+    given (`c_want`, doubled after a stage that could not make progress)."""
 
     def __init__(self, path, chunk_bytes):
         self.path, self.size = path, chunk_bytes
         self.pending, self.at_eof, self.want = b"", False, 0
-        self.raw = path.endswith((".gz", ".bgz")) and bgzf.is_bgzf(path)
+        self.route = route_of(path)
+        self.raw = self.route in ("bgzf", "gzip")
         self.cpend, self.c_at = b"", 0
-        self.files = [open(path, "rb") if self.raw else (gzip.open if path.endswith((".gz", ".bgz")) else open)(path, "rb")]
+        self.stream, self.m_at, self.c_want = None, 0, chunk_bytes
+        self.files = [open(path, "rb") if self.raw else (gzip.open if self.route == "host" else open)(path, "rb")]
         self.chunks = _Chunks(self.files[0], chunk_bytes)
 
     def _read(self):
@@ -229,7 +246,8 @@ class _Token:
         """reads and stages the next chunk: (batch, last), batch None when there is nothing left to stage; last: no
         stage follows this one"""
         if self.raw:
-            return self._stage_bgzf(al, halted, comment_delim, fwd_and_reverse)
+            stage = self._stage_bgzf if self.route == "bgzf" else self._stage_gzip
+            return stage(al, halted, comment_delim, fwd_and_reverse)
         pending, want = self.pending, self.want
         while not self.at_eof and not halted():
             nxt = self._read()
@@ -271,29 +289,67 @@ class _Token:
         self.pending = tail
         return batch, False
 
-    def _hand_over(self, tail):
-        """the rest of the file, from the member at c_at on, through Python's gzip onto the text route; zero bytes
-        after a member are skipped as gzip skips them"""
+    def _stage_gzip(self, al, halted, comment_delim, fwd_and_reverse):
+        # at least c_want compressed bytes; the stage takes what max_text of text needs
+        max_text = max(self.size, self.want)
+        while not self.at_eof and len(self.cpend) < self.c_want and not halted():
+            nxt = self._read()
+            self.cpend = self.cpend + nxt if self.cpend else nxt
+        if halted():
+            return None, True
+        if self.stream is None:
+            from .aligner import GzipStream
+            self.stream = GzipStream(al._L)
+        in_member, member_text = self.stream.state()
+        if not in_member:
+            self.m_at = self.c_at
+        batch, c_used, c_refused, consumed, ended, tail = al.stage_fastx_gzip(
+            self.stream, self.pending, self.cpend, self.at_eof, max_text, comment_delim, fwd_and_reverse)
+        self.cpend, self.c_at = self.cpend[c_used:], self.c_at + c_used
+        if ended:
+            return batch, True
+        if c_refused:
+            self._hand_over(tail, self.m_at, member_text)
+            return batch, False
+        if self.at_eof and not self.cpend and not self.stream.state()[0]:
+            return batch, True
+        self.c_want = 2 * max(self.c_want, len(self.cpend)) if c_used == 0 else self.size
+        self.want = len(tail) if consumed == 0 else 0
+        self.pending = tail
+        return batch, False
+
+    def _hand_over(self, tail, at=None, skip=0):
+        """the rest of the file, from the member at `at` (c_at) on, through Python's gzip onto the text route, less
+        the first `skip` bytes of text, which earlier stages took; zero bytes after a member are skipped as gzip skips
+        them"""
         self.chunks.close()
         f = open(self.path, "rb")
         self.files.append(f)
-        f.seek(self.c_at)
+        at = self.c_at if at is None else at
+        f.seek(at)
         while True:
             b = f.read(1 << 16)
             z = len(b) - len(b.lstrip(b"\0"))
             if z < len(b) or not b:
-                f.seek(self.c_at + z)
+                f.seek(at + z)
                 break
-            self.c_at += len(b)
+            at += len(b)
         gz = gzip.GzipFile(fileobj=f, mode="rb")
         self.files.append(gz)
+        while skip > 0:
+            b = gz.read(min(skip, 1 << 24))
+            if not b:
+                break
+            skip -= len(b)
         self.chunks = _Chunks(gz, self.size)
-        self.raw, self.pending, self.at_eof, self.want, self.cpend = False, tail, False, 0, b""
+        self.raw, self.route, self.pending, self.at_eof, self.want, self.cpend = False, "host", tail, False, 0, b""
 
     def close(self):
         self.chunks.close()
         for f in reversed(self.files):
             f.close()
+        if self.stream is not None:
+            self.stream.close()
 
 
 def align_file_workers(aligners, path, out, json=False, comment_delim=None, fwd_and_reverse=False,

@@ -57,7 +57,7 @@ static void parallel_copy(char *dst, const char *src, uint64_t n) {
 #include "kernels.cuh"
 #include "format_core.cuh"
 #include "fastx_core.cuh"
-#include "bgzf_core.cuh"
+#include "gzip_core.cuh"
 #include "fastx_host.hpp"
 #include "host_common.hpp"
 #include "index_build.hpp"
@@ -67,6 +67,17 @@ static void parallel_copy(char *dst, const char *src, uint64_t n) {
 #endif
 
 using namespace mgb;
+
+// A plain gzip stream between stages, in host memory so that the next stage may run on any device: where the next
+// stage starts, and the state of the member it is in (DESIGN.md §8 "Plain gzip input").
+struct mgb_gzip_stream {
+    bool in_member = false;
+    uint32_t bit = 0;                     // bits of the next input's first byte already decoded
+    uint64_t member_text = 0;             // text of the member staged so far (ISIZE is it modulo 2^32)
+    uint32_t crc = 0;                     // its CRC32
+    std::vector<uint8_t> window = std::vector<uint8_t>(kGzipWindow, 0);   // its last 32 KiB, right-aligned
+    uint64_t c_bits = 0, text = 0;        // compressed bits and text so far: the ratio that sizes a stage
+};
 
 namespace {
 
@@ -204,6 +215,7 @@ constexpr Region kArenaSlots { "arena", 32, 33 };             // the align pass'
 constexpr Region kPassHeapSlots { "pass heap", 33, 40 };      // record route: the heap, list and counters of a pass
 // text route: every pass keeps its heap on the device until the text is rendered
 inline Region text_heap_slots(int pass) { return { "text heap", 40 + 8 * (size_t)pass, 48 + 8 * (size_t)pass }; }
+constexpr Region kInflateSlots { "inflate", 88, 96 };        // plain gzip input: a stage's decode scratch
 constexpr Region kTextSlots { "text", 96, SIZE_MAX };         // text route: the headers and the text
 static_assert(40 + 8 * kMaxPasses <= kTextSlots.base, "the text heaps end below the text region");
 
@@ -1547,6 +1559,243 @@ int bgzf_inflate_dev(const mgb_index_t *index, const uint8_t *cbuf, BgzfWalk &w,
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------
+// Plain gzip input (mgb_fastx_stage_gzip, mgb_gzip_inflate): member headers and trailers read on the host, the DEFLATE
+// stream decoded speculatively on the device (gzip_core.cuh)
+// ---------------------------------------------------------------------------------------
+constexpr uint64_t kGzipSubBytes = 32768;        // compressed bytes per sub-range of a stage
+
+// The gzip member header (RFC 1952) at c[0, n): its length; 0 when n ends inside it; -1 when the bytes are not a header
+// this route serves (not gzip, not DEFLATE, or reserved flag bits). FHCRC is skipped unchecked, as Python's gzip does.
+int64_t gzip_header(const uint8_t *c, uint64_t n) {
+    if ((n > 0 && c[0] != 31) || (n > 1 && c[1] != 139) || (n > 2 && c[2] != 8) || (n > 3 && (c[3] & 0xe0))) return -1;
+    if (n < 10) return 0;
+    const uint8_t flg = c[3];
+    uint64_t at = 10;
+    if (flg & 4) {
+        if (n < at + 2) return 0;
+        at += 2 + rd16(c + at);
+    }
+    for (uint8_t f : { (uint8_t)8, (uint8_t)16 }) {
+        if (!(flg & f)) continue;
+        while (at < n && c[at]) ++at;
+        if (at >= n) return 0;
+        ++at;
+    }
+    if (flg & 2) at += 2;
+    return at <= n ? (int64_t)at : 0;
+}
+
+struct GzipCounts { uint64_t n_sub = 0, found = 0, confirmed = 0; };
+
+// What one stage did: it staged `text` bytes after the head, took c_used whole bytes, refused the input (the stream
+// is unchanged), or ended a member.
+struct GzipStage {
+    uint64_t text = 0, c_used = 0;
+    bool refused = false, member_end = false;
+};
+
+// One stage of stream s over c[0, n) (the first byte's first s->bit bits already decoded when in a member): the
+// member header if the stream is between members, then the DEFLATE stream from its position to the last confirmed
+// block end, or to the member's end and its checked trailer. *d_text (fastx_text_bytes of head + text, from bufs)
+// holds head then the text; *last: its last byte. Nothing is staged and s is unchanged when the stage refuses or
+// needs more input (c_used 0, not refused). inject: candidate bit offsets in c that replace the finder.
+// hand_over_unsplit: refuse a member whose first stage confirmed no candidate (see mgb_fastx_stage_gzip).
+int gzip_stage_dev(const mgb_index_t *index, mgb_gzip_stream *s, const uint8_t *c, uint64_t n, bool c_eof,
+                   uint64_t max_text, uint64_t sub_bytes, const std::vector<uint64_t> *inject,
+                   bool hand_over_unsplit, const char *head,
+                   uint64_t head_bytes, Stream &st, DevBufs &bufs, uint8_t **d_text, uint8_t *last, GzipStage *out,
+                   GzipCounts *counts, mgb_stats_t *stats) {
+    (void)index;
+    int rc;
+    *out = GzipStage();
+    mgb_gzip_stream g = *s;
+    uint64_t hdr = 0;
+    bool go = n > 0;
+    if (!g.in_member && n) {
+        const int64_t h = gzip_header(c, n);
+        if (h < 0 || (h == 0 && c_eof)) out->refused = true;
+        go = h > 0;
+        if (h > 0) {
+            hdr = (uint64_t)h;
+            g.in_member = true; g.bit = 0; g.member_text = 0; g.crc = 0;
+            std::fill(g.window.begin(), g.window.end(), 0);
+        }
+    } else if (!g.in_member) {
+        go = false;                                                   // the end of the input, between members
+    }
+    const uint64_t start = hdr * 8 + g.bit, sub_bits = sub_bytes * 8;
+    if (g.in_member && start >= n * 8) {
+        go = false;
+        if (c_eof) out->refused = true;                               // cut off after the header or a block
+    }
+    std::unique_ptr<DevBufs> ib;
+    GzipArgs a;
+    std::memset(&a, 0, sizeof(a));
+    std::vector<GzipSub> res;
+    std::vector<uint64_t> cand;
+    std::vector<GzipLink> links;
+    uint64_t end = start, text = 0;
+    bool final = false;
+    if (go) {
+        // as many sub-ranges as max_text needs at the stream's ratio so far (3 before any text), and the bytes their
+        // decodes may run into
+        const double ratio = g.c_bits ? std::max(1.0, 8.0 * g.text / g.c_bits) : 3.0;
+        const uint64_t all = (n * 8 - start + sub_bits - 1) / sub_bits;
+        uint64_t n_sub = std::min<uint64_t>(all, (uint64_t)std::min(1e12, (double)max_text / (ratio * sub_bytes)) + 2);
+        uint64_t up = std::min<uint64_t>(n, (start + n_sub * sub_bits) / 8 + std::max<uint64_t>(4 * sub_bytes, 262144));
+        uint64_t cap = std::max<uint64_t>(16 * sub_bytes, 262144);
+        bool retried = false;
+        for (;;) {
+            if (n_sub > 0xffffffffull) return fail(MGB_ERR_OVERFLOW, "too many gzip sub-ranges in one stage");
+            ib.reset(new DevBufs(st, bufs.ws, kInflateSlots));
+            a.start = start; a.sub_bits = sub_bits; a.n_sub = (uint32_t)n_sub; a.cap = (uint32_t)cap; a.cbytes = up;
+            uint8_t *d_c = nullptr;
+            if ((rc = ib->alloc(&d_c, up)) || (rc = ib->alloc(&a.cand, n_sub)) || (rc = ib->alloc(&a.res, n_sub))
+                || (rc = ib->alloc(&a.sym, n_sub * cap)))
+                return rc;
+            a.cbuf = d_c;
+            if ((rc = h2d(d_c, c, up, st))) return rc;
+            stats->h2d_bytes += up;
+            cand.assign(n_sub, kGzipNone);
+            if (inject) {
+                cand[0] = start;
+                for (uint64_t p : *inject)
+                    if (p > start && p < up * 8) {
+                        const uint64_t j = (p - start) / sub_bits;
+                        if (j < n_sub && p < cand[j]) cand[j] = p;
+                    }
+                if ((rc = h2d(a.cand, cand.data(), n_sub * 8, st))) return rc;
+            }
+#if defined(MGB_HOST_EMU)
+            BgzfShared sh;
+            if (!inject) for (uint32_t j = 0; j < a.n_sub; ++j) gzip_find_sub(a, j, sh);
+            for (uint32_t j = 0; j < a.n_sub; ++j) gzip_decode_sub(a, j, sh);
+#else
+            const unsigned grid = (unsigned)std::min<uint64_t>((n_sub + kGzipWarps - 1) / kGzipWarps, (uint64_t)index->num_sms * 16);
+            if (!inject) k_gzip_find<<<grid, 32 * kGzipWarps, 0, st.s>>>(a);
+            k_gzip_decode<<<grid, 32 * kGzipWarps, 0, st.s>>>(a);
+            CUDA_TRY(cudaGetLastError());
+#endif
+            stats->kernel_launches += inject ? 1 : 2;
+            res.resize(n_sub);
+            if ((rc = d2h(cand.data(), a.cand, n_sub * 8, st)) || (rc = d2h(res.data(), a.res, n_sub * sizeof(GzipSub), st))
+                || (rc = sync(st)))
+                return rc;
+            stats->d2h_bytes += n_sub * (8 + sizeof(GzipSub));
+            // the chain: sub-range 0 starts at a block boundary; the sub-range whose candidate a confirmed decode ended
+            // at exactly is confirmed too, and every block end a confirmed decode passed is the stream's
+            links.clear();
+            end = start; text = 0; final = false;
+            uint64_t j = 0, confirmed = 0;
+            uint32_t why = kGzipStop;
+            for (;;) {
+                const GzipSub &r = res[j];
+                if (r.reach > g.member_text + text) { why = kBgzfBadStream; break; }     // before the member's start
+                if (r.len) links.push_back(GzipLink{ j * cap, head_bytes + text, r.len, 0 });
+                text += r.len;
+                end = r.end;
+                if (r.status == kGzipFinal) { final = true; break; }
+                if (r.status != kGzipStop) { why = r.status; break; }
+                const uint64_t k = (r.end - start) / sub_bits;
+                if (k <= j || k >= n_sub || cand[k] != r.end) break;
+                ++confirmed;
+                if (text >= max_text) break;
+                j = k;
+            }
+            counts->n_sub += n_sub;
+            counts->confirmed += confirmed;
+            for (uint64_t k = 1; k < n_sub; ++k) counts->found += cand[k] != kGzipNone && cand[k] <= end;
+            if (why == kBgzfBadStream) { out->refused = true; break; }
+            if (end > start || final) {
+                // a member's first stage that decoded on one warp alone is a member the finder cannot see into
+                // (stored or fixed-Huffman blocks): the command leaves it to the host whole
+                if (hand_over_unsplit && g.member_text == 0 && !final && n_sub >= 2 && confirmed == 0 && !retried)
+                    out->refused = true;
+                break;
+            }
+            // no block ended: a block larger than the slot or than the bytes uploaded gets one sub-range with room
+            retried = true;
+            if (why == kBgzfBadSize && cap < (1ull << 28)) { n_sub = 1; cap *= 8; continue; }
+            if (why == kGzipShort && up < n) { n_sub = 1; up = n; continue; }
+            if (why == kBgzfBadSize || c_eof) out->refused = true;            // too large, or cut off
+            go = false;
+            break;
+        }
+        if (out->refused) go = false;
+    }
+    // the trailer: CRC32 and ISIZE of the member, after its last byte
+    const uint64_t tb = (end + 7) / 8;
+    if (go && final && tb + 8 > n) {
+        if (c_eof) out->refused = true;
+        go = false;
+    }
+    if ((rc = bufs.alloc(d_text, fastx_text_bytes(head_bytes + (go ? text : 0))))) return rc;
+    if (head_bytes && (rc = h2d(*d_text, head, head_bytes, st))) return rc;
+    stats->h2d_bytes += head_bytes;
+    *last = head_bytes ? (uint8_t)head[head_bytes - 1] : 0;
+    if (!go) return 0;
+    if (links.size() > 0xffffffffull) return fail(MGB_ERR_OVERFLOW, "too many gzip sub-ranges in one stage");
+    const uint64_t n_links = links.size(), pieces = (text + kGzipCrcPiece - 1) / kGzipCrcPiece;
+    std::vector<uint32_t> parts(pieces);
+    if (n_links) {
+        GzipLink *d_links = nullptr;
+        if ((rc = ib->alloc(&d_links, n_links)) || (rc = ib->alloc(&a.win, (n_links + 1) * kGzipWindow))
+            || (rc = ib->alloc(&a.crc_parts, pieces)))
+            return rc;
+        if ((rc = h2d(d_links, links.data(), n_links * sizeof(GzipLink), st)) || (rc = h2d(a.win, g.window.data(), kGzipWindow, st)))
+            return rc;
+        stats->h2d_bytes += n_links * sizeof(GzipLink) + kGzipWindow;
+        a.links = d_links; a.n_links = (uint32_t)n_links; a.text = *d_text; a.n_text = text;
+#if defined(MGB_HOST_EMU)
+        for (uint32_t i = 0; i < a.n_links; ++i)
+            for (uint32_t x = 0; x < kGzipWindow; ++x) gzip_window_at(a, i, x);
+        for (uint32_t i = 0; i < a.n_links; ++i)
+            for (uint32_t x = 0; x < links[i].len; ++x) gzip_resolve_at(a, i, x);
+        // the CRC32 parts run over the new text, after the head
+        a.text = *d_text + head_bytes;
+        BgzfShared sh;
+        bgzf_crc_table(sh);
+        for (uint64_t p = 0; p < pieces; ++p) gzip_crc_piece(a, p, sh.crc);
+#else
+        k_gzip_window<<<1, 1024, 0, st.s>>>(a);
+        k_gzip_resolve<<<(unsigned)std::min<uint64_t>(n_links, (uint64_t)index->num_sms * 16), 256, 0, st.s>>>(a);
+        a.text = *d_text + head_bytes;
+        k_gzip_crc<<<(unsigned)std::max<uint64_t>(1, std::min<uint64_t>((pieces + 255) / 256, (uint64_t)index->num_sms * 8)), 256, 0, st.s>>>(a);
+        CUDA_TRY(cudaGetLastError());
+#endif
+        stats->kernel_launches += 3;
+        if ((rc = d2h(parts.data(), a.crc_parts, pieces * 4, st))
+            || (rc = d2h(g.window.data(), a.win + n_links * kGzipWindow, kGzipWindow, st))
+            || (rc = d2h(last, *d_text + head_bytes + text - 1, 1, st)) || (rc = sync(st)))
+            return rc;
+        stats->d2h_bytes += pieces * 4 + kGzipWindow + 1;
+    }
+    uint32_t crc = 0;
+    const uint32_t whole = crc_x8n(kGzipCrcPiece);
+    for (uint64_t p = 0; p < pieces; ++p)
+        crc = crc_multmodp(p + 1 < pieces ? whole : crc_x8n(text - p * kGzipCrcPiece), crc) ^ parts[p];
+    g.crc = crc_multmodp(crc_x8n(text), g.crc) ^ crc;
+    g.member_text += text;
+    g.text += text;
+    g.c_bits += end - start;
+    if (final) {
+        if (rd32(c + tb) != g.crc || rd32(c + tb + 4) != (uint32_t)g.member_text) {
+            out->refused = true;
+            *last = head_bytes ? (uint8_t)head[head_bytes - 1] : 0;
+            return 0;
+        }
+        g.in_member = false; g.bit = 0;
+        out->c_used = tb + 8;
+        out->member_end = true;
+    } else {
+        out->c_used = end / 8; g.bit = (uint32_t)(end % 8);
+    }
+    out->text = text;
+    *s = g;
+    return 0;
+}
+
 // k-mer to node ids of every read on `strands` strands: the forward strand's into out_f, the reverse complement's into
 // *out_r (resized to the batch's k-mers); *koff: where each read's k-mers start
 static int map_nodes(const mgb_index_t *index, const char *seqs, const uint64_t *offsets, uint32_t n, uint32_t strands,
@@ -2491,6 +2740,36 @@ struct mgb_fastx_batch {
     }
 };
 
+// The records of a compressed stage's text d_text[0, text_bytes) (device memory of fastx_text_bytes(text_bytes)
+// bytes; last: its last byte) parsed into batch b, which keeps text[consumed, end) for the next stage's head (the whole
+// text when the host restatement parses it).
+static int stage_text(const mgb_index_t *index, mgb_fastx_batch *b, const uint8_t *d_text, uint64_t text_bytes,
+                      uint8_t last, bool at_eof, const char *comment_delim, bool fwd_rev, uint64_t *consumed,
+                      int *ended) {
+    Stream &st = b->cw.st;
+    int rc;
+    *consumed = 0; *ended = 0;
+    if ((rc = fastx_parse_text(index, d_text, text_bytes, last, at_eof, comment_delim, fwd_rev, st, b->bufs, &b->dev,
+                               &b->parse)))
+        return rc;
+    if (b->dev.refused) {            // the host restatement parses the inflated text
+        b->text.resize(text_bytes);
+        if ((text_bytes && (rc = d2h(b->text.data(), d_text, text_bytes, st))) || (rc = sync(st))) return rc;
+        b->parse.d2h_bytes += text_bytes;
+        fastx_parse_host(b->text.data(), text_bytes, at_eof, comment_delim, fwd_rev, &b->host, consumed, ended);
+        b->tail_at = *consumed;
+    } else {
+        *consumed = b->dev.consumed;
+        b->text.resize(text_bytes - *consumed);
+        if ((b->text.size() && (rc = d2h(b->text.data(), d_text + *consumed, b->text.size(), st))) || (rc = sync(st)))
+            return rc;
+        b->parse.d2h_bytes += b->text.size();
+    }
+    const std::vector<uint64_t> &offs = b->dev.refused ? b->host.offsets : b->dev.offsets;
+    if (offs.size() - 1 > 0xffffffffull) return fail(MGB_ERR_OVERFLOW, "more than 2^32 - 1 records in one chunk");
+    return MGB_OK;
+}
+
 extern "C" {
 
 int mgb_fastx_stage(const mgb_index_t *index, const char *buf, uint64_t bytes, int at_eof, const char *comment_delim,
@@ -2542,37 +2821,105 @@ int mgb_fastx_stage_bgzf(const mgb_index_t *index, const char *head, uint64_t he
     std::unique_ptr<mgb_fastx_batch> b(new mgb_fastx_batch(index));
     int rc = b->cw.ready();
     if (rc) return rc;
-    Stream &st = b->cw.st;
     BgzfWalk w;
     bgzf_walk(cbuf, cbytes, c_eof != 0, max_text, &w);
     uint8_t *d_text = nullptr, last = 0;
     uint64_t text_bytes = 0, n_ok = 0;
-    if ((rc = bgzf_inflate_dev(index, cbuf, w, head, head_bytes, st, b->bufs, &d_text, &text_bytes, &n_ok, &last,
+    if ((rc = bgzf_inflate_dev(index, cbuf, w, head, head_bytes, b->cw.st, b->bufs, &d_text, &text_bytes, &n_ok, &last,
                                &b->parse)))
         return rc;
     const bool at_eof = c_eof && w.c_end == cbytes && !w.refused;
-    *consumed = 0; *ended = 0;
-    if ((rc = fastx_parse_text(index, d_text, text_bytes, last, at_eof, comment_delim, fwd_rev, st, b->bufs, &b->dev,
-                               &b->parse)))
+    if ((rc = stage_text(index, b.get(), d_text, text_bytes, last, at_eof, comment_delim, fwd_rev, consumed, ended)))
         return rc;
-    if (b->dev.refused) {            // the host restatement parses the inflated text
-        b->text.resize(text_bytes);
-        if ((text_bytes && (rc = d2h(b->text.data(), d_text, text_bytes, st))) || (rc = sync(st))) return rc;
-        b->parse.d2h_bytes += text_bytes;
-        fastx_parse_host(b->text.data(), text_bytes, at_eof, comment_delim, fwd_rev, &b->host, consumed, ended);
-        b->tail_at = *consumed;
-    } else {
-        *consumed = b->dev.consumed;
-        b->text.resize(text_bytes - *consumed);
-        if ((b->text.size() && (rc = d2h(b->text.data(), d_text + *consumed, b->text.size(), st))) || (rc = sync(st)))
-            return rc;
-        b->parse.d2h_bytes += b->text.size();
-    }
-    const std::vector<uint64_t> &offs = b->dev.refused ? b->host.offsets : b->dev.offsets;
-    if (offs.size() - 1 > 0xffffffffull) return fail(MGB_ERR_OVERFLOW, "more than 2^32 - 1 records in one chunk");
     *c_consumed = w.c_end;
     *c_refused = w.refused ? 1 : 0;
     *out = b.release();
+    return MGB_OK;
+}
+
+int mgb_gzip_stream_create(mgb_gzip_stream_t **out) {
+    if (!out) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    *out = new mgb_gzip_stream();
+    return MGB_OK;
+}
+
+void mgb_gzip_stream_free(mgb_gzip_stream_t *stream) { delete stream; }
+
+int mgb_gzip_stream_state(const mgb_gzip_stream_t *stream, int *in_member, uint64_t *member_text) {
+    if (!stream || !in_member || !member_text) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    *in_member = stream->in_member ? 1 : 0;
+    *member_text = stream->in_member ? stream->member_text : 0;
+    return MGB_OK;
+}
+
+int mgb_fastx_stage_gzip(const mgb_index_t *index, mgb_gzip_stream_t *stream, const char *head, uint64_t head_bytes,
+                         const uint8_t *cbuf, uint64_t cbytes, int c_eof, uint64_t max_text, const char *comment_delim,
+                         int flags, uint64_t *c_consumed, int *c_refused, uint64_t *consumed, int *ended,
+                         mgb_fastx_batch_t **out) {
+    if (!index || !stream || !c_consumed || !c_refused || !consumed || !ended || !out || (!head && head_bytes)
+        || (!cbuf && cbytes))
+        return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (flags & ~MGB_FASTX_FWD_AND_REVERSE) return fail(MGB_ERR_INVALID_ARGUMENT, "unknown flags");
+    std::unique_ptr<mgb_fastx_batch> b(new mgb_fastx_batch(index));
+    int rc = b->cw.ready();
+    if (rc) return rc;
+    uint8_t *d_text = nullptr, last = 0;
+    GzipStage g;
+    GzipCounts counts;
+    if ((rc = gzip_stage_dev(index, stream, cbuf, cbytes, c_eof != 0, max_text, kGzipSubBytes, nullptr, true, head,
+                             head_bytes, b->cw.st, b->bufs, &d_text, &last, &g, &counts, &b->parse)))
+        return rc;
+    const bool at_eof = c_eof && g.c_used == cbytes && !g.refused && !stream->in_member;
+    if ((rc = stage_text(index, b.get(), d_text, head_bytes + g.text, last, at_eof, comment_delim,
+                         (flags & MGB_FASTX_FWD_AND_REVERSE) != 0, consumed, ended)))
+        return rc;
+    *c_consumed = g.c_used;
+    *c_refused = g.refused ? 1 : 0;
+    *out = b.release();
+    return MGB_OK;
+}
+
+int mgb_gzip_inflate(const mgb_index_t *index, const uint8_t *cbuf, uint64_t cbytes, int c_eof, uint64_t sub_bytes,
+                     const uint64_t *cands, uint64_t n_cands, char *out, uint64_t out_cap, uint64_t *out_bytes,
+                     uint64_t *c_consumed, int *refused, uint64_t *counts) {
+    if (!index || (!cbuf && cbytes) || (!cands && n_cands) || (!out && out_cap) || !out_bytes || !c_consumed
+        || !refused || !counts)
+        return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    CallWorkspace cw(index);
+    int rc = cw.ready();
+    if (rc) return rc;
+    mgb_stats_t stats;
+    std::memset(&stats, 0, sizeof(stats));
+    mgb_gzip_stream s;
+    GzipCounts cnt;
+    std::vector<char> text;
+    uint64_t at = 0;
+    bool ref = false;
+    for (;;) {
+        std::vector<uint64_t> inject;
+        for (uint64_t i = 0; i < n_cands; ++i) if (cands[i] >= at * 8) inject.push_back(cands[i] - at * 8);
+        DevBufs bufs(cw.st, cw.w, kBatchSlots);
+        uint8_t *d_text = nullptr, last = 0;
+        GzipStage g;
+        if ((rc = gzip_stage_dev(index, &s, cbuf + at, cbytes - at, c_eof != 0, UINT64_MAX,
+                                 sub_bytes ? sub_bytes : kGzipSubBytes, cands ? &inject : nullptr, false, nullptr, 0,
+                                 cw.st,
+                                 bufs, &d_text, &last, &g, &cnt, &stats)))
+            return rc;
+        if (g.text) {
+            text.resize(text.size() + g.text);
+            if ((rc = d2h(text.data() + text.size() - g.text, d_text, g.text, cw.st)) || (rc = sync(cw.st))) return rc;
+        }
+        at += g.c_used;
+        ref = g.refused;
+        if (ref || (!g.c_used && !g.member_end)) break;
+    }
+    counts[0] = cnt.n_sub; counts[1] = cnt.found; counts[2] = cnt.confirmed;
+    *out_bytes = text.size();
+    *c_consumed = at;
+    *refused = ref ? 1 : 0;
+    if (text.size() > out_cap) return fail(MGB_ERR_OVERFLOW, "output buffer too small");
+    if (text.size()) std::memcpy(out, text.data(), text.size());
     return MGB_OK;
 }
 

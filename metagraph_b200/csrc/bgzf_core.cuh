@@ -167,14 +167,29 @@ MGB_HD void bgzf_match(uint8_t *out, uint32_t o, uint32_t len, uint32_t dist, ui
     wsync();
 }
 
-// lit/len symbols up to end-of-block into out[*o, isize)
-MGB_HD uint32_t bgzf_codes(BgzfBits &r, BgzfShared &sh, uint8_t *out, uint32_t *o, uint32_t isize) {
+// Where a block's output goes. BgzfByteSink: the bytes of a BGZF block (k_bgzf_inflate); a sink with the same members
+// writes the 16-bit symbols of a speculative decode (gzip_core.cuh). cap: the most output the sink takes; reach: whether
+// a back-reference of `dist` from output position o is valid for the sink.
+struct BgzfByteSink {
+    uint8_t *out;
+    uint32_t cap;
+    MGB_HD bool reach(uint32_t o, uint32_t dist) const { return dist <= o; }
+    MGB_HD void lit(uint32_t o, uint32_t sym) { if (wlane() == 0) out[o] = (uint8_t)sym; }
+    MGB_HD void match(uint32_t o, uint32_t len, uint32_t dist) { bgzf_match(out, o, len, dist, cap); }
+    MGB_HD void stored(uint32_t o, const uint8_t *src, uint32_t len) {
+        for (uint32_t i = wlane(); i < len; i += kWarp) out[o + i] = src[i];
+        wsync();
+    }
+};
+
+// lit/len symbols up to end-of-block into the sink at [*o, cap)
+template <class Sink> MGB_HD uint32_t bgzf_codes(BgzfBits &r, BgzfShared &sh, Sink &s, uint32_t *o) {
     for (;;) {
         int sym = bgzf_decode(r, sh.lcount, sh.lsym);
         if (sym < 0) return kBgzfBadStream;
         if (sym < 256) {
-            if (*o >= isize) return kBgzfBadSize;
-            if (wlane() == 0) out[*o] = (uint8_t)sym;
+            if (*o >= s.cap) return kBgzfBadSize;
+            s.lit(*o, (uint32_t)sym);
             ++*o;
             continue;
         }
@@ -185,9 +200,9 @@ MGB_HD uint32_t bgzf_codes(BgzfBits &r, BgzfShared &sh, uint8_t *out, uint32_t *
         const int ds = bgzf_decode(r, sh.dcount, sh.dsym);
         if (ds < 0 || ds >= 30 || !bgzf_need(r, kBgzfDistExtra[ds])) return kBgzfBadStream;
         const uint32_t dist = kBgzfDistBase[ds] + bgzf_take(r, kBgzfDistExtra[ds]);
-        if (dist > *o) return kBgzfBadStream;
-        if (len > isize - *o) return kBgzfBadSize;
-        bgzf_match(out, *o, len, dist, isize);
+        if (!s.reach(*o, dist)) return kBgzfBadStream;
+        if (len > s.cap - *o) return kBgzfBadSize;
+        s.match(*o, len, dist);
         *o += len;
     }
 }
@@ -275,47 +290,53 @@ MGB_HD uint32_t bgzf_crc(BgzfShared &sh, const uint8_t *out, uint32_t n) {
     return crc;
 }
 
+// one DEFLATE block (header and body) into the sink at *o; *last: its BFINAL bit
+template <class Sink> MGB_HD uint32_t bgzf_block(BgzfBits &r, BgzfShared &sh, Sink &s, uint32_t *o, uint32_t *last) {
+    if (!bgzf_need(r, 3)) return kBgzfBadStream;
+    *last = bgzf_take(r, 1);
+    const uint32_t type = bgzf_take(r, 2);
+    if (type == 0) {                                  // stored: LEN, NLEN from the next byte boundary
+        bgzf_take(r, r.cnt & 7);
+        if (!bgzf_need(r, 32)) return kBgzfBadStream;
+        const uint32_t len = bgzf_take(r, 16), nlen = bgzf_take(r, 16);
+        if (len != (~nlen & 0xffff)) return kBgzfBadStream;
+        // the bytes still in the bit buffer go back to the payload
+        const uint64_t at = r.pos - r.cnt / 8;
+        r.pos = at; r.buf = 0; r.cnt = 0;
+        if (len > r.end - at) return kBgzfBadStream;
+        if (len > s.cap - *o) return kBgzfBadSize;
+        MGB_BGZF_ASSERT(at + len <= r.end && *o + len <= s.cap);
+        s.stored(*o, r.p + at, len);
+        r.pos += len;
+        *o += len;
+        return kBgzfOk;
+    }
+    if (type == 1) {
+        bgzf_fixed(sh);
+        return bgzf_codes(r, sh, s, o);
+    }
+    if (type == 2) {
+        const uint32_t status = bgzf_dynamic(r, sh);
+        return status == kBgzfOk ? bgzf_codes(r, sh, s, o) : status;
+    }
+    return kBgzfBadStream;
+}
+
 // block b with one warp: inflate, then check the stream's end, the length and the CRC32 against the trailer
 MGB_HD void bgzf_inflate_block(const BgzfArgs &a, uint32_t b, BgzfShared &sh) {
     const BgzfBlock blk = a.blocks[b];
-    uint8_t *out = a.text + blk.t_off;
+    BgzfByteSink out{a.text + blk.t_off, blk.isize};
     BgzfBits r;
     r.p = a.cbuf; r.pos = blk.c_off; r.end = blk.c_off + blk.c_len; r.buf = 0; r.cnt = 0;
     uint32_t o = 0, status = kBgzfOk, last = 0;
     while (!last && status == kBgzfOk) {
-        if (!bgzf_need(r, 3)) { status = kBgzfBadStream; break; }
-        last = bgzf_take(r, 1);
-        const uint32_t type = bgzf_take(r, 2);
-        if (type == 0) {                                  // stored: LEN, NLEN from the next byte boundary
-            bgzf_take(r, r.cnt & 7);
-            if (!bgzf_need(r, 32)) { status = kBgzfBadStream; break; }
-            const uint32_t len = bgzf_take(r, 16), nlen = bgzf_take(r, 16);
-            if (len != (~nlen & 0xffff)) { status = kBgzfBadStream; break; }
-            // the bytes still in the bit buffer go back to the payload
-            const uint64_t at = r.pos - r.cnt / 8;
-            r.pos = at; r.buf = 0; r.cnt = 0;
-            if (len > r.end - at) { status = kBgzfBadStream; break; }
-            if (len > blk.isize - o) { status = kBgzfBadSize; break; }
-            MGB_BGZF_ASSERT(at + len <= r.end && o + len <= blk.isize);
-            for (uint32_t i = wlane(); i < len; i += kWarp) out[o + i] = a.cbuf[at + i];
-            wsync();
-            r.pos += len;
-            o += len;
-        } else if (type == 1) {
-            bgzf_fixed(sh);
-            status = bgzf_codes(r, sh, out, &o, blk.isize);
-        } else if (type == 2) {
-            status = bgzf_dynamic(r, sh);
-            if (status == kBgzfOk) status = bgzf_codes(r, sh, out, &o, blk.isize);
-        } else {
-            status = kBgzfBadStream;
-        }
+        status = bgzf_block(r, sh, out, &o, &last);
         wsync();
     }
     // the stream ends in the payload's last byte (the trailer follows it), and holds ISIZE bytes
     if (status == kBgzfOk && (r.pos != r.end || r.cnt >= 8)) status = kBgzfBadStream;
     if (status == kBgzfOk && o != blk.isize) status = kBgzfBadSize;
-    if (status == kBgzfOk && bgzf_crc(sh, out, o) != blk.crc) status = kBgzfBadCrc;
+    if (status == kBgzfOk && bgzf_crc(sh, out.out, o) != blk.crc) status = kBgzfBadCrc;
     if (wlane() == 0) a.status[b] = status;
     wsync();
 }
