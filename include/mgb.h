@@ -270,6 +270,14 @@ typedef struct mgb_gzip_stream mgb_gzip_stream_t;
 int mgb_gzip_stream_create(mgb_gzip_stream_t **out);
 void mgb_gzip_stream_free(mgb_gzip_stream_t *stream);
 int mgb_gzip_stream_state(const mgb_gzip_stream_t *stream, int *in_member, uint64_t *member_text);
+/* A stream as one relocatable byte block, so that another process may stage its next part (the `--distributed`
+ * command passes it on with the token): its bit position, 32 KiB window, running CRC32 and length, and whether it is
+ * inside a member. mgb_gzip_stream_export writes it into caller memory of at least mgb_gzip_stream_export_bytes bytes;
+ * mgb_gzip_stream_import rebuilds a stream from such a block (free it with mgb_gzip_stream_free). A stream is not tied
+ * to an index or a device. */
+uint64_t mgb_gzip_stream_export_bytes(const mgb_gzip_stream_t *stream);
+int mgb_gzip_stream_export(const mgb_gzip_stream_t *stream, void *dst, uint64_t capacity);
+int mgb_gzip_stream_import(const void *block, uint64_t bytes, mgb_gzip_stream_t **out);
 /* mgb_fastx_stage_bgzf for plain gzip input. cbuf holds the stream's next bytes (its first byte partly decoded when
  * the stream is inside a member). Stages `head` followed by the text of the stream, inflated on index's device, up to
  * the last DEFLATE block boundary it confirmed once the text reaches max_text, or up to the member's end, where the

@@ -109,6 +109,12 @@ def load_library(path=None):
     L.mgb_gzip_stream_free.argtypes = [vp]
     L.mgb_gzip_stream_state.restype = i
     L.mgb_gzip_stream_state.argtypes = [vp, ctypes.POINTER(i), ctypes.POINTER(u64)]
+    L.mgb_gzip_stream_export_bytes.restype = u64
+    L.mgb_gzip_stream_export_bytes.argtypes = [vp]
+    L.mgb_gzip_stream_export.restype = i
+    L.mgb_gzip_stream_export.argtypes = [vp, vp, u64]
+    L.mgb_gzip_stream_import.restype = i
+    L.mgb_gzip_stream_import.argtypes = [vp, u64, ctypes.POINTER(vp)]
     L.mgb_fastx_stage_gzip.restype = i
     L.mgb_fastx_stage_gzip.argtypes = [vp, vp, vp, u64, vp, u64, i, u64, cp, i, ctypes.POINTER(u64), ctypes.POINTER(i),
                                        ctypes.POINTER(u64), ctypes.POINTER(i), ctypes.POINTER(vp)]
@@ -170,7 +176,8 @@ REQUIRED_SYMBOLS = [
     "mgb_align_batch_text", "mgb_results_text", "mgb_align_fastx_text", "mgb_fastx_parse", "mgb_index_replicate",
     "mgb_fastx_stage", "mgb_align_fastx_batch_text", "mgb_fastx_batch_free", "mgb_fastx_stage_bgzf",
     "mgb_fastx_batch_tail", "mgb_bgzf_inflate", "mgb_gzip_stream_create", "mgb_gzip_stream_free",
-    "mgb_gzip_stream_state", "mgb_fastx_stage_gzip", "mgb_gzip_inflate",
+    "mgb_gzip_stream_state", "mgb_fastx_stage_gzip", "mgb_gzip_inflate", "mgb_gzip_stream_export_bytes",
+    "mgb_gzip_stream_export", "mgb_gzip_stream_import",
 ]
 MGB_TEXT_TSV, MGB_TEXT_JSON = 1, 2
 MGB_FASTX_FWD_AND_REVERSE = 1

@@ -609,6 +609,22 @@ class GzipStream:
         _lib.check(self._L, self._L.mgb_gzip_stream_state(self.handle, ctypes.byref(m), ctypes.byref(t)))
         return bool(m.value), t.value
 
+    def export(self):
+        """mgb_gzip_stream_export: the stream's state as bytes, which from_export rebuilds in any process"""
+        n = int(self._L.mgb_gzip_stream_export_bytes(self.handle))
+        buf = ctypes.create_string_buffer(n)
+        _lib.check(self._L, self._L.mgb_gzip_stream_export(self.handle, buf, n))
+        return buf.raw
+
+    @classmethod
+    def from_export(cls, L, block):
+        """mgb_gzip_stream_import: a new stream in library L with the state `block` (from export) holds"""
+        s = cls.__new__(cls)
+        s._L, s.handle = L, ctypes.c_void_p()
+        block = bytes(block)
+        _lib.check(L, L.mgb_gzip_stream_import(block, len(block), ctypes.byref(s.handle)))
+        return s
+
     def close(self):
         if self.handle:
             self._L.mgb_gzip_stream_free(self.handle)

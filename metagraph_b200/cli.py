@@ -17,6 +17,10 @@ Any other .gz/.bgz file (plain gzip, as gzip and pigz write it) goes up compress
 a member on the device (mgb_fastx_stage_gzip), decoding the DEFLATE stream from many points at once. Where the device
 route refuses, the file is reopened at the current member's start with Python's gzip, the text of that member already
 staged is skipped, and the rest takes the text route: the same bytes, or the same error, as Python's gzip.
+
+With --distributed the command is one rank of a torchrun job: rank c mod W stages and aligns chunk c, the token goes
+from rank to rank as a small message (the file is read by offset on every rank), and rank 0 gathers and writes the
+texts in chunk order; the same bytes as one process with the same chunk size (align_file_distributed).
 """
 import argparse
 import gzip
@@ -57,9 +61,13 @@ def _parser():
     p.add_argument("--header-comment-delim", default=None, help="join the FASTA/FASTQ name and comment with this")
     p.add_argument("-p", "--parallel", type=int, default=1,
                    help="accepted for compatibility; changes no output (--devices sets the workers)")
-    p.add_argument("--devices", default="0", metavar="LIST",
+    p.add_argument("--devices", default=None, metavar="LIST",
                    help="comma-separated CUDA ordinals, one worker each (an ordinal listed twice runs two workers on "
                         "that device's one index), or `all`: every visible device once [0]")
+    p.add_argument("--distributed", action="store_true",
+                   help="run as one rank of a torchrun job (RANK, WORLD_SIZE and LOCAL_RANK from its environment): "
+                        "rank c mod WORLD_SIZE aligns chunk c on device LOCAL_RANK mod the device count, and rank 0 "
+                        "writes all the output")
     p.add_argument("--batch-size", type=int, default=100000000,
                    help="accepted for compatibility; changes no output")
     p.add_argument("--align-only-forwards", action="store_true")
@@ -100,7 +108,24 @@ def parse_args(argv):
         raise UsageError("alignment penalties should be given as positive integers")
     if args.align_alternative_alignments == 0:
         raise UsageError("align-alternative-alignments must be > 0")
+    if args.distributed and args.devices is not None:
+        raise UsageError("--devices cannot be combined with --distributed: each rank uses device LOCAL_RANK mod the "
+                         "device count")
+    if args.devices is None:
+        args.devices = "0"
     return args
+
+
+def dist_env():
+    """(RANK, WORLD_SIZE, LOCAL_RANK) as torchrun sets them; UsageError when one is missing or bad"""
+    try:
+        rank, world, local = (int(os.environ[v]) for v in ("RANK", "WORLD_SIZE", "LOCAL_RANK"))
+    except (KeyError, ValueError):
+        raise UsageError("--distributed needs RANK, WORLD_SIZE and LOCAL_RANK in the environment (run it under "
+                         "torchrun)")
+    if not 0 <= rank < world or local < 0:
+        raise UsageError("--distributed: bad RANK %d, WORLD_SIZE %d or LOCAL_RANK %d" % (rank, world, local))
+    return rank, world, local
 
 
 def devices_of(spec, count):
@@ -227,7 +252,8 @@ class _Token:
     starts at file offset `c_at`), and on the gzip route the stream's state and the compressed bytes a stage is
     given (`c_want`, doubled after a stage that could not make progress)."""
 
-    def __init__(self, path, chunk_bytes):
+    def __init__(self, path, chunk_bytes, reader=None):
+        """reader(file, chunk_bytes): what reads the file's chunks (_Chunks, one chunk ahead on a thread, by default)"""
         self.path, self.size = path, chunk_bytes
         self.pending, self.at_eof, self.want = b"", False, 0
         self.route = route_of(path)
@@ -235,7 +261,7 @@ class _Token:
         self.cpend, self.c_at = b"", 0
         self.stream, self.m_at, self.c_want = None, 0, chunk_bytes
         self.files = [open(path, "rb") if self.raw else (gzip.open if self.route == "host" else open)(path, "rb")]
-        self.chunks = _Chunks(self.files[0], chunk_bytes)
+        self.chunks = (reader or _Chunks)(self.files[0], chunk_bytes)
 
     def _read(self):
         nxt = self.chunks.next()
@@ -352,6 +378,186 @@ class _Token:
             self.stream.close()
 
 
+class _OffsetChunks:
+    """_Chunks by file offset: chunk j is the file's bytes [j*size, (j+1)*size), the bytes the j-th read of _Chunks
+    returns, so that any process can go on reading where another stopped; `n` counts the chunks read"""
+
+    def __init__(self, f, size):
+        self.f, self.size, self.n = f, size, 0
+
+    def next(self):
+        self.f.seek(self.n * self.size)
+        self.n += 1
+        return self.f.read(self.size)
+
+    def close(self):
+        pass
+
+
+# token kinds between ranks: the state follows (LIVE); the file was handed over to Python's gzip on rank `held`
+# (HELD); no chunk follows (OVER); a rank failed, so no rank stages (STOP)
+_LIVE, _HELD, _OVER, _STOP = 0, 1, 2, 3
+# what each rank reports for a round: its chunk's text (TEXT, LAST when no chunk follows it), no chunk and the file
+# goes on (SKIP), no chunk and the file has ended (ENDED), or an error message (ERROR)
+_TEXT, _LAST, _SKIP, _ENDED, _ERROR = 0, 1, 2, 3, 4
+_TAG_TOKEN, _TAG_STATE, _TAG_TEXT = 1, 2, 3
+# A token message is _TOKEN_INTS int64s -- kind, held, the _RankToken state in the order _TOKEN_STATE names it, and the
+# length of the body -- then the body: the text tail and the gzip stream's state (mgb_gzip_stream_export).
+_TOKEN_STATE = ("chunks_read", "at_eof", "want", "c_at", "m_at", "c_want", "tail_bytes", "stream_bytes")
+_TOKEN_INTS = 2 + len(_TOKEN_STATE) + 1
+
+
+class _RankToken(_Token):
+    """The _Token of one rank of `align --distributed`. It reads the file by offset (_OffsetChunks), so its state
+    crosses processes as a small message (dump / load): the chunks read and at_eof, c_at, the text tail and grow state,
+    and on the gzip route the stream (mgb_gzip_stream_export). The compressed bytes not yet staged are the file's bytes
+    from c_at to the end of the last chunk read, so the receiving rank reads them itself. Once handed over to Python's
+    gzip (route "host") it stays on this rank."""
+
+    def __init__(self, path, chunk_bytes):
+        super().__init__(path, chunk_bytes, _OffsetChunks)
+
+    def dump(self):
+        """(the state, in _TOKEN_STATE's order; the body: the text tail then the stream's state)"""
+        st = self.stream.export() if self.stream is not None else b""
+        return [self.chunks.n, int(self.at_eof), self.want, self.c_at, self.m_at, self.c_want, len(self.pending),
+                len(st)], self.pending + st
+
+    def load(self, state, body, L):
+        n, at_eof, self.want, self.c_at, self.m_at, self.c_want, n_pending, n_stream = state
+        self.chunks.n, self.at_eof = n, bool(at_eof)
+        self.pending = body[:n_pending]
+        if self.stream is not None:
+            self.stream.close()
+            self.stream = None
+        if n_stream:
+            from .aligner import GzipStream
+            self.stream = GzipStream.from_export(L, body[n_pending:n_pending + n_stream])
+        if self.raw:
+            f = self.files[0]
+            f.seek(self.c_at)
+            self.cpend = f.read(max(0, n * self.size - self.c_at))
+
+
+def _token_msg(kind, held, token=None):
+    """a token message (header ints, body) of this kind; the state of `token` when it is LIVE"""
+    state, body = token.dump() if token is not None else ([0] * len(_TOKEN_STATE), b"")
+    return [kind, held] + state + [len(body)], body
+
+
+class DistributedError(RuntimeError):
+    """the error that stopped `align --distributed` on some rank, raised on every rank"""
+
+
+def align_file_distributed(aligner, path, out, json=False, comment_delim=None, fwd_and_reverse=False,
+                           chunk_bytes=CHUNK_BYTES):
+    """align_file across the ranks of the default process group (gloo): chunk c is staged and aligned by rank c mod W,
+    and rank 0 writes every text to `out` (None elsewhere) in chunk order; the same bytes as align_file for the same
+    chunk size. The ranks go in rounds of W chunks. In a round the token goes around the ring 0 -> 1 -> ... -> W-1 -> 0
+    as a message (_RankToken.dump), each rank staging its chunk before it passes the token on and aligning it after;
+    then the texts and one status per rank go to rank 0 (sharding.gather_blocks), which writes them. So a rank holds
+    at most one staged batch and one text, and stages chunk c only after rank 0 has written text c - W. From a hand-over
+    to Python's gzip on, the rank that made it stages every chunk, one per round.
+
+    Every error on a rank becomes that rank's ERROR status: opening the file, staging, passing the token on, aligning,
+    and on rank 0 writing (reported in the next round, whose token is then a STOP; when the file has no next round,
+    rank 0 alone raises it and the caller's agreement after the file passes it on). Every rank learns every status, so
+    the first error or the end of the file stops all of them after the same round: rank 0 writes the texts before the
+    failed chunk, and every rank raises DistributedError with the error's message. Returns the bytes written."""
+    import torch.distributed as dist
+    from .sharding import gather_blocks
+    rank, W = dist.get_rank(), dist.get_world_size()
+    token, failed, written = None, None, 0
+    try:
+        token = _RankToken(path, chunk_bytes)
+    except Exception as e:
+        failed = str(e)
+    msg = _token_msg(_LIVE, 0, token) if token is not None else _token_msg(_STOP, 0)    # rank 0's, for round 1
+    try:
+        while True:
+            if rank:
+                msg = _recv_token((rank - 1) % W)
+            (kind, held), state, body = msg[0][:2], msg[0][2:-1], msg[1]
+            batch, code, block, msg = None, _SKIP, b"", None
+            if failed is None and (kind == _LIVE or (kind == _HELD and held == rank)):
+                try:
+                    if kind == _LIVE and W > 1:
+                        token.load(state, body, aligner._L)
+                    batch, last = token.stage(aligner, lambda: False, comment_delim, fwd_and_reverse)
+                    code = _TEXT
+                    if batch is None or last:
+                        kind, code = _OVER, _LAST if batch is not None else _ENDED
+                    elif token.route == "host":
+                        kind, held = _HELD, rank
+                    msg = _token_msg(kind, held, token if kind == _LIVE else None)
+                except Exception as e:
+                    if batch is not None:
+                        aligner.free_staged(batch)
+                        batch = None
+                    failed = str(e)
+            elif kind in (_OVER, _STOP):
+                code = _ENDED
+            if failed is not None:
+                code, block, msg = _ERROR, failed.encode("utf-8", "replace"), _token_msg(_STOP, held)
+            elif msg is None:
+                msg = _token_msg(kind, held)
+            sent = _send_token(msg, (rank + 1) % W) if W > 1 else []
+            if batch is not None:
+                try:
+                    block = aligner.align_staged_text(batch, json)     # consumes the batch
+                except Exception as e:
+                    code, block = _ERROR, str(e).encode("utf-8", "replace")
+            if rank == 0 and W > 1:
+                msg = _recv_token(W - 1)
+            for q in sent:
+                q.wait()
+            codes, blocks = gather_blocks(block, code, tag=_TAG_TEXT)
+            block = None
+            for r, c in enumerate(codes):
+                if c == _ERROR:
+                    error = blocks[r].decode("utf-8", "replace") if blocks is not None else "rank %d failed" % r
+                    raise DistributedError(failed if rank == 0 and failed is not None else error)
+                if c in (_TEXT, _LAST) and out is not None and failed is None:
+                    try:
+                        out.write(blocks[r])
+                        written += len(blocks[r])
+                    except Exception as e:      # reported in the next round
+                        failed = str(e)
+            if any(c in (_LAST, _ENDED) for c in codes):
+                if failed is not None:
+                    raise DistributedError(failed)
+                return written
+    finally:
+        if token is not None:
+            token.close()
+
+
+def _send_token(msg, dst):
+    """isends a token message (header ints, body bytes) to rank dst; returns the works to wait for"""
+    import torch
+    import torch.distributed as dist
+    hdr, body = msg
+    works = [dist.isend(torch.tensor(hdr, dtype=torch.int64), dst, tag=_TAG_TOKEN)]
+    if body:
+        works.append(dist.isend(torch.frombuffer(bytearray(body), dtype=torch.uint8), dst, tag=_TAG_STATE))
+    return works
+
+
+def _recv_token(src):
+    """the token message rank src sent: (header ints, body bytes)"""
+    import torch
+    import torch.distributed as dist
+    hdr = torch.zeros(_TOKEN_INTS, dtype=torch.int64)
+    dist.recv(hdr, src, tag=_TAG_TOKEN)
+    hdr = [int(x) for x in hdr.tolist()]
+    body = b""
+    if hdr[-1]:
+        t = torch.empty(hdr[-1], dtype=torch.uint8)
+        dist.recv(t, src, tag=_TAG_STATE)
+        body = t.numpy().tobytes()
+    return hdr, body
+
+
 def align_file_workers(aligners, path, out, json=False, comment_delim=None, fwd_and_reverse=False,
                        chunk_bytes=CHUNK_BYTES):
     """align_file with one worker thread per aligner; the same bytes go to `out`. Chunk i is staged by worker i mod W,
@@ -448,9 +654,16 @@ def main(argv=None):
         return 2
     try:
         args = parse_args(argv[1:])
+        if args.distributed:
+            env = dist_env()
         from . import _lib
         from .aligner import B200Aligner, BOSSTable, DBGSuccinctIndex
-        devices = devices_of(args.devices, _lib.load_library().mgb_device_count())
+        count = _lib.load_library().mgb_device_count()
+        if args.distributed:
+            if not count:
+                raise UsageError("--distributed: no CUDA device is visible")
+            return main_distributed(args, env[0], env[2] % count)
+        devices = devices_of(args.devices, count)
         boss = BOSSTable.from_dbg(args.graph)
         alphabet = {0: "dna", 1: "protein"}.get(boss.alphabet, "code %d" % boss.alphabet)
         cfg = config_of(args, boss.k, alphabet)
@@ -502,3 +715,69 @@ def main(argv=None):
         for ix in indexes.values():
             ix.close()
     return 0
+
+
+def main_distributed(args, rank, device):
+    """main() for one rank of `align --distributed`: every rank loads the graph and builds its own index on `device`,
+    and the files are aligned one after the other by all ranks (align_file_distributed). Only rank 0 writes the output
+    and the error. The ranks agree (_agree) after the set-up, before each file (it exists on every rank, and rank 0
+    could open -o) and after it (rank 0 could write and close its output), so an error on any rank stops every rank
+    with the same exit code; they meet at a barrier before they return, so no rank ends while rank 0 still writes."""
+    import torch.distributed as dist
+    from .aligner import B200Aligner, BOSSTable, DBGSuccinctIndex
+    dist.init_process_group("gloo")
+    index = None
+    try:
+        error = None
+        try:
+            boss = BOSSTable.from_dbg(args.graph)
+            alphabet = {0: "dna", 1: "protein"}.get(boss.alphabet, "code %d" % boss.alphabet)
+            cfg = config_of(args, boss.k, alphabet)
+            index = DBGSuccinctIndex(boss, device=device)
+            aligner = B200Aligner(index, cfg)
+        except Exception as e:
+            error = "error: %s" % e
+        if _agree(error, rank):
+            return 1
+        for path in args.files:
+            out, error = None, None
+            try:
+                if not os.path.exists(path):
+                    error = "ERROR: Cannot read from file %s" % path
+                elif rank == 0:
+                    # reopened and truncated per input (cli/align.cpp:409-411)
+                    out = open(args.outfile, "wb") if args.outfile else sys.stdout.buffer
+            except Exception as e:
+                error = "error: %s" % e
+            if _agree(error, rank):
+                return 1
+            try:
+                align_file_distributed(aligner, path, out, args.json, args.header_comment_delim, args.fwd_and_reverse,
+                                       CHUNK_BYTES)
+            except Exception as e:
+                error = "error: %s" % e
+            if out is not None:
+                try:
+                    out.close() if args.outfile else out.flush()
+                except Exception as e:
+                    error = error or "error: %s" % e
+            if _agree(error, rank):
+                return 1
+        return 0
+    finally:
+        if rank == 0:
+            sys.stderr.flush()
+        dist.barrier()
+        if index is not None:
+            index.close()
+        dist.destroy_process_group()
+
+
+def _agree(error, rank):
+    """every rank's error line (None: no error) to every rank: True when some rank has one, which rank 0 then prints
+    (the first in rank order)"""
+    from .sharding import gather_blocks
+    codes, lines = gather_blocks((error or "").encode("utf-8", "replace"), int(error is not None))
+    if rank == 0 and any(codes):
+        sys.stderr.write("%s\n" % lines[codes.index(1)].decode("utf-8", "replace"))
+    return any(codes)

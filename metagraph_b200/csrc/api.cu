@@ -2852,6 +2852,41 @@ int mgb_gzip_stream_state(const mgb_gzip_stream_t *stream, int *in_member, uint6
     return MGB_OK;
 }
 
+// Relocatable form of a gzip stream (what the token carries between processes): header, then the 32 KiB window.
+namespace {
+struct GzipStreamHdr { uint64_t magic; uint32_t in_member, bit; uint64_t member_text; uint32_t crc, window;
+                       uint64_t c_bits, text; };
+const uint64_t kGzipStreamMagic = 0x314d525453475a47ull;     // "GZGSTRM1"
+}
+uint64_t mgb_gzip_stream_export_bytes(const mgb_gzip_stream_t *stream) {
+    (void)stream;
+    return sizeof(GzipStreamHdr) + kGzipWindow;
+}
+int mgb_gzip_stream_export(const mgb_gzip_stream_t *s, void *dst, uint64_t capacity) {
+    if (!s || !dst) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    if (capacity < mgb_gzip_stream_export_bytes(s)) return fail(MGB_ERR_INVALID_ARGUMENT, "export buffer too small");
+    GzipStreamHdr h { kGzipStreamMagic, s->in_member ? 1u : 0u, s->bit, s->member_text, s->crc, kGzipWindow,
+                      s->c_bits, s->text };
+    std::memcpy(dst, &h, sizeof(h));
+    std::memcpy((char*)dst + sizeof(h), s->window.data(), kGzipWindow);
+    return MGB_OK;
+}
+int mgb_gzip_stream_import(const void *block, uint64_t bytes, mgb_gzip_stream_t **out) {
+    if (!block || !out) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    GzipStreamHdr h;
+    if (bytes < sizeof(h)) return fail(MGB_ERR_INVALID_ARGUMENT, "bad gzip stream block");
+    std::memcpy(&h, block, sizeof(h));
+    if (h.magic != kGzipStreamMagic || h.window != kGzipWindow || bytes < sizeof(h) + kGzipWindow || h.in_member > 1
+        || h.bit > 7)
+        return fail(MGB_ERR_INVALID_ARGUMENT, "bad gzip stream block");
+    std::unique_ptr<mgb_gzip_stream> s(new mgb_gzip_stream());
+    s->in_member = h.in_member != 0; s->bit = h.bit; s->member_text = h.member_text; s->crc = h.crc;
+    s->c_bits = h.c_bits; s->text = h.text;
+    std::memcpy(s->window.data(), (const char*)block + sizeof(h), kGzipWindow);
+    *out = s.release();
+    return MGB_OK;
+}
+
 int mgb_fastx_stage_gzip(const mgb_index_t *index, mgb_gzip_stream_t *stream, const char *head, uint64_t head_bytes,
                          const uint8_t *cbuf, uint64_t cbytes, int c_eof, uint64_t max_text, const char *comment_delim,
                          int flags, uint64_t *c_consumed, int *c_refused, uint64_t *consumed, int *ended,

@@ -3,7 +3,8 @@ index is replicated per HBM, there is no collective on the data path. Only the p
 rank exports its results as one relocatable byte block (mgb_results_export: the records as the kernel packed
 them), the sizes are all-gathered, the blocks go to rank 0 with point-to-point sends (NCCL over NVLink with device
 tensors, gloo with CPU tensors in the CPU tests) and rank 0 rebuilds one result set per shard
-(mgb_results_import) and emits them in input order."""
+(mgb_results_import) and emits them in input order. align_sharded_text gathers text instead: each rank renders its
+shard on its own device and rank 0 concatenates the blocks (gather_blocks), which `align --distributed` uses too."""
 import ctypes
 
 import numpy as np
@@ -81,6 +82,37 @@ class ResultGather:
         return out
 
 
+def gather_blocks(block, code=0, device=None, dst=0, tag=0):
+    """Gathers one byte block per rank on rank `dst`, with one int (`code`) per rank that every rank learns: sizes and
+    codes are all-gathered, and the blocks go to dst with point-to-point sends, as ResultGather sends its blocks
+    (device: a CUDA device for NCCL, None for gloo with CPU tensors). Returns (codes, blocks): the codes in rank order
+    on every rank, and on dst the blocks (bytes) in rank order, elsewhere None."""
+    import torch
+    import torch.distributed as dist
+    rank, world = dist.get_rank(), dist.get_world_size()
+    dev = device if device is not None else torch.device("cpu")
+    meta = torch.tensor([len(block), code], dtype=torch.int64, device=dev)
+    metas = [torch.zeros(2, dtype=torch.int64, device=dev) for _ in range(world)]
+    dist.all_gather(metas, meta)
+    metas = [[int(x) for x in m.tolist()] for m in metas]
+    codes = [m[1] for m in metas]
+    if rank != dst:
+        if block:
+            blk = torch.frombuffer(bytearray(block), dtype=torch.uint8).to(dev)
+            for q in dist.batch_isend_irecv([dist.P2POp(dist.isend, blk, dst, tag=tag)]):
+                q.wait()
+        return codes, None
+    bufs, ops = {}, []
+    for r in range(world):
+        if r != rank and metas[r][0]:
+            bufs[r] = torch.empty(metas[r][0], dtype=torch.uint8, device=dev)
+            ops.append(dist.P2POp(dist.irecv, bufs[r], r, tag=tag))
+    for q in (dist.batch_isend_irecv(ops) if ops else []):
+        q.wait()
+    return codes, [bytes(block) if r == rank else bufs[r].cpu().numpy().tobytes() if r in bufs else b""
+                   for r in range(world)]
+
+
 def align_sharded(aligner, batch, format_fn, device=None):
     """Aligns this rank's shard of `batch` ([(header, seq)]) and gathers the results on rank 0, which formats them
     in input order with format_fn(header, AlignmentResults). Returns the list of entries on rank 0 (one per read,
@@ -107,3 +139,16 @@ def align_sharded(aligner, batch, format_fn, device=None):
         finally:
             aligner._L.mgb_results_free(h)
     return out
+
+
+def align_sharded_text(aligner, batch, json=False, device=None):
+    """What aligner.align_batch_text(batch, json) returns for the whole `batch` ([(header, seq)]), with the reads
+    sharded across ranks: each rank renders its shard's TSV or JSON on its own device (mgb_align_batch_text) and rank 0
+    gathers the text blocks (gather_blocks: NCCL with `device` a CUDA device, gloo with None). Returns the bytes on rank
+    0, None elsewhere."""
+    import torch.distributed as dist
+    rank, world = dist.get_rank(), dist.get_world_size()
+    lo, hi = shard_range(len(batch), rank, world)
+    text = aligner.align_batch_text(batch[lo:hi], json) if hi > lo else b""
+    _, blocks = gather_blocks(text, device=device)
+    return None if blocks is None else b"".join(blocks)
