@@ -312,6 +312,59 @@ int mgb_fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes, i
                     int flags, int device_route, char *seqs, uint64_t max_seq_bytes, uint64_t *offsets, char *names,
                     uint64_t max_name_bytes, uint64_t *name_offsets, uint64_t max_records, uint64_t *n_records,
                     uint64_t *consumed, int *ended, int *refused);
+/* ---- device-resident batches ---------------------------------------------------------- */
+
+/* The same seed-and-extend as mgb_align_batch over n_reads reads that already sit in device memory on index's device
+ * (a basecaller's output, a torch tensor); the results stay on the device as columns (mgb_device_results_write).
+ *   stream   cudaStream_t of the caller (NULL = the legacy default stream). Before reading d_seqs or offsets the call
+ *            makes its own stream wait on an event recorded on `stream`, so reads produced by work still queued there
+ *            may be passed.
+ *   d_seqs   device memory on index's device (checked with cudaPointerGetAttributes: a host pointer or another device's
+ *            pointer is MGB_ERR_INVALID_ARGUMENT); read r is d_seqs[offsets[r], offsets[r + 1]). It may start at any
+ *            byte and end at the end of its allocation: the route first copies the reads device to device into the
+ *            batch's own 16-byte-aligned buffer with 64 bytes of padding, and no kernel reads the caller's buffer.
+ *            NULL is accepted when the reads hold no characters.
+ *   offsets  [n_reads + 1], host memory, or device memory on index's device when offsets_on_device = 1. Device offsets
+ *            are downloaded once (8 bytes per read). Then they are checked as mgb_align_batch checks them
+ *            (non-decreasing, read length): MGB_ERR_INVALID_ARGUMENT.
+ * A configuration fails exactly as it fails in mgb_align_batch, with the same code and text. The call blocks the host
+ * until the align passes are done, as mgb_align_batch does (retry passes are decided on the host); per pass only a
+ * 48-byte summary comes down, plus 4 bytes per read that overflowed its arena. The whole batch runs as one piece on
+ * one stream. The handle holds one of the index's working-memory sets, as a staged FASTX batch does, until it is
+ * freed; a batch too large for device memory fails with MGB_ERR_CUDA. */
+typedef struct mgb_device_results mgb_device_results_t;
+int mgb_align_batch_device(const mgb_index_t *index, const mgb_config_t *config, const char *d_seqs,
+                           const uint64_t *offsets, int offsets_on_device, uint32_t n_reads, void *stream,
+                           mgb_device_results_t **out);
+/* Element counts of the columns: n_reads, alignments, sequence bytes, CIGAR ops and node ids (0 with MGB_NODES_NONE). */
+typedef struct { uint64_t n_reads, n_alignments, sequence_bytes, cigar_ops, nodes; } mgb_device_sizes_t;
+int mgb_device_results_sizes(const mgb_device_results_t *res, mgb_device_sizes_t *sizes);
+/* The counters of the batch; num_seeds .. num_reads_retried equal mgb_align_batch's for the same reads. h2d_bytes and
+ * d2h_bytes count what crossed PCIe: up, the offsets and their k-mer offsets (16 bytes per read) and each pass's read
+ * list (4 bytes per read; pass 0's only when no read was answered before it); down, device offsets, 48 bytes per pass,
+ * each retry list and 32 bytes of totals. */
+const mgb_stats_t *mgb_device_results_stats(const mgb_device_results_t *res);
+/* Caller-allocated device arrays on index's device, sized from mgb_device_sizes_t. Alignment i has the mgb_alignment_t
+ * fields of the i-th record mgb_align_batch returns for the same reads, in the same order. */
+typedef struct {
+    uint64_t *read_first;        /* [n_reads + 1]: the alignments of read r are [read_first[r], read_first[r + 1]) */
+    uint32_t *read_index;        /* [n_alignments] each: the read's position in the batch, then the mgb_alignment_t fields */
+    uint8_t *orientation;
+    int32_t *score;
+    uint32_t *offset, *query_begin, *query_len, *num_nodes, *sequence_len, *num_cigar_ops;
+    char *sequence;              /* [sequence_bytes]: the path spellings, back to back */
+    uint64_t *sequence_offsets;  /* [n_alignments + 1] */
+    uint32_t *cigar;             /* [cigar_ops]: (len << 3) | op */
+    uint64_t *cigar_offsets;     /* [n_alignments + 1] */
+    uint64_t *nodes;             /* [nodes]: node ids (none with MGB_NODES_NONE) */
+    uint64_t *node_offsets;      /* [n_alignments + 1] */
+} mgb_device_columns_t;
+/* Enqueues the column writes on `stream` (cudaStream_t, NULL = legacy default) and returns without synchronising. A
+ * NULL pointer for an array with at least one element: MGB_ERR_INVALID_ARGUMENT. May be called more than once. */
+int mgb_device_results_write(const mgb_device_results_t *res, const mgb_device_columns_t *dst, void *stream);
+/* Waits for the last mgb_device_results_write, then returns the working memory to the index. NULL is a no-op. */
+void mgb_device_results_free(mgb_device_results_t *res);
+
 /* The text block of a result set of mgb_align_batch_text (owned by it); MGB_ERR_INVALID_ARGUMENT for a record set. */
 int mgb_results_text(const mgb_results_t *results, const char **text, uint64_t *bytes);
 

@@ -41,6 +41,20 @@ class mgb_stats_t(ctypes.Structure):
                [(n, ctypes.c_uint64) for n in ("h2d_bytes", "d2h_bytes", "kernel_launches")]
 
 
+class mgb_device_sizes_t(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_uint64) for n in ("n_reads", "n_alignments", "sequence_bytes", "cigar_ops", "nodes")]
+
+
+# mgb_device_columns_t: device pointers, in the order of include/mgb.h
+DEVICE_COLUMNS = ("read_first", "read_index", "orientation", "score", "offset", "query_begin", "query_len", "num_nodes",
+                  "sequence_len", "num_cigar_ops", "sequence", "sequence_offsets", "cigar", "cigar_offsets", "nodes",
+                  "node_offsets")
+
+
+class mgb_device_columns_t(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in DEVICE_COLUMNS]
+
+
 class mgb_boss_t(ctypes.Structure):
     _fields_ = [("n_plus_1", ctypes.c_uint64), ("W", ctypes.POINTER(ctypes.c_uint8)),
                 ("last", ctypes.POINTER(ctypes.c_uint8)), ("F", ctypes.c_uint64 * 32),
@@ -156,6 +170,16 @@ def load_library(path=None):
     L.mgb_set_pipeline_pieces.restype = None
     L.mgb_set_pipeline_pieces.argtypes = [u32]
     L.mgb_set_host_threads.restype = None
+    L.mgb_align_batch_device.restype = i
+    L.mgb_align_batch_device.argtypes = [vp, ctypes.POINTER(mgb_config_t), vp, vp, i, u32, vp, ctypes.POINTER(vp)]
+    L.mgb_device_results_sizes.restype = i
+    L.mgb_device_results_sizes.argtypes = [vp, ctypes.POINTER(mgb_device_sizes_t)]
+    L.mgb_device_results_stats.restype = ctypes.POINTER(mgb_stats_t)
+    L.mgb_device_results_stats.argtypes = [vp]
+    L.mgb_device_results_write.restype = i
+    L.mgb_device_results_write.argtypes = [vp, ctypes.POINTER(mgb_device_columns_t), vp]
+    L.mgb_device_results_free.restype = None
+    L.mgb_device_results_free.argtypes = [vp]
     L.mgb_set_host_threads.argtypes = [i]
     _libs[path] = L
     return L
@@ -177,7 +201,8 @@ REQUIRED_SYMBOLS = [
     "mgb_fastx_stage", "mgb_align_fastx_batch_text", "mgb_fastx_batch_free", "mgb_fastx_stage_bgzf",
     "mgb_fastx_batch_tail", "mgb_bgzf_inflate", "mgb_gzip_stream_create", "mgb_gzip_stream_free",
     "mgb_gzip_stream_state", "mgb_fastx_stage_gzip", "mgb_gzip_inflate", "mgb_gzip_stream_export_bytes",
-    "mgb_gzip_stream_export", "mgb_gzip_stream_import",
+    "mgb_gzip_stream_export", "mgb_gzip_stream_import", "mgb_align_batch_device", "mgb_device_results_sizes",
+    "mgb_device_results_stats", "mgb_device_results_write", "mgb_device_results_free",
 ]
 MGB_TEXT_TSV, MGB_TEXT_JSON = 1, 2
 MGB_FASTX_FWD_AND_REVERSE = 1

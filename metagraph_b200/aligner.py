@@ -10,6 +10,7 @@
 Everything computes through the C-ABI in include/mgb.h (metagraph_b200/_lib/libmgb.so).
 """
 import ctypes
+import dataclasses
 
 import numpy as np
 
@@ -125,6 +126,7 @@ class DBGSuccinctIndex:
             v.ctypes.data if v is not None else None, boss.k, boss.alphabet, suffix_len, device,
             ctypes.byref(h)))
         self.handle = h
+        self.device = int(device)
         if mode:     # DeBruijnGraph::Mode: 1 = CANONICAL (graph built from the sequences and their reverse complements)
             try:
                 _lib.check(self._L, self._L.mgb_index_set_mode(h, int(mode)))
@@ -143,7 +145,7 @@ class DBGSuccinctIndex:
         h = ctypes.c_void_p()
         _lib.check(self._L, self._L.mgb_index_replicate(self.handle, int(device), ctypes.byref(h)))
         rep = DBGSuccinctIndex.__new__(DBGSuccinctIndex)
-        rep._L, rep.k, rep.mode, rep.handle = self._L, self.k, self.mode, h
+        rep._L, rep.k, rep.mode, rep.handle, rep.device = self._L, self.k, self.mode, h, int(device)
         return rep
 
     def __del__(self):
@@ -401,6 +403,39 @@ def results_of_handle(L, res, seq_batch):
     return out
 
 
+@dataclasses.dataclass
+class DeviceAlignments:
+    """Alignments of B200Aligner.align_tensors as torch tensors on the index's device. The alignments of read r are
+    [read_first[r], read_first[r + 1]); alignment i has the fields of mgb_alignment_t (int32 for the uint32 ones), its
+    path spelling sequence[sequence_offsets[i]:sequence_offsets[i + 1]], its CIGAR words ((len << 3) | op) and node ids
+    likewise. nodes is empty when the config's result_nodes is MGB_NODES_NONE."""
+    read_first: object          # int64 [n_reads + 1]
+    read_index: object          # int32 [n_alignments]
+    orientation: object         # uint8
+    score: object               # int32
+    offset: object
+    query_begin: object
+    query_len: object
+    num_nodes: object
+    sequence_len: object
+    num_cigar_ops: object
+    sequence: object            # uint8 [sequence bytes]
+    sequence_offsets: object    # int64 [n_alignments + 1]
+    cigar: object               # int32 [CIGAR ops]
+    cigar_offsets: object       # int64 [n_alignments + 1]
+    nodes: object               # int64 [node ids]
+    node_offsets: object        # int64 [n_alignments + 1]
+    stats: dict
+
+
+def _column_dtypes(torch):
+    i32, i64 = torch.int32, torch.int64
+    return {"read_first": i64, "read_index": i32, "orientation": torch.uint8, "score": i32, "offset": i32,
+            "query_begin": i32, "query_len": i32, "num_nodes": i32, "sequence_len": i32, "num_cigar_ops": i32,
+            "sequence": torch.uint8, "sequence_offsets": i64, "cigar": i32, "cigar_offsets": i64, "nodes": i64,
+            "node_offsets": i64}
+
+
 class B200Aligner:
     """IDBGAligner over the H100 kernels (Seeder = SuffixSeeder<UniMEMSeeder>, Extender =
     DefaultColumnExtender, as DBGAligner<> in dbg_aligner.hpp:42-45)."""
@@ -441,6 +476,57 @@ class B200Aligner:
     def stats_of(self, res):
         st = self._L.mgb_results_stats(res).contents
         return {n: getattr(st, n) for n, _ in _lib.mgb_stats_t._fields_}
+
+    def align_tensors(self, reads, offsets):
+        """mgb_align_batch_device: aligns reads already in GPU memory and returns DeviceAlignments on that device.
+
+        reads: 1-D torch.uint8 tensor with stride 1 on the index's device (a slice that starts anywhere in its storage
+        is fine); offsets: int64 tensor [n + 1] on the CPU or on that device, read r = reads[offsets[r]:offsets[r + 1]].
+        The work is ordered after what is queued on torch's current stream, and the columns are written on it. With the
+        host-emulation library (tests) the "device" is the host and both tensors are CPU tensors."""
+        import torch
+        emu = hasattr(self._L, "mgb_emu_whole_read_hits")
+        device = torch.device("cpu") if emu else torch.device("cuda", self.graph.device)
+        if not isinstance(reads, torch.Tensor) or not isinstance(offsets, torch.Tensor):
+            raise ValueError("align_tensors takes torch tensors")
+        if reads.dtype != torch.uint8 or reads.dim() != 1 or (reads.numel() > 1 and reads.stride(0) != 1):
+            raise ValueError("reads must be a 1-D torch.uint8 tensor with stride 1")
+        if reads.device != device:
+            raise ValueError("reads must be on %s (the index's device), not %s" % (device, reads.device))
+        if offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1:
+            raise ValueError("offsets must be a 1-D torch.int64 tensor of n_reads + 1 entries")
+        if offsets.device not in (torch.device("cpu"), device):
+            raise ValueError("offsets must be on the CPU or on %s, not %s" % (device, offsets.device))
+        n_reads = offsets.numel() - 1
+        if n_reads >= 1 << 32:
+            raise ValueError("at most 2^32 - 1 reads per batch")
+        offsets = offsets.contiguous()
+        first, last = offsets[[0, -1]].tolist()
+        if first < 0 or last > reads.numel():
+            raise ValueError("offsets [%d, %d] outside the %d bytes of reads" % (first, last, reads.numel()))
+        on_device = not emu and offsets.device == device
+        stream = None if emu else torch.cuda.current_stream(device).cuda_stream
+        c = self.config.to_c() if not isinstance(self.config, mgb_config_t) else self.config
+        h = ctypes.c_void_p()
+        _lib.check(self._L, self._L.mgb_align_batch_device(self.graph.handle, ctypes.byref(c), reads.data_ptr() or None,
+                                                           offsets.data_ptr(), int(on_device), n_reads, stream,
+                                                           ctypes.byref(h)))
+        try:
+            z = _lib.mgb_device_sizes_t()
+            _lib.check(self._L, self._L.mgb_device_results_sizes(h, ctypes.byref(z)))
+            st = self._L.mgb_device_results_stats(h).contents
+            stats = {n: getattr(st, n) for n, _ in _lib.mgb_stats_t._fields_}
+            count = {"read_first": z.n_reads + 1, "sequence": z.sequence_bytes, "cigar": z.cigar_ops, "nodes": z.nodes,
+                     "sequence_offsets": z.n_alignments + 1, "cigar_offsets": z.n_alignments + 1,
+                     "node_offsets": z.n_alignments + 1}
+            out = {n: torch.empty(count.get(n, z.n_alignments), dtype=dt, device=device)
+                   for n, dt in _column_dtypes(torch).items()}
+            cols = _lib.mgb_device_columns_t(**{n: (t.data_ptr() if t.numel() else None) for n, t in out.items()})
+            _lib.check(self._L, self._L.mgb_device_results_write(h, ctypes.byref(cols), stream))
+        finally:
+            self._L.mgb_device_results_free(h)
+        self.last_stats = stats
+        return DeviceAlignments(stats=stats, **out)
 
     def align_batch(self, seq_batch, callback=None):
         """seq_batch: list of (header, sequence). Calls callback(header, AlignmentResults) in input

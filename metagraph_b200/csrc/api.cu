@@ -58,6 +58,7 @@ static void parallel_copy(char *dst, const char *src, uint64_t n) {
 #include "format_core.cuh"
 #include "fastx_core.cuh"
 #include "gzip_core.cuh"
+#include "columns_core.cuh"
 #include "fastx_host.hpp"
 #include "host_common.hpp"
 #include "index_build.hpp"
@@ -218,6 +219,7 @@ inline Region text_heap_slots(int pass) { return { "text heap", 40 + 8 * (size_t
 constexpr Region kInflateSlots { "inflate", 88, 96 };        // plain gzip input: a stage's decode scratch
 constexpr Region kTextSlots { "text", 96, SIZE_MAX };         // text route: the headers and the text
 static_assert(40 + 8 * kMaxPasses <= kTextSlots.base, "the text heaps end below the text region");
+static_assert(kMaxPasses <= kColumnsMaxPasses, "ColumnsArgs holds a heap per pass");
 
 #if defined(MGB_HOST_EMU)
 struct Workspace {};
@@ -1941,6 +1943,7 @@ struct Call {
     int text_format;                                    // 0: records; MGB_TEXT_TSV / MGB_TEXT_JSON
     int32_t min_path_score;
     bool dev_input;          // reads and headers are device memory (the file route), offsets host memory
+    bool device_results = false;   // mgb_align_batch_device: the passes are classified on the device (classify_pass)
 };
 
 // One contiguous range of reads [lo, lo + n) of a batch, processed start to finish on its own
@@ -2286,9 +2289,54 @@ struct PassState {
     std::vector<uint32_t> list;      // the pass's reads; empty on pass 0 after k_prepare_exact until its launches are in
     uint32_t n_pass = 0;
     std::vector<uint32_t> read_heap; // which pass produced the read's alignments
+    uint32_t L_retry = 0;            // device route: the longest read of list
+    uint8_t *pass_of = nullptr;      // device route: read_heap on the device
     float align_ms = 0, d2h_ms = 0;
     void all_reads(uint32_t n) { list.resize(n); std::iota(list.begin(), list.end(), 0u); }
 };
+
+// Device route (mgb_align_batch_device): the classification of run_pass on the device (k_pass_classify). Only the
+// pass's summary comes back, and the list of the reads that overflowed when there are any: it becomes ps->list.
+static int classify_pass(const Call &c, const Batch &b, const Seeded &sd, int pass, const uint32_t *d_list,
+                         uint32_t n_list, DevBufs &heap_bufs, Stream &st, PassState *ps, Piece *res) {
+    constexpr size_t kSumWords = sizeof(PassSummary) / 4;
+    uint32_t *d_block = nullptr;                 // the summary, then the retry list
+    int rc;
+    if ((rc = heap_bufs.alloc(&d_block, kSumWords + n_list)) || (rc = dev_zero(d_block, sizeof(PassSummary), st))) return rc;
+    const ClassifyArgs a { d_list, n_list, sd.hdr, b.offsets, ps->pass_of, (uint32_t)pass,
+                           reinterpret_cast<PassSummary*>(d_block), d_block + kSumWords };
+#if defined(MGB_HOST_EMU)
+    (void)c;
+    for (uint32_t t = 0; t < n_list; ++t) {
+        const uint32_t r = a.list ? a.list[t] : t;
+        if (classify_read(a, r, *a.sum)) { MGB_EMU_HIT(EMU_READ_OVERFLOW); a.retry[a.sum->n_retry++] = r; }
+    }
+#else
+    if (n_list) {
+        const unsigned grid = (unsigned)kern_dna::read_path_grid(std::min<uint64_t>((n_list + 255) / 256, (uint64_t)c.index->num_sms * 8));
+        kern_dna::log_launch("k_pass_classify", grid, 256, (uint64_t)grid * 256, n_list);     // a lane per read
+        k_pass_classify<<<grid, 256, 0, st.s>>>(a);
+        CUDA_TRY(cudaGetLastError());
+    }
+#endif
+    PassSummary sum;
+    record(st, 3);
+    if ((rc = d2h(&sum, a.sum, sizeof(sum), st)) || (rc = sync(st))) return rc;
+    ps->list.resize(sum.n_retry);
+    if (sum.n_retry && ((rc = d2h(ps->list.data(), a.retry, (size_t)sum.n_retry * 4, st)) || (rc = sync(st)))) return rc;
+    record(st, 4);
+    if ((rc = sync(st))) return rc;
+    ps->d2h_ms += elapsed_ms(st, 3, 4);
+    std::sort(ps->list.begin(), ps->list.end());     // the record route's order, so every pass runs as it does there
+    mgb_stats_t &s = res->stats;
+    s.num_seeds += sum.num_seeds; s.num_extensions += sum.num_extensions; s.num_explored_nodes += sum.num_explored_nodes;
+    s.dp_cells += sum.dp_cells; s.dp_columns += sum.dp_columns; s.num_reads_retried += sum.n_retry;
+    s.d2h_bytes += sizeof(PassSummary) + (uint64_t)sum.n_retry * 4;
+    s.kernel_launches += n_list ? 1 : 0;
+    ps->n_pass = sum.n_retry;
+    ps->L_retry = sum.max_retry_len;
+    return 0;
+}
 
 // One align pass over ps->list: its buffers (or those pass 0 takes over from k_prepare_exact), k_exact_reads and
 // k_align, the download of the headers (and on the record route the heap), and the classification of the reads. The
@@ -2384,6 +2432,8 @@ static int run_pass(const Call &c, const Batch &b, const Seeded &sd, const PassP
                  (double)ph[3] / n_align, (double)ph[4] / n_align, (double)ph[5] / n_align,
                  (double)ph[6] / n_align, n_align);
 #endif
+    if (c.device_results) return classify_pass(c, b, sd, pass, listed ? nullptr : d_list, listed ? n_reads : n_pass,
+                                               heap_bufs, st, ps, res);
     if (used > heap_cap) used = heap_cap;
     if (text) used = 0;                        // the records stay on the device
     else {
@@ -2720,6 +2770,206 @@ static int fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes
     else *consumed = dev->consumed;
     return MGB_OK;
 }
+
+} // extern "C"
+
+// ---------------------------------------------------------------------------------------
+// device-resident batches (mgb_align_batch_device): align_range's stages on reads already in device memory, one piece
+// on one stream; the passes are classified on the device and the records stay in the pass heaps until the caller's
+// columns are written (columns_core.cuh)
+// ---------------------------------------------------------------------------------------
+struct mgb_device_results {
+    explicit mgb_device_results(const mgb_index_t *ix) : cw(ix) {}
+    ~mgb_device_results();
+    CallWorkspace cw;                 // the working memory the columns are read from, held until the handle is freed
+    std::deque<DevBufs> bufs;         // the batch's buffers, every pass's heap and the columns' counts
+    ColumnsArgs ca;
+    mgb_device_sizes_t sizes;
+    mgb_stats_t stats;
+#if !defined(MGB_HOST_EMU)
+    mutable cudaEvent_t written = nullptr;     // recorded after the last mgb_device_results_write
+#endif
+};
+
+mgb_device_results::~mgb_device_results() {
+#if !defined(MGB_HOST_EMU)
+    if (written) { cudaEventSynchronize(written); cudaEventDestroy(written); }
+#endif
+}
+
+#if !defined(MGB_HOST_EMU)
+static bool on_device(const void *p, int device) {
+    cudaPointerAttributes at;
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == device;
+}
+#endif
+
+static int align_device(const mgb_index_t *index, const mgb_config_t *config, const char *d_seqs, const uint64_t *offsets,
+                        bool offsets_on_device, uint32_t n_reads, void *stream, mgb_device_results *res) {
+    DevConfig dcfg;
+    std::string err;
+    int rc = lower_config(*config, index->view.k, index->alphabet, &dcfg, &err);
+    if (rc) return fail(rc, err);
+    if (index->view.mode != 0) { dcfg.canonical = 1; dcfg.forward_and_reverse_complement = 1; }   // as align_batch
+    Piece piece;
+    mgb_stats_t &stats = piece.stats;
+    std::memset(&stats, 0, sizeof(stats));
+    CallWorkspace &cw = res->cw;
+    if ((rc = cw.ready())) return rc;
+    Stream &st = cw.st;
+#if !defined(MGB_HOST_EMU)
+    if ((d_seqs && !on_device(d_seqs, index->device)) || (offsets_on_device && !on_device(offsets, index->device)))
+        return fail(MGB_ERR_INVALID_ARGUMENT, "the reads (and device offsets) must be device memory on the index's device");
+    {   // the caller's work queued on its stream comes first
+        cudaEvent_t ev;
+        CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        cudaError_t e = cudaEventRecord(ev, (cudaStream_t)stream);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(st.s, ev, 0);
+        cudaEventDestroy(ev);
+        CUDA_TRY(e);
+    }
+#else
+    (void)stream;
+#endif
+    record(st, 0);
+    // the offsets on the host, relative to the first read (upload_batch checks them)
+    std::vector<uint64_t> offs((size_t)n_reads + 1);
+    if (offsets_on_device) {
+        if ((rc = d2h(offs.data(), offsets, offs.size() * 8, st)) || (rc = sync(st))) return rc;
+        stats.d2h_bytes += offs.size() * 8;
+    } else {
+        std::memcpy(offs.data(), offsets, offs.size() * 8);
+    }
+    const uint64_t base = offs[0];
+    if (offs[n_reads] < base) return fail(MGB_ERR_INVALID_ARGUMENT, "offsets must be non-decreasing");
+    const uint64_t chars = offs[n_reads] - base;
+    if (!d_seqs && chars) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    for (uint64_t &o : offs) o -= base;
+    // The reads are copied into the batch's own buffer first: k_prepare_exact's word loads and the other kernels' reads
+    // past a read's end assume a 16-byte-aligned base and 64 bytes of slack, which a caller's buffer need not have.
+    DevBufs &bufs = res->bufs.emplace_back(st, cw.w, kBatchSlots);
+    char *seqs = nullptr;
+    if ((rc = bufs.alloc(&seqs, chars + 64))) return rc;
+#if defined(MGB_HOST_EMU)
+    if (chars) std::memcpy(seqs, d_seqs + base, chars);
+#else
+    if (chars) CUDA_TRY(cudaMemcpyAsync(seqs, d_seqs + base, chars, cudaMemcpyDeviceToDevice, st.s));
+#endif
+    Batch b; std::vector<uint64_t> koff;
+    if ((rc = upload_batch(index, seqs, offs.data(), n_reads, dcfg.forward_and_reverse_complement, st, bufs, &b, &koff,
+                           &stats, true)))
+        return rc;
+    const Call c { index, dcfg, seqs, offs.data(), nullptr, nullptr, 0, config->min_path_score, true, true };
+    int lq = b.L_max + 1 <= 512 ? (int)((b.L_max + 1 + 15) & ~15u) : 0;      // as align_range
+    if (const char *e = std::getenv("MGB_TEST_LQ")) lq = std::atoi(e);
+    Seeded sd;
+    if ((rc = prepare_and_seed(c, b, lq, st, bufs, &sd, &stats))) return rc;
+
+    DevBufs &cb = res->bufs.emplace_back(st, cw.w, kTextSlots);
+    PassState ps;
+    if ((rc = cb.alloc(&ps.pass_of, (size_t)n_reads + 1))) return rc;
+    ps.n_pass = n_reads;
+    if (!sd.prep_exact) ps.all_reads(n_reads);
+    TextArgs ta;                     // (run_pass leaves every pass's heap in ta.heap)
+    std::memset(&ta, 0, sizeof(ta));
+    Ticks tick { std::getenv("MGB_DEBUG") != nullptr, 0, n_reads };
+    for (int pass = 0; ps.n_pass; ++pass) {
+        const uint32_t scale = 1u << (2 * pass);
+        if (pass == kMaxPasses) return fail(MGB_ERR_OVERFLOW, "a read exceeded the largest per-read work arena");
+        const uint32_t L_pass = pass ? ps.L_retry : b.L_max;
+        if (pass > 0 || !sd.prep_exact) stats.h2d_bytes += (uint64_t)ps.n_pass * 4;     // run_pass uploads the list
+        DevBufs arena_bufs(st, cw.w, kArenaSlots);
+        DevBufs &heap_bufs = res->bufs.emplace_back(st, cw.w, text_heap_slots(pass));
+        PassPlan plan;
+        if ((rc = pass_plan(c, b, L_pass, scale, lq, ps.n_pass, arena_bufs, &plan))
+            || (rc = run_pass(c, b, sd, plan, pass, scale, lq, seqs, offs.data(), koff, arena_bufs, heap_bufs, nullptr,
+                              st, tick, &ps, &ta, &piece)))
+            return rc;
+    }
+
+    // every read's alignments, sequence bytes, CIGAR ops and node ids; their scans; the totals come down
+    ColumnsArgs &ca = res->ca;
+    std::memset(&ca, 0, sizeof(ca));
+    ca.hdr = sd.hdr; ca.pass_of = ps.pass_of;
+    for (int p = 0; p < kMaxPasses; ++p) ca.heap[p] = ta.heap[p];
+    ca.n_reads = n_reads; ca.no_nodes = dcfg.result_nodes != 0;
+    for (uint64_t *&x : ca.cnt) if ((rc = cb.alloc(&x, (size_t)n_reads + 1))) return rc;
+#if defined(MGB_HOST_EMU)
+    for (uint32_t r = 0; r < n_reads; ++r) columns_size_read(ca, r);
+#else
+    if (n_reads) {
+        const unsigned grid = (unsigned)kern_dna::read_path_grid(std::min<uint64_t>((n_reads + 7) / 8, (uint64_t)index->num_sms * 16));
+        kern_dna::log_launch("k_columns_size", grid, 256, (uint64_t)grid * 8, n_reads);     // a warp per read
+        k_columns_size<<<grid, 256, 0, st.s>>>(ca);
+        CUDA_TRY(cudaGetLastError());
+    }
+#endif
+    for (uint64_t *x : ca.cnt) if ((rc = scan_u64(x, n_reads, st, cb))) return rc;
+    uint64_t tot[4];
+    for (int i = 0; i < 4; ++i) if ((rc = d2h(&tot[i], ca.cnt[i] + n_reads, 8, st))) return rc;
+    if ((rc = sync(st))) return rc;
+    stats.d2h_bytes += sizeof(tot);
+    stats.kernel_launches += (n_reads ? 1 : 0) + 4 * (n_reads ? 3 : 2);
+    stats.h2d_ms = elapsed_ms(st, 0, 1);
+    stats.seed_kernel_ms = elapsed_ms(st, 1, 2);
+    stats.align_kernel_ms = ps.align_ms; stats.d2h_ms = ps.d2h_ms;
+    res->sizes = mgb_device_sizes_t { n_reads, tot[0], tot[1], tot[2], tot[3] };
+    res->stats = stats;
+    return MGB_OK;
+}
+
+extern "C" {
+
+int mgb_align_batch_device(const mgb_index_t *index, const mgb_config_t *config, const char *d_seqs,
+                           const uint64_t *offsets, int offsets_on_device, uint32_t n_reads, void *stream,
+                           mgb_device_results_t **out) {
+    if (!index || !config || !offsets || !out) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    std::unique_ptr<mgb_device_results> res(new mgb_device_results(index));
+    if (const int rc = align_device(index, config, d_seqs, offsets, offsets_on_device != 0, n_reads, stream, res.get()))
+        return rc;
+    *out = res.release();
+    return MGB_OK;
+}
+
+int mgb_device_results_sizes(const mgb_device_results_t *res, mgb_device_sizes_t *sizes) {
+    if (!res || !sizes) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    *sizes = res->sizes;
+    return MGB_OK;
+}
+
+const mgb_stats_t *mgb_device_results_stats(const mgb_device_results_t *res) { return res ? &res->stats : nullptr; }
+
+int mgb_device_results_write(const mgb_device_results_t *res, const mgb_device_columns_t *dst, void *stream) {
+    if (!res || !dst) return fail(MGB_ERR_INVALID_ARGUMENT, "null argument");
+    const mgb_device_sizes_t &z = res->sizes;
+    const mgb_device_columns_t &d = *dst;
+    if (!d.read_first || !d.sequence_offsets || !d.cigar_offsets || !d.node_offsets
+        || (z.n_alignments && (!d.read_index || !d.orientation || !d.score || !d.offset || !d.query_begin || !d.query_len
+                               || !d.num_nodes || !d.sequence_len || !d.num_cigar_ops))
+        || (z.sequence_bytes && !d.sequence) || (z.cigar_ops && !d.cigar) || (z.nodes && !d.nodes))
+        return fail(MGB_ERR_INVALID_ARGUMENT, "a column with at least one element has a null pointer");
+    ColumnsArgs a = res->ca;
+    a.dst = d;
+#if defined(MGB_HOST_EMU)
+    (void)stream;
+    columns_write_ends(a);
+    for (uint32_t r = 0; r < a.n_reads; ++r) columns_write_read(a, r);
+#else
+    const mgb_index_t *index = res->cw.ix;
+    CUDA_TRY(cudaSetDevice(index->device));
+    const unsigned grid = (unsigned)std::max<uint64_t>(1, kern_dna::read_path_grid(
+        std::min<uint64_t>((a.n_reads + 7) / 8, (uint64_t)index->num_sms * 16)));
+    kern_dna::log_launch("k_columns_write", grid, 256, (uint64_t)grid * 8, a.n_reads);     // a warp per read
+    k_columns_write<<<grid, 256, 0, (cudaStream_t)stream>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    if (!res->written) CUDA_TRY(cudaEventCreateWithFlags(&res->written, cudaEventDisableTiming));
+    CUDA_TRY(cudaEventRecord(res->written, (cudaStream_t)stream));
+#endif
+    return MGB_OK;
+}
+
+void mgb_device_results_free(mgb_device_results_t *res) { delete res; }
 
 } // extern "C"
 
