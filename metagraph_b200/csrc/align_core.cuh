@@ -154,6 +154,21 @@ struct OutAln {
     uint32_t n_nodes, seq_len, n_cigar;
 };
 
+// One alignment of a read's packed records (OutAln | node ids unless result_nodes | CIGAR | sequence, each part padded
+// to 8, as k_align and the whole-read writers pack them): the reader every consumer of the heaps goes through
+struct RecView {
+    OutAln o; const uint64_t *nodes; const uint32_t *cigar; const char *seq;
+};
+MGB_HOSTDEV const char *rec_next(const char *p, bool no_nodes, RecView *v) {
+    v->o = *reinterpret_cast<const OutAln*>(p);
+    p += sizeof(OutAln);
+    v->nodes = no_nodes ? nullptr : reinterpret_cast<const uint64_t*>(p);
+    if (!no_nodes) p += 8ull * v->o.n_nodes;
+    v->cigar = reinterpret_cast<const uint32_t*>(p); p += (4ull * v->o.n_cigar + 7) & ~7ull;
+    v->seq = p; p += ((uint64_t)v->o.seq_len + 7) & ~7ull;
+    return p;
+}
+
 struct ReadStats { uint32_t num_seeds, num_extensions, num_explored_nodes, dp_columns; uint64_t dp_cells; };
 #if defined(MGB_HOST_EMU)
 extern "C" unsigned long long mgb_emu_whole_read_hits;   // host emulation (tests) only: reads answered by exact_read_strand()

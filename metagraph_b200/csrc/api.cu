@@ -209,16 +209,16 @@ inline void hostbuf_release(HostBuf b) { g_pinned_pool.release(b); }
 // index keeps between calls (slot i = the i-th request of the call): cudaMalloc of GB-sized arenas per
 // call is slow, and stream-ordered pools stall when two streams trade memory back and forth.
 // Every DevBufs takes consecutive slots of one region, and an allocation past the region's end fails, in both builds.
-constexpr int kMaxPasses = 6;          // align_range gives up on a read after six passes
+constexpr int kMaxPasses = 6;          // align_piece gives up on a read after six passes
 struct Region { const char *name; size_t base, end; };
 constexpr Region kBatchSlots { "batch", 0, 32 };              // the batch's buffers; the file route's parse
 constexpr Region kArenaSlots { "arena", 32, 33 };             // the align pass's arena
 constexpr Region kPassHeapSlots { "pass heap", 33, 40 };      // record route: the heap, list and counters of a pass
-// text route: every pass keeps its heap on the device until the text is rendered
-inline Region text_heap_slots(int pass) { return { "text heap", 40 + 8 * (size_t)pass, 48 + 8 * (size_t)pass }; }
+// text and columns routes: every pass keeps its heap on the device until the text or the columns are made from it
+inline Region kept_heap_slots(int pass) { return { "kept heap", 40 + 8 * (size_t)pass, 48 + 8 * (size_t)pass }; }
 constexpr Region kInflateSlots { "inflate", 88, 96 };        // plain gzip input: a stage's decode scratch
 constexpr Region kTextSlots { "text", 96, SIZE_MAX };         // text route: the headers and the text
-static_assert(40 + 8 * kMaxPasses <= kTextSlots.base, "the text heaps end below the text region");
+static_assert(40 + 8 * kMaxPasses <= kTextSlots.base, "the kept heaps end below the text region");
 static_assert(kMaxPasses <= kColumnsMaxPasses, "ColumnsArgs holds a heap per pass");
 
 #if defined(MGB_HOST_EMU)
@@ -1150,7 +1150,7 @@ struct TextArgs {
     const char *names; const uint64_t *name_off;     // and their headers
     const ReadHdr *hdr;                              // per read: n_aln and heap_off of the pass that answered it
     const uint8_t *pass;                             // ... and that pass
-    const char *heap[kMaxPasses];                    // the output heap of every pass
+    const char *heap[kMaxPasses];                    // the output heap of every pass (PassState::heap)
     uint32_t n_reads, k, json, result_nodes;
     int32_t min_path_score;
     uint64_t *off;         // k_text_size: bytes of each read's text; after the scan its offset, off[n_reads] = total
@@ -1164,14 +1164,12 @@ template <class S> MGB_HD void text_read(const TextArgs &a, uint32_t r, S &s) {
     const uint32_t n_aln = a.hdr[r].n_aln;
     const char *p = n_aln ? a.heap[a.pass[r]] + a.hdr[r].heap_off : nullptr;
     if (!a.json) tsv_head(s, rd);
-    for (uint32_t i = 0; i < n_aln; ++i) {            // OutAln | node ids (unless result_nodes) | CIGAR | sequence
-        const OutAln o = *reinterpret_cast<const OutAln*>(p);
-        TextAln t { o.orientation, o.score, o.offset, o.query_begin, o.query_len, o.n_nodes, o.seq_len, o.n_cigar,
-                    nullptr, nullptr, nullptr };
-        p += sizeof(OutAln);
-        if (!a.result_nodes) { t.nodes = reinterpret_cast<const uint64_t*>(p); p += 8ull * o.n_nodes; }
-        t.cigar = reinterpret_cast<const uint32_t*>(p); p += (4ull * o.n_cigar + 7) & ~7ull;
-        t.seq = p; p += ((uint64_t)o.seq_len + 7) & ~7ull;
+    for (uint32_t i = 0; i < n_aln; ++i) {
+        RecView v;
+        p = rec_next(p, a.result_nodes != 0, &v);
+        const OutAln &o = v.o;
+        const TextAln t { o.orientation, o.score, o.offset, o.query_begin, o.query_len, o.n_nodes, o.seq_len, o.n_cigar,
+                          v.nodes, v.cigar, v.seq };
         if (a.json) json_aln(s, rd, t, i > 0, a.k); else tsv_aln(s, t);
     }
     if (!a.json) {
@@ -1934,16 +1932,21 @@ static void debug_left_over(const IndexView &ix, const PrepExactArgs &pa, const 
     }
 }
 
-// What is the same for every piece of one mgb_align_batch / mgb_align_batch_text call
+// Where a call's alignments go. records: mgb_alignment_t on the host (mgb_align_batch); text: TSV or JSON rendered on
+// the device (mgb_align_batch_text and the file route); columns: the caller's device arrays (mgb_align_batch_device),
+// with every pass classified on the device. The text and columns routes keep every pass's heap on the device.
+enum class Route { records, text, columns };
+
+// What is the same for every piece of one call
 struct Call {
     const mgb_index_t *index;
     const DevConfig &dcfg;
+    Route route;
     const char *seqs; const uint64_t *offsets;          // the batch's reads
     const char *names; const uint64_t *name_offsets;    // text route: their headers
-    int text_format;                                    // 0: records; MGB_TEXT_TSV / MGB_TEXT_JSON
+    int text_format;                                    // text route: MGB_TEXT_TSV / MGB_TEXT_JSON
     int32_t min_path_score;
-    bool dev_input;          // reads and headers are device memory (the file route), offsets host memory
-    bool device_results = false;   // mgb_align_batch_device: the passes are classified on the device (classify_pass)
+    bool dev_input;          // reads (and headers) are device memory (the file and columns routes), offsets host memory
 };
 
 // One contiguous range of reads [lo, lo + n) of a batch, processed start to finish on its own
@@ -1964,7 +1967,7 @@ struct Piece {
     uint64_t *src_off = nullptr; uint32_t *src_heap = nullptr;   // views into the enclosing mgb_results
     HostBuf text;                    // text route: the piece's text
     uint64_t text_bytes = 0;
-    mgb_stats_t stats;
+    mgb_stats_t stats = {};
     int rc = 0; std::string err;
     ~Piece() { for (HostBuf b : heaps) hostbuf_release(b); if (text.p) hostbuf_release(text); }
 };
@@ -1991,20 +1994,18 @@ static const uint64_t *rebase_offsets(const uint64_t *all, uint32_t lo, uint32_t
     return local->data();
 }
 
-// the packed records of one read (OutAln | node ids unless no_nodes | CIGAR | sequence) as `count` mgb_alignment_t
+// the packed records of one read as `count` mgb_alignment_t
 static void unpack_records(const char *p, uint32_t count, bool no_nodes, uint32_t read_index, mgb_alignment_t *dst) {
     for (uint32_t i = 0; i < count; ++i) {
-        const OutAln *o = (const OutAln*)p;
+        RecView v;
+        p = rec_next(p, no_nodes, &v);
+        const OutAln &o = v.o;
         mgb_alignment_t al;
         std::memset(&al, 0, sizeof(al));
-        al.read_index = read_index; al.orientation = (uint8_t)o->orientation; al.score = o->score;
-        al.offset = o->offset; al.query_begin = o->query_begin; al.query_len = o->query_len;
-        al.num_nodes = o->n_nodes; al.sequence_len = o->seq_len; al.num_cigar_ops = o->n_cigar;
-        p += sizeof(OutAln);
-        if (no_nodes) al.nodes = nullptr;
-        else { al.nodes = (const uint64_t*)p; p += 8ull * o->n_nodes; }
-        al.cigar = (const uint32_t*)p; p += (4ull * o->n_cigar + 7) & ~7ull;
-        al.sequence = p; p += ((uint64_t)o->seq_len + 7) & ~7ull;
+        al.read_index = read_index; al.orientation = (uint8_t)o.orientation; al.score = o.score;
+        al.offset = o.offset; al.query_begin = o.query_begin; al.query_len = o.query_len;
+        al.num_nodes = o.n_nodes; al.sequence_len = o.seq_len; al.num_cigar_ops = o.n_cigar;
+        al.nodes = v.nodes; al.cigar = v.cigar; al.sequence = v.seq;
         dst[i] = al;
     }
 }
@@ -2059,10 +2060,10 @@ static int launch_subk(const mgb_index_t *index, const SubkArgs &sk, uint32_t L_
     return 0;
 }
 
-// text route: the piece's headers go up with its reads, and the text's arguments are set
-static int upload_headers(const Call &c, const Batch &b, const char *names, const uint64_t *name_offs, Stream &st,
+// text route: the piece's headers go up ahead of its reads, and the text's arguments that do not come from the passes
+// are set
+static int upload_headers(const Call &c, uint32_t n_reads, const char *names, const uint64_t *name_offs, Stream &st,
                           DevBufs &text_bufs, TextArgs *ta, mgb_stats_t *stats) {
-    const uint32_t n_reads = b.n_reads;
     const uint64_t name_bytes = name_offs[n_reads];
     char *d_names = c.dev_input ? const_cast<char*>(names) : nullptr; uint64_t *d_name_off = nullptr;
     int rc = c.dev_input ? 0 : text_bufs.alloc(&d_names, name_bytes + 64);
@@ -2070,7 +2071,7 @@ static int upload_headers(const Call &c, const Batch &b, const char *names, cons
     if (!rc && name_bytes && !c.dev_input) rc = h2d(d_names, names, name_bytes, st);
     if (!rc) rc = h2d(d_name_off, name_offs, ((size_t)n_reads + 1) * 8, st);
     stats->h2d_bytes += (c.dev_input ? 0 : name_bytes) + ((size_t)n_reads + 1) * 8;
-    ta->seqs = b.seqs; ta->offsets = b.offsets; ta->names = d_names; ta->name_off = d_name_off;
+    ta->names = d_names; ta->name_off = d_name_off;
     ta->n_reads = n_reads; ta->k = c.index->view.k; ta->json = c.text_format == MGB_TEXT_JSON;
     ta->result_nodes = c.dcfg.result_nodes; ta->min_path_score = c.min_path_score;
     return rc;
@@ -2284,21 +2285,33 @@ static void debug_exact_counts(const Call &c, uint32_t lo, const Batch &b, const
 #endif
 }
 
-// The align passes of a piece so far
+// The align passes of a piece so far. Whether run_pass classifies a pass on the host (into read_heap) or on the device
+// (into pass_of), it leaves the next pass's list in read order, its length and its longest read here.
 struct PassState {
     std::vector<uint32_t> list;      // the pass's reads; empty on pass 0 after k_prepare_exact until its launches are in
     uint32_t n_pass = 0;
-    std::vector<uint32_t> read_heap; // which pass produced the read's alignments
-    uint32_t L_retry = 0;            // device route: the longest read of list
-    uint8_t *pass_of = nullptr;      // device route: read_heap on the device
+    uint32_t L_retry = 0;            // the longest read of list, after the first pass: it sizes the next pass's arena
+    const char *heap[kMaxPasses] = {};   // every pass's output heap on the device
+    std::vector<uint8_t> read_heap;  // host classification: the pass that answered each read (its heap of the piece)
+    ReadHdr *hdr_host = nullptr;     // host classification: the headers of the pass, downloaded
+    uint8_t *pass_of = nullptr;      // device classification: read_heap on the device
     float align_ms = 0, d2h_ms = 0;
     void all_reads(uint32_t n) { list.resize(n); std::iota(list.begin(), list.end(), 0u); }
 };
 
-// Device route (mgb_align_batch_device): the classification of run_pass on the device (k_pass_classify). Only the
-// pass's summary comes back, and the list of the reads that overflowed when there are any: it becomes ps->list.
+// k_pass_classify's work one read after the other: the host classification, and the device one in the emulation build.
+// a.retry may be a.list, which is then compacted in place.
+static void classify_reads(const ClassifyArgs &a) {
+    for (uint32_t t = 0; t < a.n_list; ++t) {
+        const uint32_t r = a.list ? a.list[t] : t;
+        if (classify_read(a, r, *a.sum)) { MGB_EMU_HIT(EMU_READ_OVERFLOW); a.retry[a.sum->n_retry++] = r; }
+    }
+}
+
+// The classification on the device (k_pass_classify): only the summary comes back, into *sum, and the list of the reads
+// that overflowed when there are any, into ps->list.
 static int classify_pass(const Call &c, const Batch &b, const Seeded &sd, int pass, const uint32_t *d_list,
-                         uint32_t n_list, DevBufs &heap_bufs, Stream &st, PassState *ps, Piece *res) {
+                         uint32_t n_list, DevBufs &heap_bufs, Stream &st, PassState *ps, PassSummary *sum, Piece *res) {
     constexpr size_t kSumWords = sizeof(PassSummary) / 4;
     uint32_t *d_block = nullptr;                 // the summary, then the retry list
     int rc;
@@ -2307,10 +2320,7 @@ static int classify_pass(const Call &c, const Batch &b, const Seeded &sd, int pa
                            reinterpret_cast<PassSummary*>(d_block), d_block + kSumWords };
 #if defined(MGB_HOST_EMU)
     (void)c;
-    for (uint32_t t = 0; t < n_list; ++t) {
-        const uint32_t r = a.list ? a.list[t] : t;
-        if (classify_read(a, r, *a.sum)) { MGB_EMU_HIT(EMU_READ_OVERFLOW); a.retry[a.sum->n_retry++] = r; }
-    }
+    classify_reads(a);
 #else
     if (n_list) {
         const unsigned grid = (unsigned)kern_dna::read_path_grid(std::min<uint64_t>((n_list + 255) / 256, (uint64_t)c.index->num_sms * 8));
@@ -2319,35 +2329,28 @@ static int classify_pass(const Call &c, const Batch &b, const Seeded &sd, int pa
         CUDA_TRY(cudaGetLastError());
     }
 #endif
-    PassSummary sum;
     record(st, 3);
-    if ((rc = d2h(&sum, a.sum, sizeof(sum), st)) || (rc = sync(st))) return rc;
-    ps->list.resize(sum.n_retry);
-    if (sum.n_retry && ((rc = d2h(ps->list.data(), a.retry, (size_t)sum.n_retry * 4, st)) || (rc = sync(st)))) return rc;
+    if ((rc = d2h(sum, a.sum, sizeof(*sum), st)) || (rc = sync(st))) return rc;
+    ps->list.resize(sum->n_retry);
+    if (sum->n_retry && ((rc = d2h(ps->list.data(), a.retry, (size_t)sum->n_retry * 4, st)) || (rc = sync(st)))) return rc;
     record(st, 4);
     if ((rc = sync(st))) return rc;
     ps->d2h_ms += elapsed_ms(st, 3, 4);
-    std::sort(ps->list.begin(), ps->list.end());     // the record route's order, so every pass runs as it does there
-    mgb_stats_t &s = res->stats;
-    s.num_seeds += sum.num_seeds; s.num_extensions += sum.num_extensions; s.num_explored_nodes += sum.num_explored_nodes;
-    s.dp_cells += sum.dp_cells; s.dp_columns += sum.dp_columns; s.num_reads_retried += sum.n_retry;
-    s.d2h_bytes += sizeof(PassSummary) + (uint64_t)sum.n_retry * 4;
-    s.kernel_launches += n_list ? 1 : 0;
-    ps->n_pass = sum.n_retry;
-    ps->L_retry = sum.max_retry_len;
+    std::sort(ps->list.begin(), ps->list.end());     // read order, as the host classification leaves it
+    res->stats.d2h_bytes += sizeof(PassSummary) + (uint64_t)sum->n_retry * 4;
+    res->stats.kernel_launches += n_list ? 1 : 0;
     return 0;
 }
 
 // One align pass over ps->list: its buffers (or those pass 0 takes over from k_prepare_exact), k_exact_reads and
-// k_align, the download of the headers (and on the record route the heap), and the classification of the reads. The
-// reads that overflowed their arena become ps->list, the next pass's reads.
+// k_align, then the classification of the reads, on the columns route on the device, on the others on the host after
+// the download of the headers (and on the record route the heap). The reads that overflowed their arena become
+// ps->list, the next pass's reads.
 static int run_pass(const Call &c, const Batch &b, const Seeded &sd, const PassPlan &p, int pass, uint32_t scale,
                     int lq, const char *seqs, const uint64_t *offsets, const std::vector<uint64_t> &koff,
-                    DevBufs &arena_bufs, DevBufs &heap_bufs, ReadHdr *hdr_host, Stream &st, Ticks &tick,
-                    PassState *ps, TextArgs *ta, Piece *res) {
+                    DevBufs &arena_bufs, DevBufs &heap_bufs, Stream &st, Ticks &tick, PassState *ps, Piece *res) {
     const mgb_index_t *index = c.index;
     const uint32_t k = index->view.k, n_reads = b.n_reads, n_pass = ps->n_pass;
-    const bool text = c.text_format != 0;
     const bool listed = pass == 0 && sd.prep_exact;      // pass 0 after k_prepare_exact
     const uint64_t heap_cap = listed ? sd.pa.ex.heap_cap : heap_cap_of(b, c.dcfg, k, n_pass, scale);
     char *d_arena = nullptr, *d_heap = nullptr; uint32_t *d_list = nullptr, *d_rest = nullptr;
@@ -2363,11 +2366,13 @@ static int run_pass(const Call &c, const Batch &b, const Seeded &sd, const PassP
             || (sd.exact_reads && (rc = heap_bufs.alloc(&d_rest, n_pass))))
             return rc;
     }
-    ta->heap[pass] = d_heap;
+    ps->heap[pass] = d_heap;
     tick("pass: arena/heap alloc");
     if (!listed && ((rc = h2d(d_list, ps->list.data(), (size_t)n_pass * 4, st)) || (rc = dev_zero(d_used, 8, st))
                     || (rc = dev_zero(d_next, 16, st))))
         return rc;
+    // only the columns route counts the list in h2d_bytes (the record route's count is the one bench.py reports)
+    if (!listed && c.route == Route::columns) res->stats.h2d_bytes += (uint64_t)n_pass * 4;
     // the read-dependent part of the gate (exact_read_strand); max_len keeps what k_align's own exit required
     ExactArgs ea;
     std::memset(&ea, 0, sizeof(ea));
@@ -2432,65 +2437,101 @@ static int run_pass(const Call &c, const Batch &b, const Seeded &sd, const PassP
                  (double)ph[3] / n_align, (double)ph[4] / n_align, (double)ph[5] / n_align,
                  (double)ph[6] / n_align, n_align);
 #endif
-    if (c.device_results) return classify_pass(c, b, sd, pass, listed ? nullptr : d_list, listed ? n_reads : n_pass,
-                                               heap_bufs, st, ps, res);
-    if (used > heap_cap) used = heap_cap;
-    if (text) used = 0;                        // the records stay on the device
-    else {
-        HostBuf heap_host = hostbuf_acquire((size_t)used + 16);
-        tick("pass: host buffer");
-        if (!heap_host.p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
-        res->heaps.push_back(heap_host);
-        res->heap_bytes.push_back(used);
-        if (used && (rc = d2h(heap_host.p, d_heap, used, st))) return rc;
+    PassSummary sum = {};
+    if (c.route == Route::columns) {
+        if ((rc = classify_pass(c, b, sd, pass, listed ? nullptr : d_list, n_pass, heap_bufs, st, ps, &sum, res)))
+            return rc;
+    } else {
+        if (used > heap_cap) used = heap_cap;
+        if (c.route == Route::text) used = 0;      // the records stay on the device
+        else {
+            HostBuf heap_host = hostbuf_acquire((size_t)used + 16);
+            tick("pass: host buffer");
+            if (!heap_host.p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
+            res->heaps.push_back(heap_host);
+            res->heap_bytes.push_back(used);
+            if (used && (rc = d2h(heap_host.p, d_heap, used, st))) return rc;
+        }
+        if ((rc = d2h(ps->hdr_host, sd.hdr, (size_t)n_reads * sizeof(ReadHdr), st)) || (rc = sync(st))) return rc;
+        record(st, 4);
+        if ((rc = sync(st))) return rc;
+        ps->d2h_ms += elapsed_ms(st, 3, 4);
+        res->stats.d2h_bytes += used + (size_t)n_reads * sizeof(ReadHdr);
+        tick("pass: d2h");
+        if (listed) ps->all_reads(n_reads);
+        classify_reads(ClassifyArgs { ps->list.data(), n_pass, ps->hdr_host, offsets, ps->read_heap.data(),
+                                      (uint32_t)pass, &sum, ps->list.data() });
+        tick("pass: classify");
     }
-    if ((rc = d2h(hdr_host, sd.hdr, (size_t)n_reads * sizeof(ReadHdr), st)) || (rc = sync(st))) return rc;
-    record(st, 4);
-    if ((rc = sync(st))) return rc;
-    ps->d2h_ms += elapsed_ms(st, 3, 4);
-    res->stats.d2h_bytes += used + (size_t)n_reads * sizeof(ReadHdr);
-    tick("pass: d2h");
-    // classify this pass; alignments are materialised in read order after the last pass
-    std::vector<uint32_t> retry;
-    const uint32_t heap_id = text ? (uint32_t)pass : (uint32_t)res->heaps.size() - 1;
-    if (ps->list.size() != n_pass) ps->all_reads(n_reads);
-    for (uint32_t r : ps->list) {
-        const ReadHdr &h = hdr_host[r];
-        if (h.status == MGB_READ_OVERFLOW) { MGB_EMU_HIT(EMU_READ_OVERFLOW); retry.push_back(r); continue; }
-        res->stats.num_seeds += h.stats.num_seeds; res->stats.num_extensions += h.stats.num_extensions;
-        res->stats.num_explored_nodes += h.stats.num_explored_nodes; res->stats.dp_cells += h.stats.dp_cells;
-        res->stats.dp_columns += h.stats.dp_columns;
-        res->count[r] = h.n_aln;
-        res->first[r] = h.heap_off;          // byte offset for now, patched by materialise
-        ps->read_heap[r] = heap_id;
-    }
-    res->stats.num_reads_retried += retry.size();
-    ps->list.swap(retry);
-    ps->n_pass = (uint32_t)ps->list.size();
-    tick("pass: classify");
+    mgb_stats_t &s = res->stats;
+    s.num_seeds += sum.num_seeds; s.num_extensions += sum.num_extensions; s.num_explored_nodes += sum.num_explored_nodes;
+    s.dp_cells += sum.dp_cells; s.dp_columns += sum.dp_columns; s.num_reads_retried += sum.n_retry;
+    ps->list.resize(sum.n_retry);
+    ps->n_pass = sum.n_retry;
+    ps->L_retry = sum.max_retry_len;
     return 0;
 }
 
-// record route: mgb_alignment_t records in read order, from the heaps the passes downloaded
-static void materialise(const Call &c, const std::vector<uint32_t> &read_heap, Piece *res) {
+// record route: mgb_alignment_t records in read order (res->first), from the heaps the passes downloaded
+static void materialise(const Call &c, const PassState &ps, Piece *res) {
     const uint32_t n_reads = res->n_reads;
-    std::vector<uint64_t> byte_off(res->first, res->first + n_reads);
-    for (uint32_t r = 0; r < n_reads; ++r) { res->src_off[r] = byte_off[r]; res->src_heap[r] = read_heap[r]; }
-    uint64_t pos = 0;
-    for (uint32_t r = 0; r < n_reads; ++r) { res->first[r] = pos; pos += res->count[r]; }
-    res->n_alns = pos;
+    for (uint32_t r = 0; r < n_reads; ++r) { res->src_off[r] = ps.hdr_host[r].heap_off; res->src_heap[r] = ps.read_heap[r]; }
     #pragma omp parallel for schedule(static) num_threads(host_team()) if (n_reads > 20000)
     for (int64_t r = 0; r < (int64_t)n_reads; ++r)
-        unpack_records(res->heaps[read_heap[r]].p + byte_off[r], res->count[r], c.dcfg.result_nodes != 0,
+        unpack_records(res->heaps[res->src_heap[r]].p + res->src_off[r], res->count[r], c.dcfg.result_nodes != 0,
                        res->lo + (uint32_t)r, res->alns + res->first[r]);
 }
 
+// What every route runs on one piece of res->n_reads reads (seqs and offsets relative to the piece), after the caller
+// has recorded event 0: upload, preparation and seeding, and the align passes until no read overflows its arena. Every
+// pass's heap buffers go into the caller's heap_keep, so the heaps can outlive the call; ps comes prepared for the
+// route's classification (read_heap and hdr_host, or pass_of).
+static int align_piece(const Call &c, const char *seqs, const uint64_t *offsets, CallWorkspace &cw, DevBufs &bufs,
+                       std::deque<DevBufs> &heap_keep, Ticks &tick, Batch *b, Seeded *sd, PassState *ps, Piece *res) {
+    const uint32_t n_reads = res->n_reads;
+    Stream &st = cw.st;
+    std::vector<uint64_t> koff;
+    int rc = upload_batch(c.index, seqs, offsets, n_reads, c.dcfg.forward_and_reverse_complement, st, bufs, b, &koff,
+                          &res->stats, c.dev_input);
+    if (rc) return rc;
+    tick("upload_batch (host part)");
+    // query length k_align stages on chip (0: none; MGB_TEST_LQ: test knob that forces the unstaged path)
+    int lq = b->L_max + 1 <= 512 ? (int)((b->L_max + 1 + 15) & ~15u) : 0;
+    if (const char *e = std::getenv("MGB_TEST_LQ")) lq = std::atoi(e);
+    if ((rc = prepare_and_seed(c, *b, lq, st, bufs, sd, &res->stats))) return rc;
+
+    // align passes: all reads with scale 1, overflowed reads again with larger arenas. Pass 0 after k_prepare_exact
+    // takes its list from the device and needs the host's copy of all n_reads only once it is done: filling it first
+    // would delay the launches behind it.
+    ps->n_pass = n_reads;
+    if (!sd->prep_exact) ps->all_reads(n_reads);
+    for (int pass = 0; ps->n_pass; ++pass) {
+        const uint32_t scale = 1u << (2 * pass);
+        if (pass == kMaxPasses) return fail(MGB_ERR_OVERFLOW, "a read exceeded the largest per-read work arena");
+        // the arena fits the longest read of the pass: on a retry pass the reads that overflowed, not the batch
+        const uint32_t L_pass = pass ? ps->L_retry : b->L_max;
+        DevBufs arena_bufs(st, cw.w, kArenaSlots);
+        DevBufs &heap_bufs = heap_keep.emplace_back(st, cw.w, c.route == Route::records ? kPassHeapSlots
+                                                                                        : kept_heap_slots(pass));
+        PassPlan plan;
+        if ((rc = pass_plan(c, *b, L_pass, scale, lq, ps->n_pass, arena_bufs, &plan))
+            || (rc = run_pass(c, *b, *sd, plan, pass, scale, lq, seqs, offsets, koff, arena_bufs, heap_bufs, st, tick,
+                              ps, res)))
+            return rc;
+    }
+    res->stats.h2d_ms = elapsed_ms(st, 0, 1);
+    res->stats.seed_kernel_ms = elapsed_ms(st, 1, 2);
+    res->stats.align_kernel_ms = ps->align_ms; res->stats.d2h_ms = ps->d2h_ms;
+    return MGB_OK;
+}
+
+// The record and text routes on one piece of a call: the piece's offsets rebased, its headers uploaded (text route),
+// align_piece, then the text rendered on the device or the records materialised on the host.
 static int align_range(const Call &c, uint32_t lo, uint32_t n_reads, Piece *res) {
     const mgb_index_t *index = c.index;
     Ticks tick { std::getenv("MGB_DEBUG") != nullptr, lo, n_reads };
-    std::memset(&res->stats, 0, sizeof(res->stats));
     res->lo = lo; res->n_reads = n_reads;
-    const bool text = c.text_format != 0;
+    const bool text = c.route == Route::text;
     // offsets relative to the first character of the piece
     // (device-resident reads: the piece starts at the 16-byte word that holds its first character, as the kernels'
     // word reads assume)
@@ -2508,70 +2549,38 @@ static int align_range(const Call &c, uint32_t lo, uint32_t n_reads, Piece *res)
     HostBuf hdr_buf = hostbuf_acquire(((size_t)n_reads + 1) * sizeof(ReadHdr));
     if (!hdr_buf.p) return fail(MGB_ERR_CUDA, "host buffer allocation failed");
     struct HdrGuard { HostBuf b; ~HdrGuard() { hostbuf_release(b); } } hdr_guard{ hdr_buf };
+    PassState ps;
+    ps.hdr_host = (ReadHdr*)hdr_buf.p;
+    ps.read_heap.assign(n_reads, 0);
     DevBufs bufs(st, cw.w, kBatchSlots), text_bufs(st, cw.w, kTextSlots);
-    Batch b; std::vector<uint64_t> koff;
+    std::deque<DevBufs> heap_keep;       // the text route keeps every pass's heap until the text is rendered
     record(st, 0);
     tick("setup");
-    if ((rc = upload_batch(index, seqs, offsets, n_reads, c.dcfg.forward_and_reverse_complement, st, bufs, &b, &koff,
-                           &res->stats, c.dev_input)))
-        return rc;
     TextArgs ta;
     std::memset(&ta, 0, sizeof(ta));
-    if (text && (rc = upload_headers(c, b, names, name_offs, st, text_bufs, &ta, &res->stats))) return rc;
-    tick("upload_batch (host part)");
-    // query length k_align stages on chip (0: none; MGB_TEST_LQ: test knob that forces the unstaged path)
-    int lq = b.L_max + 1 <= 512 ? (int)((b.L_max + 1 + 15) & ~15u) : 0;
-    if (const char *e = std::getenv("MGB_TEST_LQ")) lq = std::atoi(e);
-    Seeded sd;
-    if ((rc = prepare_and_seed(c, b, lq, st, bufs, &sd, &res->stats))) return rc;
-
-    // align passes: all reads with scale 1, overflowed reads again with larger arenas. Pass 0 after k_prepare_exact
-    // takes its list from the device and needs the host's copy of all n_reads only once it is done: filling it first
-    // would delay the launches behind it.
-    PassState ps;
-    ps.read_heap.assign(n_reads, 0);
-    ps.n_pass = n_reads;
-    if (!sd.prep_exact) ps.all_reads(n_reads);
-    std::deque<DevBufs> heap_keep;       // the text route keeps every pass's heap until the text is rendered
-    for (int pass = 0; ps.n_pass; ++pass) {
-        const uint32_t scale = 1u << (2 * pass);
-        if (pass == kMaxPasses) return fail(MGB_ERR_OVERFLOW, "a read exceeded the largest per-read work arena");
-        // the arena fits the longest read of the pass: on a retry pass the reads that overflowed, not the batch
-        uint32_t L_pass = b.L_max;
-        if (pass > 0) {
-            L_pass = 0;
-            for (uint32_t r : ps.list) L_pass = std::max<uint32_t>(L_pass, (uint32_t)(offsets[r + 1] - offsets[r]));
-        }
-        DevBufs arena_bufs(st, cw.w, kArenaSlots);
-        DevBufs &heap_bufs = heap_keep.emplace_back(st, cw.w, text ? text_heap_slots(pass) : kPassHeapSlots);
-        PassPlan plan;
-        if ((rc = pass_plan(c, b, L_pass, scale, lq, ps.n_pass, arena_bufs, &plan))
-            || (rc = run_pass(c, b, sd, plan, pass, scale, lq, seqs, offsets, koff, arena_bufs, heap_bufs,
-                              (ReadHdr*)hdr_buf.p, st, tick, &ps, &ta, res)))
-            return rc;
-    }
+    if (text && (rc = upload_headers(c, n_reads, names, name_offs, st, text_bufs, &ta, &res->stats))) return rc;
+    Batch b; Seeded sd;
+    if ((rc = align_piece(c, seqs, offsets, cw, bufs, heap_keep, tick, &b, &sd, &ps, res))) return rc;
+    // each read's records in read order: the last pass's headers hold the count of every read, from the pass that
+    // answered it
+    uint64_t pos = 0;
+    for (uint32_t r = 0; r < n_reads; ++r) { res->count[r] = ps.hdr_host[r].n_aln; res->first[r] = pos; pos += res->count[r]; }
+    res->n_alns = pos;
     if (text && n_reads) {      // every read's pass goes up (its heap offset is in sd.hdr already), then the text comes down
         uint8_t *d_pass = nullptr;
-        const std::vector<uint8_t> pass_of(ps.read_heap.begin(), ps.read_heap.end());
         rc = text_bufs.alloc(&d_pass, n_reads);
-        if (!rc) rc = h2d(d_pass, pass_of.data(), n_reads, st);
+        if (!rc) rc = h2d(d_pass, ps.read_heap.data(), n_reads, st);
         res->stats.h2d_bytes += n_reads;
-        ta.hdr = sd.hdr; ta.pass = d_pass;
+        ta.seqs = b.seqs; ta.offsets = b.offsets; ta.hdr = sd.hdr; ta.pass = d_pass;
+        std::copy(ps.heap, ps.heap + kMaxPasses, ta.heap);
         if (rc || (rc = render_text(index, ta, text_bufs, st, &res->text, &res->text_bytes, &res->stats))) return rc;
         tick("text");
     }
-    res->stats.h2d_ms = elapsed_ms(st, 0, 1);
-    res->stats.seed_kernel_ms = elapsed_ms(st, 1, 2);
-    res->stats.align_kernel_ms = ps.align_ms; res->stats.d2h_ms = ps.d2h_ms;
     tick("free device buffers");
-    if (text) {                                   // counts only: the text route has no records on the host
-        uint64_t pos = 0;
-        for (uint32_t r = 0; r < n_reads; ++r) { res->first[r] = pos; pos += res->count[r]; }
-        res->n_alns = pos;
-        return MGB_OK;
+    if (!text) {
+        materialise(c, ps, res);
+        tick("materialise");
     }
-    materialise(c, ps.read_heap, res);
-    tick("materialise");
     return MGB_OK;
 }
 
@@ -2603,19 +2612,24 @@ int mgb_config_check(const mgb_index_t *index, const mgb_config_t *config) {
 
 } // extern "C"
 
+// the configuration of an align call on the device: lower_config, then the graph mode's override
+static int call_config(const mgb_index_t *index, const mgb_config_t &config, DevConfig *dcfg) {
+    std::string err;
+    if (const int rc = lower_config(config, index->view.k, index->alphabet, dcfg, &err)) return fail(rc, err);
+    if (index->view.mode != 0) {                  // CANONICAL-mode graph, or a PRIMARY one with CanonicalDBG semantics
+        dcfg->canonical = 1;                      // (get_mode() == CANONICAL): both strands, no RCDBG view
+        dcfg->forward_and_reverse_complement = 1; // (dbg_aligner.cpp:224-226)
+    }
+    return MGB_OK;
+}
+
 // mgb_align_batch (text_format 0) and mgb_align_batch_text (MGB_TEXT_TSV / MGB_TEXT_JSON, with the headers)
 // dev_input: seqs and names are device memory (the file route's parsed chunk), the offsets host memory
 static int align_batch(const mgb_index_t *index, const mgb_config_t *config, const char *seqs, const uint64_t *offsets,
                        const char *names, const uint64_t *name_offsets, uint32_t n_reads, int text_format,
                        mgb_results_t **out, bool dev_input = false) {
     DevConfig dcfg;
-    std::string err;
-    int rc = lower_config(*config, index->view.k, index->alphabet, &dcfg, &err);
-    if (rc) return fail(rc, err);
-    if (index->view.mode != 0) {                 // CANONICAL-mode graph, or a PRIMARY one with CanonicalDBG semantics
-        dcfg.canonical = 1;                      // (get_mode() == CANONICAL): both strands, no RCDBG view
-        dcfg.forward_and_reverse_complement = 1; // (dbg_aligner.cpp:224-226)
-    }
+    if (const int rc = call_config(index, *config, &dcfg)) return rc;
     // the text route: TSV lines print no node ids, so its records carry none; JSON records need them on the device
     if (text_format) dcfg.result_nodes = text_format == MGB_TEXT_TSV ? MGB_NODES_NONE : MGB_NODES_U64;
 
@@ -2664,7 +2678,8 @@ static int align_batch(const mgb_index_t *index, const mgb_config_t *config, con
             pieces[i].src_heap = res->src_heap.data() + piece_lo(i);
         }
     }
-    const Call call { index, dcfg, seqs, offsets, names, name_offsets, text_format, config->min_path_score, dev_input };
+    const Call call { index, dcfg, text_format ? Route::text : Route::records, seqs, offsets, names, name_offsets,
+                      text_format, config->min_path_score, dev_input };
     std::atomic<uint32_t> next{0};
     std::atomic<bool> failed{false};
     auto lane = [&]() {
@@ -2774,9 +2789,9 @@ static int fastx_parse(const mgb_index_t *index, const char *buf, uint64_t bytes
 } // extern "C"
 
 // ---------------------------------------------------------------------------------------
-// device-resident batches (mgb_align_batch_device): align_range's stages on reads already in device memory, one piece
-// on one stream; the passes are classified on the device and the records stay in the pass heaps until the caller's
-// columns are written (columns_core.cuh)
+// device-resident batches (mgb_align_batch_device), the columns route: align_piece on reads already in device memory,
+// one piece on one stream; the records stay in the pass heaps, which the handle holds, until the caller's columns are
+// written (columns_core.cuh)
 // ---------------------------------------------------------------------------------------
 struct mgb_device_results {
     explicit mgb_device_results(const mgb_index_t *ix) : cw(ix) {}
@@ -2808,13 +2823,11 @@ static bool on_device(const void *p, int device) {
 static int align_device(const mgb_index_t *index, const mgb_config_t *config, const char *d_seqs, const uint64_t *offsets,
                         bool offsets_on_device, uint32_t n_reads, void *stream, mgb_device_results *res) {
     DevConfig dcfg;
-    std::string err;
-    int rc = lower_config(*config, index->view.k, index->alphabet, &dcfg, &err);
-    if (rc) return fail(rc, err);
-    if (index->view.mode != 0) { dcfg.canonical = 1; dcfg.forward_and_reverse_complement = 1; }   // as align_batch
+    int rc = call_config(index, *config, &dcfg);
+    if (rc) return rc;
     Piece piece;
+    piece.n_reads = n_reads;
     mgb_stats_t &stats = piece.stats;
-    std::memset(&stats, 0, sizeof(stats));
     CallWorkspace &cw = res->cw;
     if ((rc = cw.ready())) return rc;
     Stream &st = cw.st;
@@ -2856,43 +2869,19 @@ static int align_device(const mgb_index_t *index, const mgb_config_t *config, co
 #else
     if (chars) CUDA_TRY(cudaMemcpyAsync(seqs, d_seqs + base, chars, cudaMemcpyDeviceToDevice, st.s));
 #endif
-    Batch b; std::vector<uint64_t> koff;
-    if ((rc = upload_batch(index, seqs, offs.data(), n_reads, dcfg.forward_and_reverse_complement, st, bufs, &b, &koff,
-                           &stats, true)))
-        return rc;
-    const Call c { index, dcfg, seqs, offs.data(), nullptr, nullptr, 0, config->min_path_score, true, true };
-    int lq = b.L_max + 1 <= 512 ? (int)((b.L_max + 1 + 15) & ~15u) : 0;      // as align_range
-    if (const char *e = std::getenv("MGB_TEST_LQ")) lq = std::atoi(e);
-    Seeded sd;
-    if ((rc = prepare_and_seed(c, b, lq, st, bufs, &sd, &stats))) return rc;
-
     DevBufs &cb = res->bufs.emplace_back(st, cw.w, kTextSlots);
     PassState ps;
     if ((rc = cb.alloc(&ps.pass_of, (size_t)n_reads + 1))) return rc;
-    ps.n_pass = n_reads;
-    if (!sd.prep_exact) ps.all_reads(n_reads);
-    TextArgs ta;                     // (run_pass leaves every pass's heap in ta.heap)
-    std::memset(&ta, 0, sizeof(ta));
+    const Call c { index, dcfg, Route::columns, seqs, offs.data(), nullptr, nullptr, 0, config->min_path_score, true };
     Ticks tick { std::getenv("MGB_DEBUG") != nullptr, 0, n_reads };
-    for (int pass = 0; ps.n_pass; ++pass) {
-        const uint32_t scale = 1u << (2 * pass);
-        if (pass == kMaxPasses) return fail(MGB_ERR_OVERFLOW, "a read exceeded the largest per-read work arena");
-        const uint32_t L_pass = pass ? ps.L_retry : b.L_max;
-        if (pass > 0 || !sd.prep_exact) stats.h2d_bytes += (uint64_t)ps.n_pass * 4;     // run_pass uploads the list
-        DevBufs arena_bufs(st, cw.w, kArenaSlots);
-        DevBufs &heap_bufs = res->bufs.emplace_back(st, cw.w, text_heap_slots(pass));
-        PassPlan plan;
-        if ((rc = pass_plan(c, b, L_pass, scale, lq, ps.n_pass, arena_bufs, &plan))
-            || (rc = run_pass(c, b, sd, plan, pass, scale, lq, seqs, offs.data(), koff, arena_bufs, heap_bufs, nullptr,
-                              st, tick, &ps, &ta, &piece)))
-            return rc;
-    }
+    Batch b; Seeded sd;
+    if ((rc = align_piece(c, seqs, offs.data(), cw, bufs, res->bufs, tick, &b, &sd, &ps, &piece))) return rc;
 
     // every read's alignments, sequence bytes, CIGAR ops and node ids; their scans; the totals come down
     ColumnsArgs &ca = res->ca;
     std::memset(&ca, 0, sizeof(ca));
     ca.hdr = sd.hdr; ca.pass_of = ps.pass_of;
-    for (int p = 0; p < kMaxPasses; ++p) ca.heap[p] = ta.heap[p];
+    std::copy(ps.heap, ps.heap + kMaxPasses, ca.heap);
     ca.n_reads = n_reads; ca.no_nodes = dcfg.result_nodes != 0;
     for (uint64_t *&x : ca.cnt) if ((rc = cb.alloc(&x, (size_t)n_reads + 1))) return rc;
 #if defined(MGB_HOST_EMU)
@@ -2911,9 +2900,6 @@ static int align_device(const mgb_index_t *index, const mgb_config_t *config, co
     if ((rc = sync(st))) return rc;
     stats.d2h_bytes += sizeof(tot);
     stats.kernel_launches += (n_reads ? 1 : 0) + 4 * (n_reads ? 3 : 2);
-    stats.h2d_ms = elapsed_ms(st, 0, 1);
-    stats.seed_kernel_ms = elapsed_ms(st, 1, 2);
-    stats.align_kernel_ms = ps.align_ms; stats.d2h_ms = ps.d2h_ms;
     res->sizes = mgb_device_sizes_t { n_reads, tot[0], tot[1], tot[2], tot[3] };
     res->stats = stats;
     return MGB_OK;

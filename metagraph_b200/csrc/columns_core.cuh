@@ -3,7 +3,7 @@
 //   k_pass_classify  after an align pass, over the pass's reads: a finished read's pass id goes into pass_of, a read
 //                    that overflowed its arena is appended to the retry list (warp-aggregated), and the search
 //                    counters of the finished reads are summed into a PassSummary, the only thing the host reads back
-//                    when no read overflowed.
+//                    when no read overflowed. The record and text routes run the same classify_read on the host.
 //   k_columns_size   after the last pass, one warp per read: the read's alignments, sequence bytes, CIGAR ops and node
 //                    ids, walking its records in the heap of the pass that answered it.
 //   k_columns_write  after the four scans of those counts, one warp per read: the records as the caller's columns
@@ -20,8 +20,8 @@ namespace mgb {
 
 constexpr int kColumnsMaxPasses = 8;    // heaps a batch can be answered from (api.cu kMaxPasses)
 
-// what the host reads back after a pass: the counters run_pass sums over the finished reads, how many reads overflowed
-// and the longest of them (it sizes the next pass's arena)
+// a pass's classification: the counters of the finished reads, how many reads overflowed and the longest of them (it
+// sizes the next pass's arena); on the device route the host reads back only this after a pass with no overflow
 struct PassSummary {
     unsigned long long num_seeds, num_extensions, num_explored_nodes, dp_cells, dp_columns;
     unsigned int n_retry, max_retry_len;
@@ -36,7 +36,7 @@ struct ClassifyArgs {
 };
 
 // read r of the pass: true when it overflowed (the caller appends it); otherwise its pass and counters are recorded
-MGB_HD bool classify_read(const ClassifyArgs &a, uint32_t r, PassSummary &acc) {
+MGB_HOSTDEV bool classify_read(const ClassifyArgs &a, uint32_t r, PassSummary &acc) {
     const ReadHdr h = a.hdr[r];
     if (h.status == MGB_READ_OVERFLOW) {
         const uint32_t L = (uint32_t)(a.offsets[r + 1] - a.offsets[r]);
@@ -48,21 +48,6 @@ MGB_HD bool classify_read(const ClassifyArgs &a, uint32_t r, PassSummary &acc) {
     acc.num_explored_nodes += h.stats.num_explored_nodes; acc.dp_cells += h.stats.dp_cells;
     acc.dp_columns += h.stats.dp_columns;
     return false;
-}
-
-// One alignment of a read's packed records (OutAln | node ids unless result_nodes | CIGAR | sequence, as k_align and
-// the whole-read writers pack them)
-struct RecView {
-    OutAln o; const uint64_t *nodes; const uint32_t *cigar; const char *seq;
-};
-MGB_HD const char *rec_next(const char *p, bool no_nodes, RecView *v) {
-    v->o = *reinterpret_cast<const OutAln*>(p);
-    p += sizeof(OutAln);
-    v->nodes = no_nodes ? nullptr : reinterpret_cast<const uint64_t*>(p);
-    if (!no_nodes) p += 8ull * v->o.n_nodes;
-    v->cigar = reinterpret_cast<const uint32_t*>(p); p += (4ull * v->o.n_cigar + 7) & ~7ull;
-    v->seq = p; p += ((uint64_t)v->o.seq_len + 7) & ~7ull;
-    return p;
 }
 
 struct ColumnsArgs {
